@@ -1,20 +1,24 @@
 #!/usr/bin/env python
-"""bench.py -- column-iterations/s of the GLOM column update on N B200s (BASELINE.json metric).
+"""bench.py -- column-iterations/s of the GLOM column update on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
-A "step" is one pass of the hot path over one batch: ``Glom.forward(img, iters=12)`` at BASELINE
-configs[1] per GPU (dim=512 L=6 224/14, batch 32, bf16 tensor-core precision), i.e. 12 Jacobi column
-updates of 32x256 columns x 6 levels = 589,824 column-iterations per GPU per step.  N > 1 shards the
-batch (configs[2]: 32 images per GPU, no data-path collective) => weak scaling.
+A "step" is one pass of the hot path over one batch: ``Glom.forward(img, iters=12)`` at configs[1]
+per GPU, i.e. 12 Jacobi column updates of 32x256 columns x 6 levels = 589,824 column-iterations per GPU per
+step.  N > 1 shards the batch (configs[2]) => weak scaling.  The workloads:
+  configs[0]  dim=64   L=3 28/7    iters=2  batch 1    (smoke size)
+  configs[1]  dim=512  L=6 224/14  iters=12 batch 32   (the timed line, bf16 tensor-core precision)
+  configs[2]  configs[1] with 32 images per GPU on N GPUs
+  configs[3]  dim=1024 L=8 384/16  iters=16 batch 8 per GPU
+  configs[4]  configs[1] shapes, three frames of iters 12 -> 10 -> 6 with the state carried
 
 Regime (what the numbers mean): after the W warm-up steps the same forward runs back to back for
-``--preheat-s`` seconds (default 2 s) so that the timed K steps see the SUSTAINED state of the part (1 kW power
-cap, SM clock ~1.4-1.5 GHz), not a sub-second burst at 1.965 GHz.  The SM clock is measured on the device itself
-(``glom_b200_clock_probe``: cycles per %globaltimer nanosecond) immediately before and after the timed region and
-printed next to NVML's (lagging) reading; ``roofline.peak`` is the measured sustained cuBLAS rate when that clock is
-in the sustained band and the burst rate otherwise, and both fractions are printed.
+``--preheat-s`` seconds (default 2 s) so that the timed K steps see the sustained clock of the part rather than a
+sub-second burst.  The SM clock is measured on the device itself (``glom_b200_clock_probe``: cycles per %globaltimer
+nanosecond) immediately before and after the timed region and printed next to NVML's (lagging) reading;
+``roofline.peak`` comes from MEASURED_PEAKS.json when present, else from the H100 SXM data sheet, and is labelled
+with its source.
 
 Printed (rank 0, ONE JSON line):
   value      whole-job column-iterations/s with the images already resident in HBM, device-timed
@@ -23,11 +27,11 @@ Printed (rank 0, ONE JSON line):
              forward, D2H of the returned state into pinned host memory, all inside the timed region
   roofline   dominant kernel: algorithmic FLOPs per launch / its average duration from CUDA events recorded
              around every launch in the timed region
-  other_configs  BASELINE configs[3] (per-GPU shape) and configs[4] (3-frame continuation), and a training step
+  other_configs  configs[3] (per-GPU shape) and configs[4] (3-frame continuation), and a training step
   cpu_baseline   the reference's own CPU forward on this box's host cores (bounded sample; rank 0, N = 1 only)
 
-``--impl reference`` times the UNMODIFIED reference package (``$GLOM_REF_PATH`` -> ``baseline/_ref`` ->
-``/root/reference``; torch CPU, all host threads) on the same shapes; if it is not importable on the box it times
+``--impl reference`` times the UNMODIFIED reference package (``$GLOM_REF_PATH``, then ``baseline/_ref``; torch CPU,
+all host threads) on the same shapes; if it is not importable it times
 ``oracle/glom_oracle_torch.py`` (a torch-CPU restatement pinned on the reference's golden outputs) and says so.
 """
 import argparse
@@ -42,17 +46,18 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 CFG = dict(dim=512, levels=6, image_size=224, patch_size=14)
-CFG3 = dict(dim=1024, levels=8, image_size=384, patch_size=16)      # BASELINE configs[3], 8 images per GPU, 16 iters
+CFG3 = dict(dim=1024, levels=8, image_size=384, patch_size=16)      # configs[3], 8 images per GPU, 16 iters
 ITERS = 12
 BATCH_PER_GPU = 32
 N_PATCH = (CFG["image_size"] // CFG["patch_size"]) ** 2
 METRIC = "column-iterations/sec (BxNxLxiters) at dim=512 L=6 224/14"
 UNIT = "column-iterations/s"
-NOMINAL_FLOP_PER_CLK = 148 * 8192.0        # dense bf16: 4096 MAC/clk/SM x 148 SMs (2.25 PFLOP/s at ~1.86 GHz)
+NOMINAL_FLOP_PER_CLK = 132 * 4096.0        # dense bf16: 2048 MAC/clk/SM x 132 SMs (989 TFLOP/s at 1.83 GHz, H100 SXM)
+DUMP_BYTES = 48 << 20                      # --dump-outputs: at most this many bytes of the final state
 
 
 def flops_per_col_iter(d, L, n, iters=None):
-    """Tensor FLOPs per column-iteration: 16 d^2 (2L-1)/L + 4 n d   (SURVEY 8d).  With `iters`: the FLOPs the engine
+    """Tensor FLOPs per column-iteration: 16 d^2 (2L-1)/L + 4 n d  .  With `iters`: the FLOPs the engine
     EXECUTES per column-iteration of a call of that many steps -- the first GEMM of MLP group 0 (bottom-up net of level 0,
     whose input, the tokens, does not change during a call) runs in the call's first step only: 8 d^2 / L per
     column-iteration less in the later steps.  Rooflines use the executed figure, never the larger algorithmic one."""
@@ -63,7 +68,7 @@ def flops_per_col_iter(d, L, n, iters=None):
 
 
 def bytes_per_iter(d, L, n, B, s_state=2, s_w=2):
-    """Algorithmic HBM bytes per iteration (SURVEY 8d)."""
+    """Algorithmic HBM bytes per iteration."""
     return 2 * B * n * L * d * s_state + (2 * L - 1) * (8 * d * d + 5 * d) * s_w + B * n * d * 2 + n * d * 2
 
 
@@ -76,8 +81,8 @@ def measured_peaks():
                     burst=j["bf16_tflops"], sm_max_mhz=j.get("sm_max_mhz", 1965.0),
                     sustained_mhz=(j.get("clocks_under_load") or {}).get("sm_mhz_median"),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, sustained=1400.0, burst=1590.0, sm_max_mhz=1965.0, sustained_mhz=1300.0,
-                source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, sustained=989.0, burst=989.0, sm_max_mhz=1980.0, sustained_mhz=None,
+                source="H100 SXM data sheet (not measured)")
 
 
 # ------------------------------------------------------------------------------------ CPU arm
@@ -207,7 +212,7 @@ def run_reference_arm(args, rank, world):
         "impl": "reference", "metric": METRIC, "value": v, "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": sec * 1e3, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-        "config": {"workload": f"BASELINE configs[1] shapes: dim=512 L=6 224/14 iters={ITERS}; CPU sample batch={batch} "
+        "config": {"workload": f"configs[1] shapes: dim=512 L=6 224/14 iters={ITERS}; CPU sample batch={batch} "
                                f"of 32 per step (the metric is per column-iteration)",
                    "batch": batch, "iters": ITERS},
         "cpu_baseline": {"value": v, "unit": UNIT, "cores": arm.threads, "kind": arm.kind, "cpu": cpu_model_name(),
@@ -382,7 +387,11 @@ def main():
     ap.add_argument("--no-other-configs", action="store_true", help="skip configs[3] / configs[4] / training extras")
     ap.add_argument("--no-train", action="store_true")
     ap.add_argument("--train", action="store_true", help="(kept for compatibility: the training step is timed by default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the final state of the last timed step (first images of the batch, float32) as DIR/levels.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -480,7 +489,7 @@ def main():
         _native.kernel_clocks(reset=True)        # in-kernel (clock64, %globaltimer) samples of the timed region only
         ev0.record(stream)
         for i in range(args.steps):
-            model(dev_imgs[i % NBUF], iters=T)
+            last_out = model(dev_imgs[i % NBUF], iters=T)
             launches += model.last_launches
         ev1.record(stream)
         enqueue_clock_probe(1)
@@ -574,7 +583,7 @@ def main():
                 break
         ms_e2e = min(e2e_attempts)
 
-    # -------- the other BASELINE configs on this GPU (same sustained state; short: the box is already hot)
+    # -------- the other configs on this GPU (same sustained state; short: the GPU is already hot)
     other = {}
     peaks = measured_peaks()
     if not args.no_other_configs and args.precision == "bf16":
@@ -700,15 +709,9 @@ def main():
                     kern[k]["tflops"] = flops[k] / (ms / cnt * 1e-3) / 1e12
         cand = [k for k in ("mlp_fused", "gemm1_gelu", "gemm2_combine") if k in kern]
         dom = max(cand, key=lambda k: kern[k]["ms_per_step"]) if cand else "gemm1_gelu"
-        names = {"mlp_fused": "mlp_kernel (persistent grouped GEMM1+GELU -> GEMM2+combine tiles, tcgen05, H kept in L2)",
-                 "gemm1_gelu": "gemm_kernel<0,256> (grouped GEMM1 + bias + exact-erf GELU, tcgen05)",
-                 "gemm2_combine": "gemm_kernel<1,256> (grouped GEMM2 + 4-way combine, tcgen05)"}
-        traffic = None
-        try:   # per-launch DRAM bytes of the dominant kernel from the committed ncu --set full capture
-            with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-                traffic = json.load(f)["kernels"][dom]["dram_bytes"] if args.batch_per_gpu == BATCH_PER_GPU else None
-        except (OSError, KeyError, ValueError):
-            traffic = None
+        names = {"mlp_fused": "mlp_kernel (persistent grouped GEMM1+GELU -> GEMM2+combine tiles, wgmma, H kept in L2)",
+                 "gemm1_gelu": "gemm_kernel<0,256> (grouped GEMM1 + bias + exact-erf GELU, wgmma)",
+                 "gemm2_combine": "gemm_kernel<1,256> (grouped GEMM2 + 4-way combine, wgmma)"}
         # regime: the device-side clock decides which measured peak is the denominator
         mhz = [m for m in dev_mhz_min[:2] if m]
         clk = sum(mhz) / len(mhz) if mhz else None
@@ -727,7 +730,6 @@ def main():
                                f"-> peak = bf16_tflops{'_sustained' if regime != 'burst' else ''}" if clk else "no device clock",
                 "peaks": {"sustained": peaks["sustained"], "burst": peaks["burst"], "hbm_gbs": peaks["hbm_gbs"],
                           "sustained_measured_at_mhz": peaks["sustained_mhz"], "source": peaks["source"]},
-                "traffic": traffic, "traffic_source": "profiles/traffic.json (ncu --set full, dram__bytes_read+write)",
                 "algorithmic_bytes": algo_bytes.get(dom),
                 "flops_per_launch": flops.get(dom),
                 "whole_step": {"tflops": whole_tf,
@@ -740,18 +742,6 @@ def main():
                        "region, same sustained state; `value` / `ms_per_step` come from the un-instrumented pass",
                 "kernels": kern}
         roof["whole_step"]["frac_hbm"] = roof["whole_step"]["hbm_gbs_algorithmic"] / peaks["hbm_gbs"]
-        if traffic and kern.get(dom):
-            # the dominant kernel's HBM side: its arithmetic intensity sits at the ridge of the measured peaks, and the
-            # in-kernel counters show it waiting for operands, so both rooflines are printed
-            gbs = traffic / (kern[dom]["avg_us"] * 1e-6) / 1e9
-            roof["hbm"] = {"achieved_gbs": gbs, "peak_gbs": peaks["hbm_gbs"], "frac": gbs / peaks["hbm_gbs"],
-                           "dram_bytes_per_launch": traffic,
-                           "flop_per_dram_byte": (flops.get(dom) or 0) / traffic,
-                           "ridge_flop_per_byte": peak * 1e12 / (peaks["hbm_gbs"] * 1e9),
-                           "read_write_ceiling_gbs": 3200.0,
-                           "read_write_ceiling_source": "profiles/r2_dram_pattern_probe.txt: a kernel that only reads and "
-                                                        "writes a tensor with the GEMM2 epilogue's access pattern, one "
-                                                        "512-thread CTA per SM (copy bandwidth: MEASURED_PEAKS.json)"}
         if clocks is not None:
             # the SM clock INSIDE the tensor-core kernels of the un-instrumented timed region (rank 0): cycles and
             # %globaltimer ns bracketing each kernel's working phase, summed per kernel kind
@@ -774,7 +764,7 @@ def main():
             "scaling": "weak", "vs_baseline": None, "dtype": "bf16" if args.precision == "bf16" else "f32",
             "data": "synthetic",
             "images_per_s": global_batch * args.steps / (ms_dev * 1e-3),
-            "config": {"workload": f"BASELINE configs[{1 if world == 1 else 2}]: dim=512 L=6 224/14 iters={T} "
+            "config": {"workload": f"configs[{1 if world == 1 else 2}]: dim=512 L=6 224/14 iters={T} "
                                    f"batch={B}/GPU (global {global_batch}), Glom.forward incl. tokeniser",
                        "global_batch": global_batch, "iters": T, "parallelism": f"dp{world} (batch shards, no collective)",
                        "regime": f"{args.preheat_s:g} s of back-to-back forwards before the timed region (sustained power state)",
@@ -809,6 +799,13 @@ def main():
                 line["cpu_baseline"] = {"value": None, "unit": UNIT, "cores": 0, "kind": "unavailable",
                                         "sample": f"CPU arm failed: {type(ex).__name__}: {ex}"}
         print(json.dumps(line), flush=True)
+        if args.dump_outputs:
+            # inputs are seeded, so two builds run with the same arguments can be compared output for output; the dump is
+            # the leading images of the batch, as many as fit DUMP_BYTES
+            import numpy as np
+            keep = max(1, min(B, DUMP_BYTES // (last_out[0].numel() * 4)))
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "levels.npy"), last_out[:keep].float().cpu().numpy())
     if distributed:
         dist.barrier(device_ids=[local_rank])
         dist.destroy_process_group()

@@ -1,4 +1,4 @@
-"""B200-native GLOM column-update engine behind the glom-pytorch `Glom` API."""
+"""H100-native (sm_90a) GLOM column-update engine behind the glom-pytorch `Glom` API."""
 from ._native import GlomB200Error, LIB_PATH
 from .glom import Glom
 from .islands import Islands, islands

@@ -54,7 +54,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise GlomB200Error(
             f"{LIB_PATH} not found: build it with `python -m glom_pytorch_b200.build` "
-            "(nvcc, sm_100a). There is no CPU or PyTorch fallback for the GLOM column update.")
+            "(nvcc, sm_90a). There is no CPU or PyTorch fallback for the GLOM column update.")
     lib = ctypes.CDLL(LIB_PATH)
     vp, sz, i32 = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
     lib.glom_b200_abi_version.restype = i32
@@ -215,15 +215,15 @@ def clock_probe(out_ptr, spin_us, stream):
 
 
 def kernel_clocks(reset=True):
-    """{kind: (SM MHz inside the kernels, in-kernel ms, [wait fractions of block 0: MMA lane on operands, MMA lane on a free
-    accumulator, TMA lane on a free slot, epilogue warp 0 on an accumulator, epilogue warp 0 busy])} since the last reset."""
+    """{kind: (SM MHz inside the kernels, in-kernel ms, [6 cycle fractions of block 0, see glom_b200_kernel_clocks in
+    include/glom_b200.h])} since the last reset."""
     k = len(PROFILE_KINDS)
     mhz, ms, wf = (ctypes.c_double * k)(), (ctypes.c_double * k)(), (ctypes.c_double * (6 * k))()
     check(load().glom_b200_kernel_clocks(mhz, ms, wf, k, int(bool(reset))))
     return {PROFILE_KINDS[i]: (mhz[i], ms[i], [round(wf[6 * i + j], 4) for j in range(6)]) for i in range(k) if ms[i] > 0}
 
 
-def mlp_schedule(cfg, batch, num_sms=148):
+def mlp_schedule(cfg, batch, num_sms=132):
     """Work list of the merged MLP kernel: (list of (kind, z, m_blk, n_blk), delay).  Host only."""
     n, dl = ctypes.c_int(), ctypes.c_int()
     check(load().glom_b200_mlp_schedule(ctypes.byref(cfg), batch, num_sms, None, 0, ctypes.byref(n), ctypes.byref(dl)))

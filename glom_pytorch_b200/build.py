@@ -1,4 +1,4 @@
-"""Build libglom_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libglom_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m glom_pytorch_b200.build          # or __graft_entry__.build()
 """
@@ -12,7 +12,7 @@ LIB = os.path.join(PKG, "libglom_b200.so")
 SOURCES = ["glom_api.cu", "simt_kernels.cu", "tc_kernels.cu", "mlp_kernel.cu", "islands.cu", "bwd_kernels.cu", "tc_bwd_kernels.cu"]
 HEADERS = ["engine.h", "ptx.cuh", "tc_common.cuh", os.path.join("..", "..", "include", "glom_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-cudart", "static",
 ]
 
@@ -51,7 +51,7 @@ def build_library(force=False, verbose=False):
             sys.stderr.write(out)
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {s}")
-    link = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "static",
+    link = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-cudart", "static",
             "-Xcompiler", "-fPIC", *objs, "-o", LIB]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode:

@@ -1,4 +1,4 @@
-// Backward of the GLOM column update -- SURVEY 8 row f2: the reverse loop, the fp32 CUDA-core kernels, and the dispatch to
+// Backward of the GLOM column update -- the reverse loop, the fp32 CUDA-core kernels, and the dispatch to
 // the tensor-core GEMMs of tc_bwd_kernels.cu for the bf16 engine.
 //
 // Differentiates glom_pytorch/glom_pytorch.py:131-145 step by step in reverse, recomputing the per-step
@@ -7,7 +7,7 @@
 //   S_{t+1} = (S_t + BU(S_t, X) + TD(S_t + P) + C(S_t)) / c          (:141-142)
 // All contractions go through one strided, batched fp32 GEMM (NN / NT / TN are just stride choices), the rest
 // are small element-wise / row-reduction kernels.  With precision fp32 (or dim % 256 != 0) this file is the whole
-// backward; with precision bf16 `backward_run` sends the MLP and consensus GEMMs to tcgen05 (`mlp_backward_tc`,
+// backward; with precision bf16 `backward_run` sends the MLP and consensus GEMMs to the tensor cores (`mlp_backward_tc`,
 // `attn_bwd_gemm_tc`) and keeps the softmax / normalisation / bias reductions here.
 #include "engine.h"
 #include "ptx.cuh"
@@ -317,7 +317,7 @@ cudaError_t tokenize_backward(const float* img, const float* weight, const float
   if (d_weight) {
     const size_t total = (size_t)rows * k3;
     const size_t want = (total + 255) / 256;
-    patchify_f32_kernel<<<(int)(want < 148 * 32 ? want : 148 * 32), 256, 0, st>>>(img, patches, B, H, W, p);
+    patchify_f32_kernel<<<(int)(want < sm_count() * 32 ? want : sm_count() * 32), 256, 0, st>>>(img, patches, B, H, W, p);
     if (launches) ++*launches;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // d_weight (d, k3) += dTok^T (d x rows) . patches (rows x k3)
@@ -346,7 +346,7 @@ cudaError_t tokenize_backward(const float* img, const float* weight, const float
     if ((e = gemm_f32(q, 1, st, launches)) != cudaSuccess) return e;
     const size_t total = (size_t)B * 3 * H * W;
     const size_t want = (total + 255) / 256;
-    unpatchify_add_kernel<<<(int)(want < 148 * 32 ? want : 148 * 32), 256, 0, st>>>(dpatches, d_img, B, H, W, p);
+    unpatchify_add_kernel<<<(int)(want < sm_count() * 32 ? want : sm_count() * 32), 256, 0, st>>>(dpatches, d_img, B, H, W, p);
     if (launches) ++*launches;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
   }
@@ -362,7 +362,7 @@ __global__ void cast_bf16_rows(size_t n4, const float* __restrict__ src, __nv_bf
 
 static inline int nblk(size_t total, int block = 256) {
   const size_t want = (total + block - 1) / block;
-  return (int)(want < (size_t)148 * 32 ? (want ? want : 1) : (size_t)148 * 32);
+  return (int)(want < (size_t)sm_count() * 32 ? (want ? want : 1) : (size_t)sm_count() * 32);
 }
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return e_; } while (0)
 #define CKL() do { if (launches) ++*launches; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) return e_; } while (0)
@@ -595,7 +595,7 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
     m.d_tokens = a.d_tokens; m.d_pos = a.d_pos;
     m.d_bu_w1 = a.d_bu_w1; m.d_bu_w2 = a.d_bu_w2; m.d_td_w1 = a.d_td_w1; m.d_td_w2 = a.d_td_w2;
     m.d_bu_b1 = a.d_bu_b1; m.d_td_b1 = a.d_td_b1;
-    pack_bwd_weights_kernel<<<148 * 8, 256, 0, st>>>(g.d, g.L, a.bu_w1, a.bu_b1, a.bu_w2, a.td_w1, a.td_b1, a.td_w2,
+    pack_bwd_weights_kernel<<<sm_count() * 8, 256, 0, st>>>(g.d, g.L, a.bu_w1, a.bu_b1, a.bu_w2, a.td_w1, a.td_b1, a.td_w2,
                                                      const_cast<__nv_bfloat16*>(m.w1p), const_cast<__nv_bfloat16*>(m.w2t),
                                                      const_cast<__nv_bfloat16*>(m.w1t), const_cast<float*>(m.b1p));
     CKLI();

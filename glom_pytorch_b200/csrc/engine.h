@@ -137,7 +137,7 @@ cudaError_t launch_clock_probe(unsigned long long* out, unsigned long long spin_
 cudaError_t tc_kernel_clocks(unsigned long long* out /* [PROF_KINDS][8] */, bool reset);
 cudaError_t mlp_kernel_clocks(unsigned long long* out /* [2] */, bool reset);
 
-// bf16 tokeniser: patchify + cast (CUDA cores), then the tcgen05 GEMM
+// bf16 tokeniser: patchify + cast (CUDA cores), then the wgmma GEMM
 cudaError_t launch_patchify_bf16(const float* img, const float* w, __nv_bfloat16* patches, __nv_bfloat16* wtok, int B,
                                  int H, int W, int p, int d, int kp, cudaStream_t st, int* launches);
 int tokenize_tc(const __nv_bfloat16* patches, const __nv_bfloat16* wtok, const float* bias, float* tokens, int rows,
@@ -211,5 +211,13 @@ struct SmemOptIn {
 };
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// SM count of the current device: grid caps of the grid-stride CUDA-core kernels are a few waves of it
+static inline int sm_count() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1)
+    n = 132;
+  return n;
+}
 
 }  // namespace glom

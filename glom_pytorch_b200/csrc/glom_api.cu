@@ -78,7 +78,7 @@ static int check_cfg(const glom_b200_cfg* cfg) {
   if (cfg->precision != GLOM_B200_FP32 && cfg->precision != GLOM_B200_BF16)
     return fail(GLOM_B200_ERR_INVALID, "unknown precision %d", cfg->precision);
   if (cfg->precision == GLOM_B200_BF16 && cfg->dim % 64)
-    return fail(GLOM_B200_ERR_INVALID, "bf16 (tcgen05) precision needs dim %% 64 == 0 (got %d); use fp32 precision", cfg->dim);
+    return fail(GLOM_B200_ERR_INVALID, "bf16 (tensor-core) precision needs dim %% 64 == 0 (got %d); use fp32 precision", cfg->dim);
   if (cfg->mask_side < 0 || (cfg->mask_side > 0 && cfg->n % cfg->mask_side))
     return fail(GLOM_B200_ERR_INVALID, "mask_side %d does not tile n = %d", cfg->mask_side, cfg->n);
   return 0;
@@ -114,7 +114,7 @@ static int device_info(DeviceInfo* out) {
     e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "cudaDeviceGetAttribute: %s", cudaGetErrorString(e));
-    g_dev[dev].ok = (major == 10);
+    g_dev[dev].ok = (major == 9);
     g_dev[dev].sms = sms;
     g_dev_known[dev] = true;
     // GLOM_B200_L2_PERSIST_MB (diagnostics): set-aside for L2 lines written / read with an evict-last policy
@@ -136,7 +136,7 @@ static int device_info(DeviceInfo* out) {
     g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   }
   *out = g_dev[dev];
-  if (!out->ok) return fail(GLOM_B200_ERR_DEVICE, "device %d is not compute capability 10.x (sm_100a kernels only)", dev);
+  if (!out->ok) return fail(GLOM_B200_ERR_DEVICE, "device %d is not compute capability 9.x (sm_90a kernels only)", dev);
   return 0;
 }
 
@@ -279,8 +279,8 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
     if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "prep launch: %s", cudaGetErrorString(e));
     // The step is three launches (GEMM1+GELU, consensus, GEMM2+combine).  GLOM_B200_MERGED_MLP=1 (A/B experiment, kept
     // bit-identical and tested) replaces the two GEMM launches by the merged persistent MLP kernel (dim % 256 == 0): its
-    // list heads / dependency counters for every step are zeroed once per call.  Measured slower on B200 (profiles/README.md,
-    // r2: H does not survive in L2 between its GEMM1 and GEMM2 tiles), hence opt-in.
+    // list heads / dependency counters for every step are zeroed once per call.  Opt-in: the three-launch step is the
+    // default path.
     const char* merged_env = getenv("GLOM_B200_MERGED_MLP");     // read per call: tests toggle it in-process
     const bool split_mlp = !(merged_env && merged_env[0] == '1');
     int* sched = nullptr;

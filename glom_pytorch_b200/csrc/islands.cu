@@ -1,5 +1,4 @@
-// Island analytics on the column states (SURVEY 8 row f4; README.md:34-36 of the reference: "access to all the level
-// data across iterations for clustering, from which one can inspect for the theorized islands").
+// Island analytics on the column states.
 //
 // Input: `slabs` states of shape (n = side_h * side_w patches, L levels, d) fp32 -- e.g. the (T+1) * B slabs of
 // Glom.forward(..., return_all=True).  Per slab and level, on the patch grid (patch i = h * side_w + w):

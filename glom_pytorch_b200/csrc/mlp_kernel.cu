@@ -1,10 +1,11 @@
-// Merged persistent MLP kernel of the GLOM column update for sm_100a (dim % 256 == 0).
+// Merged persistent MLP kernel of the GLOM column update for sm_90a (dim % 256 == 0).
 //
 //   mlp_kernel: one launch per Jacobi step runs BOTH grouped GEMMs of GroupedFeedForward for all levels
 //     K1 tiles  H_g   = gelu_erf(A_g . W1_g^T + b1_g)                         (glom_pytorch.py:29-30, calls :134/:136)
 //     K2 tiles  S'_l  = (S_l + C_l + [H_bu,l | H_td,l] . [W2bu_l | W2td_l]^T + b2_l) / c_l   (:31, :137, :141-142)
-//   as 256 x 256 CTA-pair tiles (tcgen05 cta_group::2, the machinery of gemm_kernel in tc_kernels.cu) drawn from ONE
-//   ordered work list by a dynamic scheduler, with per-(level, row block) dependency counters in global memory:
+//   as 256 x 256 tiles of a cluster of two CTAs (each CTA computes 128 of the rows with the TMA + wgmma machinery of
+//   gemm_kernel in tc_kernels.cu) drawn from ONE ordered work list by a dynamic scheduler, with per-(level, row block)
+//   dependency counters in global memory:
 //
 //   * Work lists: two ordered lists, both level-major (top level last: its GEMM2 tiles cost half, which keeps the
 //     tail short) and then by 256-row block: the K1 list (per row block: both MLP groups x 4d/256 column tiles) and the
@@ -15,19 +16,15 @@
 //     (compare-and-swap on the K2 counter), else the next K1 tile (atomicAdd); once the K1 list is exhausted everybody
 //     takes K2 tiles in order (their dependencies are claimed, running, and never wait themselves: no deadlock).  The
 //     threshold is lower for a cluster whose previous tile was a K2 tile, so clusters keep their role for long stretches
-//     while the NUMBER of clusters on each kind adapts to the two kinds' actual rates.  Why roles: a K2 tile's MMAs take
-//     8x a K1 tile's and its epilogue (fp32 state in / out, C, two shadows: ~20 k cycles) as long as five K1 tiles; with
-//     two TMEM accumulator stages a K1 tile scheduled behind a K2 tile waits for that epilogue to drain (measured with
-//     the mixed in-order list of r2a: MMA lane 22 % waiting for a free accumulator).  A cluster that stays on K2 tiles
-//     hides each epilogue behind the next tile's 32 k cycles of MMAs; one that stays on K1 tiles alternates stages
-//     every ~4-7 k cycles.  H is consumed a few row blocks (~10 us) after it was written, while still in L2: the
-//     2 x 369 MB HBM round trip of the two-kernel path becomes L2 traffic plus the eventual write-back.
-//     The drawn tile is published through an 8-slot shared-memory ring to the MMA / epilogue / publisher roles of BOTH
+//     while the NUMBER of clusters on each kind adapts to the two kinds' actual rates.  H is consumed a few row blocks
+//     after it was written, while still in L2: the HBM round trip of H in the two-kernel path becomes L2 traffic plus
+//     the eventual write-back.
+//     The drawn tile is published through an 8-slot shared-memory ring to the consumer / publisher roles of BOTH
 //     CTAs of the pair and to the peer's TMA lane (local store + mbarrier for its own CTA, st.async + complete_tx for
 //     the peer).
-//   * Dependencies: the 16 epilogue warps of a CTA arrive on a shared-memory mbarrier once their stores of a tile are
+//   * Dependencies: the 8 consumer warps of a CTA arrive on a shared-memory mbarrier once their stores of a tile are
 //     issued; one publisher lane per CTA turns that into ONE gpu-scope release (red.release.gpu.add on
-//     ready[level][row block]) per CTA and K1 tile, off the epilogue warps' critical path (cumulativity: stores ->
+//     ready[level][row block]) per CTA and K1 tile, off the consumer warps' critical path (cumulativity: stores ->
 //     warp barrier -> mbarrier arrive / wait -> release).  The TMA producers of a K2 tile wait (ld.acquire.gpu) for all
 //     2 x (K1 tiles of the row block) arrivals and cross into the async proxy (fence.proxy.async.global) before their
 //     first load of H.
@@ -39,16 +36,16 @@
 namespace glom {
 
 constexpr int MLP_BN = 256;
-constexpr int MLP_STAGES = 5;
-constexpr int MLP_EPI_WARPS = 16;                 // 4 TMEM lane quadrants x 4 column parts of 64
-constexpr int MLP_CTRL_WARPS = 4;                 // TMA (+ scheduler in the leader), MMA, TMEM allocator, publisher
-constexpr int MLP_THREADS = 32 * (MLP_EPI_WARPS + MLP_CTRL_WARPS);
+constexpr int MLP_STAGES = 3;
+constexpr int MLP_CONSUMER_WARPS = 8;             // two warpgroups of 64 rows each: wgmma main loop + epilogue
+constexpr int MLP_CTRL_WARPS = 2;                 // TMA (+ scheduler in the leader), publisher
+constexpr int MLP_THREADS = 32 * (MLP_CONSUMER_WARPS + MLP_CTRL_WARPS);
 constexpr int MLP_SLOTS = 8;                      // scheduler ring
-constexpr uint32_t MLP_STAGE_BYTES = A_STAGE_BYTES + (MLP_BN / 2) * BK * 2;     // 32 KB: A (128 x 64) + half of B
-constexpr uint32_t MLP_PATCH_BYTES = 4096;        // per-warp transpose patch (K2: 32 x 32 fp32; K1: 2 KB + its bias slice)
-constexpr uint32_t MLP_TMEM_COLS = 2 * MLP_BN;    // two accumulator stages
-constexpr size_t MLP_SMEM_BYTES = 1024 + (size_t)MLP_STAGES * MLP_STAGE_BYTES + (size_t)MLP_EPI_WARPS * MLP_PATCH_BYTES + 512;
-constexpr int MLP_SEMPTY_COUNT = (MLP_EPI_WARPS + 2) + (MLP_EPI_WARPS + 2);   // leader: epilogue + MMA + publisher; peer: epilogue + TMA + publisher
+constexpr uint32_t MLP_STAGE_BYTES = A_STAGE_BYTES + MLP_BN * BK * 2;     // 48 KB: A (128 x 64) + B (256 x 64)
+constexpr uint32_t MLP_PATCH_BYTES = 4096;        // per-warp transpose patch (K2: 32 x 32 fp32; K1: 2 KB)
+constexpr size_t MLP_SMEM_BYTES = 1024 + (size_t)MLP_STAGES * MLP_STAGE_BYTES + 4 * (size_t)STG_BYTES +
+                                  (size_t)MLP_CONSUMER_WARPS * MLP_PATCH_BYTES + 4 * 32 * 4 + 512;
+constexpr int MLP_SEMPTY_COUNT = (MLP_CONSUMER_WARPS + 1) + (MLP_CONSUMER_WARPS + 2);   // leader: consumers + publisher; peer: consumers + TMA + publisher
 constexpr int MLP_MAX_LEVELS = 16;
 
 __device__ unsigned long long g_mlp_clk[2];     // in-kernel clock sample (cycles, ns), see clock_sample_begin
@@ -103,7 +100,7 @@ __host__ __device__ __forceinline__ MlpTile mlp_decode2(const MlpParams& p, int 
 }
 
 // Ring entries are PACKED tile descriptors (decoded once, by the claiming lane: the list position -> tile mapping
-// needs integer divisions, ~100 instructions that 34 warps per pair would otherwise repeat for every tile):
+// needs integer divisions, ~100 instructions that every warp of the pair would otherwise repeat for every tile):
 //   bit 0 kind | bits 1-4 level | bit 5 group within the level (K1) | bits 6-11 n_blk | bits 12-30 m_blk ; -1 = end
 __host__ __device__ __forceinline__ int mlp_pack(const MlpTile& t) {
   return t.kind | (t.l << 1) | ((t.kind == 0 ? (t.z & 1) : 0) << 5) | (t.n_blk << 6) | (t.m_blk << 12);
@@ -159,45 +156,37 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
            const MlpParams p) {
   constexpr int STAGES = MLP_STAGES;
   constexpr int BN = MLP_BN;
-  constexpr int PART_COLS = 64;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* patches = smem + (size_t)STAGES * MLP_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(patches + (size_t)MLP_EPI_WARPS * MLP_PATCH_BYTES);
+  float* stg_all = reinterpret_cast<float*>(smem + (size_t)STAGES * MLP_STAGE_BYTES);
+  uint8_t* patches = reinterpret_cast<uint8_t*>(stg_all) + 4 * STG_BYTES;
+  float* xch = reinterpret_cast<float*>(patches + (size_t)MLP_CONSUMER_WARPS * MLP_PATCH_BYTES);   // [4 pairs][32]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(xch + 4 * 32);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* sfull_bar = tempty_bar + 2;               // [MLP_SLOTS] own: tile index of the slot published
+  uint64_t* sfull_bar = empty_bar + STAGES;           // [MLP_SLOTS] own: tile index of the slot published
   uint64_t* sempty_bar = sfull_bar + MLP_SLOTS;       // [MLP_SLOTS] leader's: every consumer of both CTAs has read it
-  uint64_t* pub_bar = sempty_bar + MLP_SLOTS;         // [2] own: the 16 epilogue warps issued their stores of the tile in stage `as`
+  uint64_t* pub_bar = sempty_bar + MLP_SLOTS;         // [2] own: the consumer warps issued their stores of the tile
   int* stile = reinterpret_cast<int*>(pub_bar + 2);   // [MLP_SLOTS]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stile + MLP_SLOTS);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  constexpr int W_TMA = MLP_EPI_WARPS, W_MMA = MLP_EPI_WARPS + 1, W_ALLOC = MLP_EPI_WARPS + 2, W_SCHED = MLP_EPI_WARPS + 3;
+  constexpr int W_TMA = MLP_CONSUMER_WARPS, W_SCHED = MLP_CONSUMER_WARPS + 1;
   const uint32_t cta_rank = cluster_ctarank();
   const bool leader = cta_rank == 0;
 
   if (warp == W_TMA && lane == 0) {
     tma_prefetch_desc(&map_x); tma_prefetch_desc(&map_sb); tma_prefetch_desc(&map_sp);
     tma_prefetch_desc(&map_w1); tma_prefetch_desc(&map_h); tma_prefetch_desc(&map_w2);
-  }
-  if (warp == W_MMA && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 2 * MLP_EPI_WARPS); mbar_init(&pub_bar[i], MLP_EPI_WARPS); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], MLP_CONSUMER_WARPS); }
+    for (int i = 0; i < 2; ++i) mbar_init(&pub_bar[i], MLP_CONSUMER_WARPS);
     for (int i = 0; i < MLP_SLOTS; ++i) { mbar_init(&sfull_bar[i], 1); mbar_init(&sempty_bar[i], MLP_SEMPTY_COUNT); }
     fence_barrier_init();
   }
-  if (warp == W_ALLOC) tmem_alloc_2sm(tmem_slot, MLP_TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  cluster_sync_all();          // peer barriers initialised + both TMEM allocations done before any cross-CTA traffic
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
+  cluster_sync_all();          // peer barriers initialised before any cross-CTA traffic
   pdl_launch_dependents();
   pdl_wait();                  // global memory (counters included) is touched only after the previous kernel finished
-  const bool clk_thread = blockIdx.x == 0 && warp == W_ALLOC && lane == 0;
+  const bool clk_thread = blockIdx.x == 0 && warp == W_SCHED && lane == 0;
   ClockSample clk_s{};
   if (clk_thread) clk_s = clock_sample_begin();
 
@@ -208,7 +197,7 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
 
   if (warp == W_SCHED) {
     // ------------------------------------------------------------------ publisher (both CTAs, one lane)
-    // once all 16 epilogue warps of this CTA have issued their stores of a K1 tile: one gpu-scope release of the
+    // once all consumer warps of this CTA have issued their stores of a K1 tile: one gpu-scope release of the
     // (level, row block) counter for the whole CTA
     if (lane == 0) {
       int as = 0; uint32_t aphase = 0;
@@ -231,16 +220,15 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
     int stage = 0; uint32_t phase = 0;
     const uint64_t pol_first = l2_policy_evict_first();
     const uint32_t smem0 = smem_u32(smem);
-    const uint32_t bar0 = mapa_shared(smem_u32(&full_bar[0]), 0);
     const int kbg_n = 4 * p.d / BK;
     const int blk_skip = (p.m128 - 1) * kbg_n;
     // leader: draws the tile index and publishes it to the ring (both CTAs); peer: reads the ring like everyone else
     uint32_t pub_seq = 0;
     int last_kind = 0;
     // The draw is a chain of dependent L2 round trips (list heads -> dependency counter -> compare-and-swap / add, ~1.5 k
-    // cycles).  Done in one piece between two loads it starves the MMA pipe (measured: MMA lane 59 % waiting for
-    // operands); it is therefore split into four phases issued two k-blocks apart, so each phase's result has arrived
-    // when the next one needs it and the TMA issue stream never waits on it.
+    // cycles).  Done in one piece between two loads it would stall the load stream feeding the consumers; it is therefore
+    // split into four phases issued two k-blocks apart, so each phase's result has arrived when the next one needs it
+    // and the TMA issue stream never waits on it.
     int c_i1 = 0, c_j = 0, c_ready = 0, c_res = 0, c_mode = 0;      // c_mode: 0 = K1 add pending, 1 = K2 cas pending
     auto claim_a = [&]() {                          // list heads (approximate: others move them)
       c_i1 = *reinterpret_cast<volatile int*>(p.counter);
@@ -279,7 +267,7 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
       if (DBG && tile >= 0) { if (tile & 1) { ++dw4; if (!last_kind) dw4 += 1ull << 32; } }
       last_kind = tile >= 0 ? (tile & 1) : 0;
       const uint32_t slot = pub_seq % MLP_SLOTS, ph = (pub_seq / MLP_SLOTS) & 1u;
-      mbar_wait(&sempty_bar[slot], ph ^ 1u);                  // all 36 readers of the slot's previous use are done
+      mbar_wait(&sempty_bar[slot], ph ^ 1u);                  // all readers of the slot's previous use are done
       *reinterpret_cast<volatile int*>(&stile[slot]) = tile;
       mbar_arrive(&sfull_bar[slot]);                                        // own CTA (release.cta)
       const uint32_t rbar = mapa_shared(smem_u32(&sfull_bar[slot]), 1);
@@ -323,11 +311,7 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
             if (DBG) ++dw3;
             while (ld_acquire_gpu(ctr) < need) {
               __nanosleep(64);
-              if (clock64() - t0 > GLOM_WAIT_TIMEOUT_CYCLES) {
-                printf("glom_b200: mlp_kernel dependency wait timed out (block %d level %d row block %d: %d of %d)\n",
-                       (int)blockIdx.x, t.l, t.m_blk, ld_acquire_gpu(ctr), need);
-                __trap();
-              }
+              if (clock64() - t0 > GLOM_WAIT_TIMEOUT_CYCLES) asm volatile("trap;");
             }
             if (DBG) dw1 += (unsigned long long)(clock64() - t0);
           }
@@ -336,7 +320,6 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
         __syncwarp();
       }
       const int a_row = t.m_blk * 256 + (int)cta_rank * BM;
-      b_row += (int)cta_rank * (BN / 2);
       // K2: block (group g, 128-row block, 64-wide k block); [H_bu,l | H_td,l] are groups 2l and 2l+1
       const int blk0 = (2 * t.z * p.m128 + (a_row >> 7)) * kbg_n;
       // the row block's H is read by all nN2 column tiles: only the last one may mark it evict-first
@@ -360,17 +343,19 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
         MLP_TIMED(dw2, mbar_wait(&empty_bar[stage], phase ^ 1));
         if (elected) {
           const uint32_t sa = smem0 + (uint32_t)stage * MLP_STAGE_BYTES;
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * MLP_STAGE_BYTES);   // both CTAs' bytes land here
-          const uint32_t bar = bar0 + 8u * (uint32_t)stage;
+          uint64_t* bar = &full_bar[stage];
+          mbar_arrive_expect_tx(bar, MLP_STAGE_BYTES);
           if (t.kind == 1) {
             const int blk = blk0 + kb + (kb >= kbg_n ? blk_skip : 0);
             // last use of these lines by this column tile: evict-first keeps them from displacing weights / state
-            if (h_first) tma_load_2d_2sm_sa_hint(sa, amap, bar, 0, blk * BM, pol_first);
-            else tma_load_2d_2sm_sa(sa, amap, bar, 0, blk * BM);
+            if (h_first) tma_load_2d_hint(sa, amap, bar, 0, blk * BM, pol_first);
+            else tma_load_2d(sa, amap, bar, 0, blk * BM);
           } else {
-            tma_load_2d_2sm_sa(sa, amap, bar, a_col + kb * BK, a_row);
+            tma_load_2d(sa, amap, bar, a_col + kb * BK, a_row);
           }
-          tma_load_2d_2sm_sa(sa + A_STAGE_BYTES, bmap, bar, kb * BK, b_row);
+          // the B tile as two boxes of 128 rows
+          tma_load_2d(sa + A_STAGE_BYTES, bmap, bar, kb * BK, b_row);
+          tma_load_2d(sa + A_STAGE_BYTES + (BN / 2) * BK * 2, bmap, bar, kb * BK, b_row + BN / 2);
         }
         __syncwarp();
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -378,137 +363,106 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
       if (leader) next_tile = __shfl_sync(0xffffffffu, next_tile, elected_lane);
     }
     if (DBG && elected) { dbg[2] = dw0; dbg[3] = dw1; dbg[4] = dw2; dbg[15] = dw3; if (leader) dbg[12] = dw4; }
-  } else if (warp == W_MMA) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA only), warp-converged
-    if (leader) {
-      constexpr uint32_t idesc = umma_idesc_bf16(256, BN, 0, 0);
-      const uint32_t elected = elect_one();
-      const uint64_t a_desc0 = umma_desc_sw128(smem_u32(smem), 16, 1024);
-      const uint64_t b_desc0 = umma_desc_sw128(smem_u32(smem) + A_STAGE_BYTES, 16, 1024);
-      int stage = 0; uint32_t phase = 0;
-      int as = 0; uint32_t aphase = 0;
-      for (uint32_t seq = 0;; ++seq) {
-        int tile;
-        MLP_TIMED(dw0, tile = mlp_fetch_warp(sfull_bar, stile, sempty_leader, seq, elected));
-        if (tile < 0) break;
-        const MlpTile t = mlp_unpack(p, tile);
-        MLP_TIMED(dw1, mbar_wait(&tempty_bar[as], aphase ^ 1));      // both CTAs' epilogues drained this accumulator stage
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(as * BN);
-        for (int kb = 0; kb < t.num_kb; ++kb) {
-          MLP_TIMED(dw2, mbar_wait(&full_bar[stage], phase));
-          tc_fence_after_sync();
-          if (elected) {
-            const uint64_t ad = a_desc0 + (uint64_t)(stage * (int)(MLP_STAGE_BYTES >> 4));
-            const uint64_t bd = b_desc0 + (uint64_t)(stage * (int)(MLP_STAGE_BYTES >> 4));
-            umma_bf16_2sm(d_tmem, ad, bd, idesc, kb != 0 ? 1u : 0u);
-#pragma unroll
-            for (int k = 1; k < BK / 16; ++k) umma_bf16_2sm(d_tmem, ad + 2 * k, bd + 2 * k, idesc, 1u);
-            umma_commit_2sm(&empty_bar[stage], 3);     // frees the slot in both CTAs
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (elected) umma_commit_2sm(&tfull_bar[as], 3);          // accumulator complete -> both epilogues
-        __syncwarp();
-        if (++as == 2) { as = 0; aphase ^= 1; }
-        if (DBG) ++dw3;
-      }
-      if (DBG && elected) { dbg[5] = dw0; dbg[6] = dw1; dbg[7] = dw2; dbg[14] = dw3; }
-    }
-  } else if (warp < MLP_EPI_WARPS) {
-    // ------------------------------------------------------------------ epilogue (16 warps)
-    const int quad = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int part = warp >> 2;                // 64-column part of the tile
+  } else if (warp < MLP_CONSUMER_WARPS) {
+    // ------------------------------------------------------------------ consumers: wgmma main loop + epilogue (8 warps)
+    const int wg = warp >> 2, wi = warp & 3;
+    const int pair = warp >> 1, x = warp & 1;  // warp pair = 32-row band `pair` of the CTA's 128 rows; x = its 32-column half
+    float* stg = stg_all + pair * (STG_BYTES / 4);
     uint8_t* patch = patches + (size_t)warp * MLP_PATCH_BYTES;
-    float* bias_w = reinterpret_cast<float*>(patch + 2048);      // K1: this warp's 64 bias values (upper patch half)
+    float* xch_p = xch + pair * 32;
+    const uint32_t smem0 = smem_u32(smem);
     // H should stay in L2 until this launch's GEMM2 tiles have read it
     const uint64_t pol_h = p.h_store_policy == 0 ? l2_policy_evict_last() : l2_policy_evict_normal();
+    int stage = 0; uint32_t phase = 0;
     int as = 0; uint32_t aphase = 0;
+    float acc[BN / 2];
     for (uint32_t seq = 0;; ++seq) {
       int tile = 0;
       if (lane == 0) MLP_TIMED(dw0, tile = mlp_fetch(sfull_bar, stile, sempty_leader, seq));
       tile = __shfl_sync(0xffffffffu, tile, 0);
       if (tile < 0) break;
       const MlpTile t = mlp_unpack(p, tile);
-      const int row0 = t.m_blk * 256 + (int)cta_rank * BM + quad * 32;   // first row of this warp's 32-row band
+      const int row0 = t.m_blk * 256 + (int)cta_rank * BM + pair * 32;   // first row of this warp pair's 32-row band
       const int rows_left = p.rows - row0;                                // >= 32: whole band valid (warp-uniform)
-      // bias of this warp's columns: fetched before the accumulator wait, so the L2 latency overlaps the MMAs
-      float4 b4k2[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
-      if (t.kind == 0) {
-        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.b1 + (size_t)t.z * 4 * p.d + t.n_blk * BN + part * PART_COLS) + lane);
-        *reinterpret_cast<float2*>(bias_w + 2 * lane) = bv;
-        __syncwarp();
-      } else {
-        const float* bsrc = p.b2 + (size_t)t.z * p.d + t.n_blk * BN + part * PART_COLS + (lane & 7) * 4;
-        b4k2[0] = __ldg(reinterpret_cast<const float4*>(bsrc));
-        b4k2[1] = __ldg(reinterpret_cast<const float4*>(bsrc + 32));
-        // The combine reads this warp's 32 x 64 patch of the fp32 state (streamed to HBM by the previous step) and of C.
-        // Pull those lines into L2 now, ~20 us before the accumulator is complete: the epilogue's dependent global loads
-        // then hit L2 (measured without this: 32 k cycles per K2 tile, as long as its MMAs, and the K1 tiles that follow
-        // in the list stall on the undrained accumulator stage).
-        if (lane < rows_left) {
-          const size_t o = ((size_t)(row0 + lane) * p.L + t.z) * p.d + t.n_blk * BN + part * PART_COLS;
-          if (!p.s_bcast) {
-            prefetch_l2(p.s32_in + o);
-            prefetch_l2(p.s32_in + o + 32);
-          }
-          prefetch_l2(p.c_in + o);
+      if (t.kind == 1 && lane < rows_left) {
+        // The combine reads this band's fp32 state and C lines: pull them into L2 before the main loop, so the epilogue's
+        // dependent global loads hit L2
+        const size_t o = ((size_t)(row0 + lane) * p.L + t.z) * p.d + t.n_blk * BN + x * (BN / 2);
+#pragma unroll
+        for (int c = 0; c < BN / 2; c += 32) {
+          if (!p.s_bcast) prefetch_l2(p.s32_in + o + c);
+          if ((c & 63) == 0) prefetch_l2(p.c_in + o + c);
         }
       }
-      MLP_TIMED(dw1, mbar_wait(&tfull_bar[as], aphase));
-      tc_fence_after_sync();
-      const long long e_t0 = DBG ? clock64() : 0;
-      const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * BN + part * PART_COLS);
-      if (t.kind == 0) {
-        // H block (group, 128-row block, k block = this warp's 64-column part): 16 KB contiguous, row pitch 64
-        const int hblk = (t.z * p.m128 + (t.m_blk * 2 + (int)cta_rank)) * (4 * p.d / BK) + t.n_blk * (BN / BK) + part;
-        __nv_bfloat16* hrow = p.h + ((size_t)hblk * BM + quad * 32) * BK;
-#pragma unroll 1
-        for (int c0 = 0; c0 < PART_COLS; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(t_addr + c0, v);
-          tmem_ld_wait();
-          if (rows_left >= 32) k1_chunk<true, 1>(v, bias_w + c0, patch, hrow + c0, (size_t)BK, lane, 32, pol_h);
-          else k1_chunk<false, 1>(v, bias_w + c0, patch, hrow + c0, (size_t)BK, lane, rows_left, pol_h);
-        }
-      } else {
-        K2Chunk kc;
-        kc.l = t.z; kc.L = p.L; kc.d = p.d; kc.n = p.n; kc.row0 = row0; kc.prow0 = row0 % p.n; kc.s_bcast = p.s_bcast;
-        kc.s32_in = p.s32_in; kc.c_in = p.c_in; kc.pos = p.pos;
-        kc.s32_out = p.s32_out; kc.sb_out = p.sb_out; kc.sp_out = p.sp_out;
-        float rowsq[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) rowsq[i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;                    // slot of the k-block whose MMAs may still be running
+      for (int kb = 0; kb < t.num_kb; ++kb) {
+        MLP_TIMED(dw1, mbar_wait(&full_bar[stage], phase));
+        const uint32_t sa = smem0 + (uint32_t)stage * MLP_STAGE_BYTES;
+        wgmma_fence_regs(acc);
+        wgmma_fence();
+        wgmma_kblock<BN, 0>(acc, sa + (uint32_t)wg * (A_STAGE_BYTES / 2), sa + A_STAGE_BYTES);
+        wgmma_commit();
+        wgmma_wait<1>();                  // the previous k-block's MMAs are complete: release its slot
+        wgmma_fence_regs(acc);
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      const long long e_t0 = DBG ? clock64() : 0;
 #pragma unroll 1
-        for (int ci = 0; ci < 2; ++ci) {
-          const int c0 = ci * 32;
-          uint32_t v[32];
-          tmem_ld32(t_addr + c0, v);
-          tmem_ld_wait();
-          const int col = t.n_blk * BN + part * PART_COLS + c0;
-          const float4 b4 = ci ? b4k2[1] : b4k2[0];
+      for (int s = 0; s < BN / 64; ++s) {
+        stage_write(acc, stg, s, wi, lane);
+        named_bar_sync(1 + pair, 64);
+        uint32_t v[32];
+        stage_read(stg, x, lane, v);
+        const int cc = 64 * s + 32 * x;                               // column of this chunk inside the tile
+        if (t.kind == 0) {
+          // H block (group, 128-row block, k block = this 64-column step): 16 KB contiguous, row pitch 64
+          const int hblk = (t.z * p.m128 + (t.m_blk * 2 + (int)cta_rank)) * (4 * p.d / BK) + t.n_blk * (BN / BK) + s;
+          __nv_bfloat16* hrow = p.h + ((size_t)hblk * BM + pair * 32) * BK + 32 * x;
+          const float* bias = p.b1 + (size_t)t.z * 4 * p.d + t.n_blk * BN + cc;
+          if (rows_left >= 32) k1_chunk<true, 1>(v, bias, patch, hrow, (size_t)BK, lane, 32, pol_h);
+          else k1_chunk<false, 1>(v, bias, patch, hrow, (size_t)BK, lane, rows_left, pol_h);
+        } else {
+          K2Chunk kc;
+          kc.l = t.z; kc.L = p.L; kc.d = p.d; kc.n = p.n; kc.row0 = row0; kc.prow0 = row0 % p.n; kc.s_bcast = p.s_bcast;
+          kc.s32_in = p.s32_in; kc.c_in = p.c_in; kc.pos = p.pos;
+          kc.s32_out = p.s32_out; kc.sb_out = p.sb_out; kc.sp_out = p.sp_out;
+          const int col = t.n_blk * BN + cc;
+          const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.b2 + (size_t)t.z * p.d + col + (lane & 7) * 4));
+          float rowsq[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) rowsq[i] = 0.f;
           if (rows_left >= 32) k2_chunk<true>(v, b4, patch, kc, col, lane, 32, rowsq);
           else k2_chunk<false>(v, b4, patch, kc, col, lane, rows_left, rowsq);
-        }
-        if ((lane & 7) == 0) {
+          // one squared-norm partial per 64 columns: the two warps of the pair hold its 32-column halves, summed in chunk
+          // order (0 + first) + second as in prep_state_kernel
+          if (x == 1 && (lane & 7) == 0) {
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int r = i * 4 + (lane >> 3);
-            if (r < rows_left)
-              p.nsq_out[((size_t)(row0 + r) * p.L + t.z) * p.nparts + t.n_blk * 4 + part] = rowsq[i];
+            for (int i = 0; i < 8; ++i) xch_p[i * 4 + (lane >> 3)] = rowsq[i];
+          }
+          named_bar_sync(1 + pair, 64);
+          if (x == 0 && (lane & 7) == 0) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int r = i * 4 + (lane >> 3);
+              const float q = rowsq[i] + xch_p[i * 4 + (lane >> 3)];
+              if (r < rows_left) p.nsq_out[((size_t)(row0 + r) * p.L + t.z) * p.nparts + t.n_blk * 4 + s] = q;
+            }
           }
         }
+        named_bar_sync(1 + pair, 64);                                   // staging tile free for the next step
       }
-      // release this accumulator stage to the leader's MMA issuer: one arrival per epilogue warp of either CTA
-      tc_fence_before_sync();
+      // this warp's stores of the tile are issued: tell the CTA's publisher lane (it releases them at gpu scope for
+      // K1 tiles; the lanes' stores are ordered before lane 0's arrive by the warp barrier)
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive_cluster(mapa_shared(smem_u32(&tempty_bar[as]), 0));
-        // this warp's stores of the tile are issued: tell the CTA's publisher lane (it releases them at gpu scope for
-        // K1 tiles; the lanes' stores are ordered before lane 0's arrive by the warp barrier above)
-        mbar_arrive(&pub_bar[as]);
-      }
+      if (lane == 0) mbar_arrive(&pub_bar[as]);
       if (++as == 2) { as = 0; aphase ^= 1; }
       if (DBG) { if (t.kind == 0) dw2 += (unsigned long long)(clock64() - e_t0); else dw3 += (unsigned long long)(clock64() - e_t0); }
     }
@@ -518,14 +472,9 @@ mlp_kernel(const __grid_constant__ CUtensorMap map_x,    // tokens Xb (rows, d)
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
   if (clk_thread) clock_sample_end(clk_s, g_mlp_clk);
-  cluster_sync_all();          // no CTA exits (or frees TMEM) while its pair can still touch it
-  if (warp == W_ALLOC) {
-    tc_fence_after_sync();
-    tmem_dealloc_2sm(tmem_base, MLP_TMEM_COLS);
-  }
+  cluster_sync_all();          // no CTA exits while its pair can still touch its shared memory
 }
 
 cudaError_t mlp_kernel_clocks(unsigned long long* out /* [2] */, bool reset) {
@@ -655,9 +604,9 @@ int step_bf16_mlp_fused(const Geometry& g, const Bf16Buffers& b, int* sched, Enc
   if (dbg) {
     --dbg_left;
     static const char* names[16] = {"pub: wait epilogue stores", "pub: release", "tma: claim / fetch tile", "tma: dependency wait",
-                                    "tma: wait smem slot", "mma: fetch tile", "mma: wait accumulator free", "mma: wait operands",
-                                    "epi w0: fetch tile", "epi w0: wait accumulator", "epi w0: K1 tiles work", "epi w0: K2 tiles work",
-                                    "tma: K2 tiles (+ 2^32 per K1->K2 switch)", "epi w0: kernel total", "mma: tiles", "tma: dependency waits (count)"};
+                                    "tma: wait smem slot", "-", "-", "-",
+                                    "consumer w0: fetch tile", "consumer w0: wait operands", "consumer w0: K1 tiles epilogue", "consumer w0: K2 tiles epilogue",
+                                    "tma: K2 tiles (+ 2^32 per K1->K2 switch)", "consumer w0: kernel total", "-", "tma: dependency waits (count)"};
     std::vector<unsigned long long> h((size_t)num_sms * 16);
     if (cudaStreamSynchronize(st) == cudaSuccess &&
         cudaMemcpy(h.data(), dbg_buf, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost) == cudaSuccess) {
@@ -666,7 +615,7 @@ int step_bf16_mlp_fused(const Geometry& g, const Bf16Buffers& b, int* sched, Enc
         double sum = 0, mx_ = 0; int cnt = 0;
         for (int c = 0; c < 2 * clusters; ++c) {
           const double v = (double)h[(size_t)c * 16 + k];
-          if (((k >= 5 && k <= 7) || k == 14 || k == 12) && (c & 1)) continue;     // leader-only roles
+          if (k == 12 && (c & 1)) continue;     // leader-only role
           sum += v; if (v > mx_) mx_ = v; ++cnt;
         }
         if (k == 12) {      // packed: K2 tiles in the low word, K1 -> K2 role switches in the high word

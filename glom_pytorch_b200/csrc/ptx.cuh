@@ -1,5 +1,5 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA +
-// TMEM).  Bit layouts follow the PTX ISA's shared-memory / instruction descriptor tables.
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with
+// register accumulators), clusters.  Bit layouts follow the PTX ISA's shared-memory matrix descriptor table.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -10,7 +10,7 @@
 namespace glom {
 
 #ifndef GLOM_WAIT_TIMEOUT_CYCLES
-#define GLOM_WAIT_TIMEOUT_CYCLES (4000000000LL)   // ~2 s at 1.9 GHz: trap instead of hanging the box
+#define GLOM_WAIT_TIMEOUT_CYCLES (4000000000LL)   // ~2 s at 1.98 GHz: trap instead of hanging the GPU
 #endif
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -39,16 +39,13 @@ __device__ __forceinline__ uint32_t mbar_try_wait(uint64_t* bar, uint32_t parity
       : "memory");
   return ok;
 }
-// Bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging.
+// Bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging.  No printf here: a function
+// call between a wgmma and its wait would make ptxas serialise the warpgroup MMAs of the whole kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > GLOM_WAIT_TIMEOUT_CYCLES) {
-      printf("glom_b200: mbarrier wait timed out (block %d thread %d bar %u parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, smem_u32(bar), parity);
-      __trap();
-    }
+    if (clock64() - t0 > GLOM_WAIT_TIMEOUT_CYCLES) asm volatile("trap;");
   }
 }
 
@@ -70,11 +67,7 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
   if (try_wait()) return;
   const long long t0 = clock64();
   while (!try_wait()) {
-    if (clock64() - t0 > GLOM_WAIT_TIMEOUT_CYCLES) {
-      printf("glom_b200: cluster mbarrier wait timed out (block %d thread %d bar %u parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, smem_u32(bar), parity);
-      __trap();
-    }
+    if (clock64() - t0 > GLOM_WAIT_TIMEOUT_CYCLES) asm volatile("trap;");
   }
 }
 
@@ -83,10 +76,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 
 // One lane of a converged warp (all 32 lanes must execute this).  Control warps run their loops warp-converged and
-// predicate the TMA / MMA instructions on the elected lane: issued from inside a divergent `if (lane == 0)` region every
-// uniform-datapath instruction (UTMALDG, UTCHMMA, UTCBAR) is wrapped in an ELECT / BRA.U.ANY loop and its operands
-// are re-materialised, ~80 instructions per k-block -- measured (profiles/r2_epilogue_probe2.txt): that issue stream, not
-// the L2 feed, held the main loop at 81 % of the tensor peak; warp-converged it reaches 100 %.
+// predicate the TMA instructions on the elected lane.
 __device__ __forceinline__ uint32_t elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -94,11 +84,9 @@ __device__ __forceinline__ uint32_t elect_one() {
 }
 
 // ---------------------------------------------------------------- proxies / fences
-__device__ __forceinline__ void fence_proxy_async_smem() {  // generic-proxy smem writes -> async proxy (TMA/UMMA)
+__device__ __forceinline__ void fence_proxy_async_smem() {  // generic-proxy smem writes -> async proxy (TMA/wgmma)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -114,54 +102,70 @@ __device__ __forceinline__ void red_add_f32x4(float* dst, float4 v) {
                : "memory");
 }
 
-// ---------------------------------------------------------------- TMEM (allocation: see the CTA-pair section)
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets row (lane base + t).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors (tcgen05.mma, kind::f16)
-// Shared-memory matrix descriptor, 128-byte swizzle.  start address / LBO / SBO are encoded >> 4.
+// ---------------------------------------------------------------- wgmma (m64nNk16, bf16 in, f32 accumulators in registers)
+// Shared-memory matrix descriptor (sm_90), 128-byte swizzle.  start address / LBO / SBO are encoded >> 4.
 //   K-major operand  (rows x 64 bf16, 128 B per row):   SBO = 1024 (8 rows), LBO unused (canonical 1)
 //   MN-major operand (64 bf16 of MN contiguous per K row): LBO = bytes between 64-wide MN blocks,
 //                                                          SBO = 1024 (8 K rows)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;  // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;  // layout type: SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;  // layout type: SWIZZLE_128B
   return d;
 }
-// Instruction descriptor: D=f32, A=B=bf16, dense, no negate.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// accumulator registers: the compiler must not move their reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2, cluster of 2)
+// D[64 x N] += A[64 x 16] . B[16 x N] for the executing warpgroup.  TA / TB: 1 = operand is MN-major in shared memory.
+// Fragment of thread t (warp w = t / 32 of the warpgroup): d[4j + 2h + e] = D[16 w + (t % 32) / 4 + 8 h][8 j + 2 (t % 4) + e].
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, 1, 1, 1, %34, %35;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, 1, 1, 1, %66, %67;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, 1, 1, 1, %130, %131;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB));
+}
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (N == 256) wgmma_n256<TA, TB>(d, adesc, bdesc);
+  else if constexpr (N == 128) wgmma_n128<TA, TB>(d, adesc, bdesc);
+  else wgmma_n64<TA, TB>(d, adesc, bdesc);
+}
+
+// ---------------------------------------------------------------- clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -207,44 +211,32 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   return v;
 }
 
-// TMA load into THIS CTA's shared memory whose bytes are accounted on an mbarrier given as a
-// shared::cluster address (the pair leader's barrier).
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                int c1) {
+// TMA load into this CTA's shared memory, bytes accounted on this CTA's mbarrier `bar`
+__device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst_smem),
+      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_2sm_sa(uint32_t dst_smem, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1) {
+// same with an L2 cache policy (createpolicy value), e.g. evict-first for operands that stream through once
+__device__ __forceinline__ void tma_load_2d_hint(uint32_t dst_smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                 uint64_t policy) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(dst_smem),
-      "l"(m), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm_sa_hint(uint32_t dst_smem, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                        int c1, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint "
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint "
       "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst_smem),
-      "l"(m), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "l"(policy)
+      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_3d(uint32_t dst_smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst_smem),
+      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
 // L2 prefetch of a tensor-map box (no shared-memory destination, no completion tracking): the later TMA load of the same
 // box then hits L2 instead of waiting on HBM
 __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* m, int c0, int c1) {
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(m), "r"(c0), "r"(c1) : "memory");
-}
-// same with an L2 cache policy (createpolicy value), e.g. evict-first for operands that stream through once
-__device__ __forceinline__ void tma_load_2d_2sm_hint(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                     int c1, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint "
-      "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "l"(policy)
-      : "memory");
 }
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   uint64_t pol;
@@ -266,54 +258,8 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
-__device__ __forceinline__ void tma_load_3d_2sm(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm_sa(uint32_t dst_smem, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0,
-                                                   int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], "
-      "[%2];" ::"r"(dst_smem),
-      "l"(m), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {  // same warp id in both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[256 x N] (+)= A[256 x 16] . B[N x 16]^T over the CTA pair: each CTA supplies 128 rows of A and
-// N/2 rows of B from its own shared memory and receives its 128 rows of D in its own TMEM.
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once) on the mbarrier at this shared-memory offset in every CTA of `cta_mask` when all
-// previously issued MMAs have completed.
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
 // Programmatic dependent launch: `pdl_wait` blocks until the preceding kernel in the stream has completed and its
-// writes are visible; everything before it (barrier init, TMEM allocation, descriptor prefetch) overlaps that
+// writes are visible; everything before it (barrier init, descriptor prefetch) overlaps that
 // kernel's tail.  `pdl_launch_dependents` lets the next kernel's CTAs be scheduled as soon as SMs free up.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -350,54 +296,21 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 
 
-// Packed-pair version for the GEMM1 epilogue (FFMA2 / FADD2: two fp32 lanes per instruction):
-// gelu(acc + bias) for two neighbouring columns, returned as a bf16x2 word.  Uses u = -|x| (one OR per
-// lane instead of abs) and a degree-5 fit of log2(0.5*erfc(a/sqrt2)) on [0,6] whose leading coefficient
-// is negative, so it needs no clamp (p -> -inf, 2^p -> 0 for large |x|); |gelu error| <= 1.9e-6.
-__device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// (r2: a relu-free packed form x/2 + u (e - 1/2) with a degree-4 fit was tried -- 11 instead of 12 instructions per pair,
-// FFMA2 takes -|x| as an operand modifier and the coefficients as immediates either way -- and dropped: an even-degree fit
-// needs a clamp for |x| > 12 (the peaky golden case overflowed), which costs the instruction it saved; a degree-3 fit is
-// off by up to 6 bf16 ulps on small outputs.  profiles/r2_epilogue_probe.txt: the GELU's ALU work is what slows the tensor
-// pipe in the GEMM1 tiles, 80.7 % -> 62.7 % of peak.)
-__device__ __forceinline__ uint32_t gelu_pair_bf16(float acc0, float acc1, float bias0, float bias1) {
-  const uint64_t x = f2_add(f2_pack(acc0, acc1), f2_pack(bias0, bias1));
-  float x0, x1;
-  f2_unpack(x, x0, x1);
-  const float u0 = __uint_as_float(__float_as_uint(x0) | 0x80000000u);   // -|x|
-  const float u1 = __uint_as_float(__float_as_uint(x1) | 0x80000000u);
-  const uint64_t u = f2_pack(u0, u1);
+// gelu(acc + bias) for two neighbouring columns of the GEMM1 epilogue, returned as a bf16x2 word.  Uses u = -|x| (one OR
+// per value instead of abs) and a degree-5 fit of log2(0.5*erfc(a/sqrt2)) on [0,6] whose leading coefficient is negative,
+// so it needs no clamp (p -> -inf, 2^p -> 0 for large |x|); |gelu error| <= 1.9e-6.
+__device__ __forceinline__ float gelu_fit(float x) {
+  const float u = __uint_as_float(__float_as_uint(x) | 0x80000000u);   // -|x|
   // p(a) with a = -u: odd coefficients change sign
-  uint64_t q = f2_fma(f2_pack(0.00036467931931838393f, 0.00036467931931838393f), u,
-                      f2_pack(0.006363349035382271f, 0.006363349035382271f));
-  q = f2_fma(q, u, f2_pack(0.05013200640678406f, 0.05013200640678406f));
-  q = f2_fma(q, u, f2_pack(-0.4617065489292145f, -0.4617065489292145f));
-  q = f2_fma(q, u, f2_pack(1.150075078010559f, 1.150075078010559f));
-  q = f2_fma(q, u, f2_pack(-1.0001276731491089f, -1.0001276731491089f));
-  float q0, q1;
-  f2_unpack(q, q0, q1);
-  const uint64_t e = f2_pack(ex2_approx(q0), ex2_approx(q1));
-  const uint64_t g = f2_fma(u, e, f2_pack(fmaxf(x0, 0.0f), fmaxf(x1, 0.0f)));   // relu(x) - |x| Phi(-|x|)
-  float g0, g1;
-  f2_unpack(g, g0, g1);
-  return pack_bf16x2(g0, g1);
+  float q = fmaf(0.00036467931931838393f, u, 0.006363349035382271f);
+  q = fmaf(q, u, 0.05013200640678406f);
+  q = fmaf(q, u, -0.4617065489292145f);
+  q = fmaf(q, u, 1.150075078010559f);
+  q = fmaf(q, u, -1.0001276731491089f);
+  return fmaf(u, ex2_approx(q), fmaxf(x, 0.0f));                      // relu(x) - |x| Phi(-|x|)
+}
+__device__ __forceinline__ uint32_t gelu_pair_bf16(float acc0, float acc1, float bias0, float bias1) {
+  return pack_bf16x2(gelu_fit(acc0 + bias0), gelu_fit(acc1 + bias1));
 }
 
 }  // namespace glom

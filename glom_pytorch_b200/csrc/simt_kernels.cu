@@ -62,7 +62,7 @@ cudaError_t launch_pack(int d, int L, int precision, const float* bu_w1, const f
   char* base = static_cast<char*>(packed);
   float* b1p = reinterpret_cast<float*>(base + pl.b1_off);
   float* b2p = reinterpret_cast<float*>(base + pl.b2_off);
-  const int grid = 148 * 8, block = 256;
+  const int grid = sm_count() * 8, block = 256;
   if (precision == 1) {
     pack_weights_kernel<__nv_bfloat16><<<grid, block, 0, st>>>(
         d, L, bu_w1, bu_b1, bu_w2, bu_b2, td_w1, td_b1, td_w2, td_b2,
@@ -152,7 +152,7 @@ cudaError_t launch_prep(const Geometry& g, const float* state_in, const float* i
     if (e != cudaSuccess) return e;
   }
   const size_t n4 = (size_t)g.rows * g.d / 4;
-  cast_bf16_kernel<<<(int)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16), 256, 0, st>>>(n4, tokens, xb);
+  cast_bf16_kernel<<<(int)((n4 + 255) / 256 < sm_count() * 16 ? (n4 + 255) / 256 : sm_count() * 16), 256, 0, st>>>(n4, tokens, xb);
   if (launches) ++*launches;
   return cudaGetLastError();
 }
@@ -171,7 +171,7 @@ cudaError_t launch_broadcast_init(const Geometry& g, const float* state_in, cons
   ProfScope scope(prof, PROF_PREP, st);
   const size_t total4 = (size_t)g.rows * g.L * g.d / 4;
   const size_t want = (total4 + 255) / 256;
-  init_state_kernel<<<(int)(want < 148 * 16 ? want : 148 * 16), 256, 0, st>>>(total4, g.L, g.d, state_in, init_levels,
+  init_state_kernel<<<(int)(want < sm_count() * 16 ? want : sm_count() * 16), 256, 0, st>>>(total4, g.L, g.d, state_in, init_levels,
                                                                                 dst);
   if (launches) ++*launches;
   return cudaGetLastError();
@@ -466,7 +466,7 @@ cudaError_t launch_patchify_bf16(const float* img, const float* w, __nv_bfloat16
                                  int H, int W, int p, int d, int kp, cudaStream_t st, int* launches) {
   const size_t total = ((size_t)B * (H / p) * (W / p) + d) * (kp / 2);
   const size_t want = (total + 255) / 256;
-  patchify_bf16_kernel<<<(int)(want < 148 * 32 ? want : 148 * 32), 256, 0, st>>>(img, w, patches, wtok, B, H, W, p, d, kp);
+  patchify_bf16_kernel<<<(int)(want < sm_count() * 32 ? want : sm_count() * 32), 256, 0, st>>>(img, w, patches, wtok, B, H, W, p, d, kp);
   if (launches) ++*launches;
   return cudaGetLastError();
 }

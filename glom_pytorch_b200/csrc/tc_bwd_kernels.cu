@@ -1,15 +1,14 @@
-// Tensor-core backward of the two grouped MLPs (SURVEY 8 row f2, bf16 engine).
+// Tensor-core backward of the two grouped MLPs.
 //
 // Per reverse step and MLP group g (bottom-up l / top-down l), with x the group's input rows, dY = dL/dS_{t+1}[:, l]/c_l:
 //   P  : pre  = x W1^T + b1 ;  h = gelu(pre), gp = gelu'(pre)  (NT GEMM, K = d) -> bf16, 16 KB blocks like the forward's H
 //   H  : dh   = dY W2 ;  dpre = dh * gp                        (NT GEMM, K = d, B = W2^T)   -> dpre blocks
 //   X  : dx   = dpre W1                          (NT GEMM, K = 4d, B = W1^T)  -> fp32 (R, G, d)
 //   W  : dW2 += dY^T h ;  dW1 += dpre^T x        (TN GEMMs, K = rows; both operands read MN-major by TMA)
-// All four run on CTA pairs (cta_group::2, UMMA 256 x 256 x 16) with the forward's pipeline structure: warp-specialised
-// TMA producer / MMA issuer / epilogue warps, 128B-swizzled smem stages, double-buffered TMEM accumulators, bounded
-// mbarrier waits.  The attention backward, reductions and the scatter of dx stay on CUDA cores (bwd_kernels.cu).
-#include "engine.h"
-#include "ptx.cuh"
+// All four use the forward's pipeline structure (tc_kernels.cu): 256 x 256 tiles dealt to pairs of CTAs that compute 128
+// rows each, a TMA producer warp feeding 128B-swizzled smem stages, two wgmma consumer warpgroups with register
+// accumulators that run the epilogue, bounded mbarrier waits.  The attention backward, reductions and the scatter of dx stay on CUDA cores (bwd_kernels.cu).
+#include "tc_common.cuh"
 
 #include <stdio.h>
 
@@ -17,15 +16,25 @@ namespace glom {
 
 namespace {
 
-constexpr int BM = 128, BK = 64, BN = 256;
+constexpr int BN = 256;
 constexpr uint32_t A_BYTES = BM * BK * 2;          // 16 KB: this CTA's A tile (128 rows or 128 M-columns x 64 k)
-constexpr uint32_t B_BYTES = (BN / 2) * BK * 2;    // 16 KB: this CTA's half of the B tile
+constexpr uint32_t B_BYTES = BN * BK * 2;          // 32 KB: the B tile
 constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int STAGES = 5;
-constexpr int PARTS = 4, PART_COLS = BN / PARTS, EPI_WARPS = 4 * PARTS;
-constexpr int THREADS = 32 * (EPI_WARPS + 4);
+constexpr int STAGES = 3;
+constexpr int CONSUMER_WARPS = 8;
+constexpr int THREADS = 32 * (CONSUMER_WARPS + 1);
 constexpr uint32_t PATCH_BYTES = 4096;
-constexpr size_t SMEM_BYTES = 1024 + (size_t)STAGES * STAGE_BYTES + (size_t)EPI_WARPS * PATCH_BYTES + BN * 4 + 256;
+constexpr size_t SMEM_BYTES = 1024 + (size_t)STAGES * STAGE_BYTES + 4 * (size_t)STG_BYTES + (size_t)CONSUMER_WARPS * PATCH_BYTES +
+                              BN * 4 + 256;
+
+// one k-block for warpgroup `wg`; TA / TB: operand MN-major (64-wide boxes 8 KB apart) instead of K-major
+template <int TA, int TB>
+__device__ __forceinline__ void kblock(float (&acc)[BN / 2], uint32_t a_smem, uint32_t b_smem) {
+  const uint64_t ad = TA ? wgmma_desc_sw128(a_smem, 8192, 1024) : wgmma_desc_sw128(a_smem, 16, 1024);
+  const uint64_t bd = TB ? wgmma_desc_sw128(b_smem, 8192, 1024) : wgmma_desc_sw128(b_smem, 16, 1024);
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) wgmma_bf16<BN, TA, TB>(acc, ad + (TA ? (2048 >> 4) : 2) * k, bd + (TB ? (2048 >> 4) : 2) * k);
+}
 
 enum { BW_PRE = 0, BW_DH = 1, BW_DX = 2, BW_DW = 3, BW_BATCH = 4 };
 
@@ -122,32 +131,23 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
                 const BwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* patches = smem + (size_t)STAGES * STAGE_BYTES;
-  float* bias_s = reinterpret_cast<float*>(patches + (size_t)EPI_WARPS * PATCH_BYTES);
+  float* stg_all = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE_BYTES);
+  uint8_t* patches = reinterpret_cast<uint8_t*>(stg_all) + 4 * STG_BYTES;
+  float* bias_s = reinterpret_cast<float*>(patches + (size_t)CONSUMER_WARPS * PATCH_BYTES);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(bias_s + BN);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int W_TMA = EPI_WARPS, W_MMA = EPI_WARPS + 1, W_ALLOC = EPI_WARPS + 2;
-  const uint32_t cta_rank = cluster_ctarank();
-  const bool leader = cta_rank == 0;
+  constexpr int W_TMA = CONSUMER_WARPS;
+  const int cta_rank = (int)(blockIdx.x & 1);           // the pair's two CTAs own rows [128 r, 128 r + 128) of each tile
   const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
   const int kbg_n = 4 * p.d / BK;                     // 64-column blocks per group in the blocked buffers
 
-  if (warp == W_MMA && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 2 * EPI_WARPS); }
+  if (warp == W_TMA && lane == 0) {
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == W_ALLOC) tmem_alloc_2sm(tmem_slot, 2 * BN);
-  tc_fence_before_sync();
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();
 
@@ -162,25 +162,25 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
         for (int kb = 0; kb < t.num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           if (elected) {
-          uint8_t* sa = smem + (size_t)stage * STAGE_BYTES;
-          uint8_t* sb = sa + A_BYTES;
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * STAGE_BYTES);
-          const uint32_t bar = mapa_shared(smem_u32(&full_bar[stage]), 0);
+          const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
+          const uint32_t sb = sa + A_BYTES;
+          uint64_t* bar = &full_bar[stage];
+          mbar_arrive_expect_tx(bar, STAGE_BYTES);
           if (MODE == BW_PRE || MODE == BW_DH) {
             const int a_row = t.m_blk * 256 + (int)cta_rank * BM;
-            const int b_row = t.g * 4 * p.d + t.n_blk * BN + (int)cta_rank * (BN / 2);
+            const int b_row = t.g * 4 * p.d + t.n_blk * BN;
             if (MODE == BW_PRE) {
               const CUtensorMap* amap = (t.g == 0) ? &map_a0 : ((t.g & 1) ? &map_a2 : &map_a1);
               const int a_col = (t.g == 0) ? 0 : ((t.g & 1) ? l * p.d : (l - 1) * p.d);
-              tma_load_2d_2sm(sa, amap, bar, a_col + kb * BK, a_row);
+              tma_load_2d(sa, amap, bar, a_col + kb * BK, a_row);
             } else {
-              tma_load_2d_2sm(sa, &map_a0, bar, l * p.d + kb * BK, a_row);          // dY = gs[:, l, :]
+              tma_load_2d(sa, &map_a0, bar, l * p.d + kb * BK, a_row);          // dY = gs[:, l, :]
             }
-            tma_load_2d_2sm(sb, &map_b, bar, kb * BK, b_row);
+            for (int i = 0; i < 2; ++i) tma_load_2d(sb + i * 16384, &map_b, bar, kb * BK, b_row + i * (BN / 2));
           } else if (MODE == BW_DX) {
             const int m128 = t.m_blk * 2 + (int)cta_rank;
-            tma_load_2d_2sm(sa, &map_a0, bar, 0, ((t.g * p.m128 + m128) * kbg_n + kb) * BM);    // dpre block (16 KB)
-            tma_load_2d_2sm(sb, &map_b, bar, kb * BK, t.g * p.d + t.n_blk * BN + (int)cta_rank * (BN / 2));
+            tma_load_2d(sa, &map_a0, bar, 0, ((t.g * p.m128 + m128) * kbg_n + kb) * BM);    // dpre block (16 KB)
+            for (int i = 0; i < 2; ++i) tma_load_2d(sb + i * 16384, &map_b, bar, kb * BK, t.g * p.d + t.n_blk * BN + i * (BN / 2));
           } else if (MODE == BW_BATCH) {
             const int z = t.g, bb = z / p.L, lv = z % p.L;
             const bool seg2 = p.k_split && kb >= p.k_split;          // second product of a K-concatenated pair
@@ -191,28 +191,28 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
             const int a_mn = seg2 ? p.a_mn2 : p.a_mn, b_mn = seg2 ? p.b_mn2 : p.b_mn;
             const int a_off = a_st ? lv * p.d : 0, a_bt = a_st ? bb : z;
             const int b_off = b_st ? lv * p.d : 0, b_bt = b_st ? bb : z;
-            const int mrow = t.m_blk * 256 + (int)cta_rank * BM, ncol = t.n_blk * BN + (int)cta_rank * (BN / 2);
-            if (!a_mn) tma_load_3d_2sm(sa, am, bar, a_off + kk * BK, mrow, a_bt);
-            else for (int i = 0; i < 2; ++i) tma_load_3d_2sm(sa + i * 8192, am, bar, a_off + mrow + i * 64, kk * BK, a_bt);
-            if (!b_mn) tma_load_3d_2sm(sb, bm, bar, b_off + kk * BK, ncol, b_bt);
-            else for (int i = 0; i < 2; ++i) tma_load_3d_2sm(sb + i * 8192, bm, bar, b_off + ncol + i * 64, kk * BK, b_bt);
+            const int mrow = t.m_blk * 256 + cta_rank * BM, ncol = t.n_blk * BN;
+            if (!a_mn) tma_load_3d(sa, am, bar, a_off + kk * BK, mrow, a_bt);
+            else for (int i = 0; i < 2; ++i) tma_load_3d(sa + i * 8192, am, bar, a_off + mrow + i * 64, kk * BK, a_bt);
+            if (!b_mn) for (int i = 0; i < 2; ++i) tma_load_3d(sb + i * 16384, bm, bar, b_off + kk * BK, ncol + i * BM, b_bt);
+            else for (int i = 0; i < 4; ++i) tma_load_3d(sb + i * 8192, bm, bar, b_off + ncol + i * 64, kk * BK, b_bt);
           } else {
-            // TN: k runs over rows.  A tile = 64 k-rows x this CTA's 128 M-columns, B tile = 64 k-rows x this CTA's
-            // 128 N-columns, each as two [64 x 64] boxes (MN-major operand: 128-byte rows of 64 consecutive columns).
+            // TN: k runs over rows.  A tile = 64 k-rows x this CTA's 128 M-columns (two [64 x 64] boxes), B tile = 64 k-rows
+            // x 256 N-columns (four boxes); MN-major operands: 128-byte rows of 64 consecutive columns.
             const int r0 = kb * BK;
             const int blk_row = (t.g * p.m128 + (r0 >> 7)) * kbg_n;          // first block of this 128-row band
             const int half = (r0 >> 6) & 1;
-            const int mcol = t.m_blk * 256 + (int)cta_rank * BM;             // first M column of this CTA
-            const int ncol = t.n_blk * BN + (int)cta_rank * (BN / 2);        // first N column of this CTA
-            for (int i = 0; i < 2; ++i) {
+            const int mcol = t.m_blk * 256 + cta_rank * BM;                  // first M column of this CTA
+            const int ncol = t.n_blk * BN;                                    // first N column of the tile
+            for (int i = 0; i < 4; ++i) {
               if (t.kind == 0) {   // dW2_g = dY^T h:  A = gs[:, l, o] (row-major), B = h blocks of group g
-                tma_load_2d_2sm(sa + i * 8192, &map_a0, bar, l * p.d + mcol + i * 64, r0);
-                tma_load_2d_2sm(sb + i * 8192, &map_a2, bar, 0, (blk_row + (ncol >> 6) + i) * BM + half * 64);
+                if (i < 2) tma_load_2d(sa + i * 8192, &map_a0, bar, l * p.d + mcol + i * 64, r0);
+                tma_load_2d(sb + i * 8192, &map_a2, bar, 0, (blk_row + (ncol >> 6) + i) * BM + half * 64);
               } else {             // dW1_g = dpre^T x:  A = dpre blocks of group g, B = x of group g (row-major)
-                tma_load_2d_2sm(sa + i * 8192, &map_a1, bar, 0, (blk_row + (mcol >> 6) + i) * BM + half * 64);
+                if (i < 2) tma_load_2d(sa + i * 8192, &map_a1, bar, 0, (blk_row + (mcol >> 6) + i) * BM + half * 64);
                 const CUtensorMap* bmap = (t.g == 0) ? &map_b : ((t.g & 1) ? &map_b2 : &map_b1);
                 const int b_col = (t.g == 0) ? 0 : ((t.g & 1) ? l * p.d : (l - 1) * p.d);
-                tma_load_2d_2sm(sb + i * 8192, bmap, bar, b_col + ncol + i * 64, r0);
+                tma_load_2d(sb + i * 8192, bmap, bar, b_col + ncol + i * 64, r0);
               }
             }
           }
@@ -222,96 +222,78 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
         }
       }
     }
-  } else if (warp == W_MMA) {
-    if (leader) {
-      const uint32_t elected = elect_one();
-      const uint64_t kdesc0 = umma_desc_sw128(0, 16, 1024), mdesc0 = umma_desc_sw128(0, 8192, 1024);   // K- / MN-major, address 0
-      const int a_mn1 = (MODE == BW_DW) ? 1 : (MODE == BW_BATCH ? p.a_mn : 0);
-      const int b_mn1 = (MODE == BW_DW) ? 1 : (MODE == BW_BATCH ? p.b_mn : 0);
-      const uint32_t idesc1 = umma_idesc_bf16(256, BN, a_mn1, b_mn1);
-      const uint32_t idesc2 = umma_idesc_bf16(256, BN, p.a_mn2, p.b_mn2);      // BW_BATCH with a second product only
-      int stage = 0; uint32_t phase = 0;
-      int as = 0; uint32_t aphase = 0;
-      for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters) {
-        const Tile t = decode<MODE>(p, tile);
-        mbar_wait(&tempty_bar[as], aphase ^ 1);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(as * BN);
-        for (int kb = 0; kb < t.num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after_sync();
-          if (elected) {
-            const uint32_t a_lo = smem_u32(smem + (size_t)stage * STAGE_BYTES) >> 4;
-            const uint32_t b_lo = a_lo + (A_BYTES >> 4);
-            const bool seg2 = MODE == BW_BATCH && p.k_split && kb >= p.k_split;
-            const int a_mn = seg2 ? p.a_mn2 : a_mn1, b_mn = seg2 ? p.b_mn2 : b_mn1;
-            const uint32_t idesc = seg2 ? idesc2 : idesc1;
-            // MN-major: 16 k-rows = 2048 B, the two 64-column blocks are 8192 B apart; K-major: 32 B per 16 k
-            const uint64_t ad = (a_mn ? mdesc0 : kdesc0) + (uint64_t)a_lo, bd = (b_mn ? mdesc0 : kdesc0) + (uint64_t)b_lo;
-            const uint64_t ak = a_mn ? (2048 >> 4) : (32 >> 4), bk = b_mn ? (2048 >> 4) : (32 >> 4);
-            umma_bf16_2sm(d_tmem, ad, bd, idesc, kb != 0 ? 1u : 0u);
-#pragma unroll
-            for (int k = 1; k < BK / 16; ++k) umma_bf16_2sm(d_tmem, ad + ak * k, bd + bk * k, idesc, 1u);
-            umma_commit_2sm(&empty_bar[stage], 3);
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (elected) umma_commit_2sm(&tfull_bar[as], 3);
-        __syncwarp();
-        if (++as == 2) { as = 0; aphase ^= 1; }
-      }
-    }
-  } else if (warp < EPI_WARPS) {
-    const int quad = warp & 3, part = warp >> 2;
+  } else if (warp < W_TMA) {
+    const int wg = warp >> 2, wi = warp & 3;
+    const int quad = warp >> 1, x = warp & 1;     // warp pair = 32-row band `quad` of the CTA's 128 rows; x = 32-column half
+    float* stg = stg_all + quad * (STG_BYTES / 4);
     uint8_t* patch = patches + (size_t)warp * PATCH_BYTES;
     const int c = lane & 7, rsub = lane >> 3;
-    int as = 0; uint32_t aphase = 0;
+    const int a_mn1 = (MODE == BW_DW) ? 1 : (MODE == BW_BATCH ? p.a_mn : 0);
+    const int b_mn1 = (MODE == BW_DW) ? 1 : (MODE == BW_BATCH ? p.b_mn : 0);
+    int stage = 0; uint32_t phase = 0;
+    float frag[BN / 2];
     for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters) {
       const Tile t = decode<MODE>(p, tile);
       if (MODE == BW_PRE) {
-        named_bar_sync(1, EPI_WARPS * 32);
-        for (int i = threadIdx.x; i < BN; i += EPI_WARPS * 32) bias_s[i] = __ldg(p.b1p + (size_t)t.g * 4 * p.d + t.n_blk * BN + i);
-        named_bar_sync(1, EPI_WARPS * 32);
+        named_bar_sync(5, CONSUMER_WARPS * 32);
+        for (int i = threadIdx.x; i < BN; i += CONSUMER_WARPS * 32) bias_s[i] = __ldg(p.b1p + (size_t)t.g * 4 * p.d + t.n_blk * BN + i);
+        named_bar_sync(5, CONSUMER_WARPS * 32);
       }
-      const int row0 = t.m_blk * 256 + (int)cta_rank * BM + quad * 32;      // output row band of this warp
-      // blocked address of this lane's 4 values of row r, chunk c0: block (g, row / 128, col / 64), row % 128, col % 64
-      auto blocked_off = [&](int r, int c0) -> size_t {
-        const int row = row0 + r, col = t.n_blk * BN + part * PART_COLS + c0 + c * 4;
-        return ((size_t)((t.g * p.m128 + (row >> 7)) * kbg_n + (col >> 6)) * BM + (row & 127)) * BK + (col & 63);
-      };
-      // BW_DH: gelu'(pre) of the next 32-column chunk is fetched one chunk ahead (the first one before the accumulator
-      // is even complete), so its L2 / HBM latency is off the epilogue's critical path
-      uint2 gp_next[8];
-      auto fetch_gp = [&](int c0) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int r = i * 4 + rsub;
-          gp_next[i] = row0 + r < p.rows ? __ldg(reinterpret_cast<const uint2*>(p.pre + blocked_off(r, c0))) : make_uint2(0u, 0u);
-        }
-      };
-      if (MODE == BW_DH) fetch_gp(0);
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after_sync();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * BN + part * PART_COLS);
+      for (int i = 0; i < BN / 2; ++i) frag[i] = 0.f;
+      int prev = -1;                    // slot of the k-block whose MMAs may still be running
+      for (int kb = 0; kb < t.num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES) + (uint32_t)wg * 8192u;   // this warpgroup's 64 rows
+        const uint32_t sb = smem_u32(smem + (size_t)stage * STAGE_BYTES) + A_BYTES;
+        const bool seg2 = MODE == BW_BATCH && p.k_split && kb >= p.k_split;
+        const int sel = seg2 ? 2 * p.a_mn2 + p.b_mn2 : 2 * a_mn1 + b_mn1;
+        wgmma_fence_regs(frag);
+        wgmma_fence();
+        if (sel == 0) kblock<0, 0>(frag, sa, sb);
+        else if (sel == 1) kblock<0, 1>(frag, sa, sb);
+        else if (sel == 2) kblock<1, 0>(frag, sa, sb);
+        else kblock<1, 1>(frag, sa, sb);
+        wgmma_commit();
+        wgmma_wait<1>();                  // the previous k-block's MMAs are complete: release its slot
+        wgmma_fence_regs(frag);
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(frag);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      const int row0 = t.m_blk * 256 + cta_rank * BM + quad * 32;      // output row band of this warp pair
 #pragma unroll 1
-      for (int c0 = 0; c0 < PART_COLS; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32(t_addr + c0, v);
-        tmem_ld_wait();
+      for (int part = 0; part < BN / 64; ++part) {
+        const int c0 = 32 * x;
+        // blocked address of this lane's 4 values of row r: block (g, row / 128, col / 64), row % 128, col % 64
+        auto blocked_off = [&](int r) -> size_t {
+          const int row = row0 + r, col = t.n_blk * BN + part * 64 + c0 + c * 4;
+          return ((size_t)((t.g * p.m128 + (row >> 7)) * kbg_n + (col >> 6)) * BM + (row & 127)) * BK + (col & 63);
+        };
+        // BW_DH: gelu'(pre) of this chunk, in flight while the accumulator is staged
         uint2 gp_cur[8];
         if (MODE == BW_DH) {
 #pragma unroll
-          for (int i = 0; i < 8; ++i) gp_cur[i] = gp_next[i];
-          if (c0 + 32 < PART_COLS) fetch_gp(c0 + 32);
+          for (int i = 0; i < 8; ++i) {
+            const int r = i * 4 + rsub;
+            gp_cur[i] = row0 + r < p.rows ? __ldg(reinterpret_cast<const uint2*>(p.pre + blocked_off(r))) : make_uint2(0u, 0u);
+          }
         }
+        stage_write(frag, stg, part, wi, lane);
+        named_bar_sync(1 + quad, 64);
+        uint32_t v[32];
+        stage_read(stg, x, lane, v);
         // accumulator chunk -> patch (f32 rows of 128 B, chunk j of row r at j ^ (r & 7)) -> 4 columns x 8 rows per lane
 #pragma unroll
         for (int j = 0; j < 8; ++j)
           *reinterpret_cast<uint4*>(patch + lane * 128 + ((j ^ (lane & 7)) << 4)) =
               make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
         __syncwarp();
-        const int col = t.n_blk * BN + part * PART_COLS + c0 + c * 4;     // output column of this lane's 4 values
+        const int col = t.n_blk * BN + part * 64 + c0 + c * 4;     // output column of this lane's 4 values
         float colsum[4] = {0.f, 0.f, 0.f, 0.f};                           // BW_DH: first-layer bias gradient partials
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -320,18 +302,18 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
           const int row = row0 + r;
           if (MODE == BW_PRE || MODE == BW_DH) {
             if (row < p.rows) {
-              const size_t off = blocked_off(r, c0);
+              const size_t off = blocked_off(r);
               if (MODE == BW_PRE) {
                 // pre-activation -> h = gelu(pre) and gp = gelu'(pre), both bf16 (the `pre` buffer holds gp)
-                const float4 b4 = *reinterpret_cast<const float4*>(bias_s + part * PART_COLS + c0 + c * 4);
-                const float x[4] = {acc.x + b4.x, acc.y + b4.y, acc.z + b4.z, acc.w + b4.w};
+                const float4 b4 = *reinterpret_cast<const float4*>(bias_s + part * 64 + c0 + c * 4);
+                const float xv[4] = {acc.x + b4.x, acc.y + b4.y, acc.z + b4.z, acc.w + b4.w};
                 float hv[4], gp[4];
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                   float cdf, pdf;
-                  normal_cdf_pdf(x[e], cdf, pdf);
-                  hv[e] = x[e] * cdf;
-                  gp[e] = fmaf(x[e], pdf, cdf);
+                  normal_cdf_pdf(xv[e], cdf, pdf);
+                  hv[e] = xv[e] * cdf;
+                  gp[e] = fmaf(xv[e], pdf, cdf);
                 }
                 *reinterpret_cast<uint2*>(p.h + off) = make_uint2(pack_bf16x2(hv[0], hv[1]), pack_bf16x2(hv[2], hv[3]));
                 *reinterpret_cast<uint2*>(p.pre + off) = make_uint2(pack_bf16x2(gp[0], gp[1]), pack_bf16x2(gp[2], gp[3]));
@@ -396,21 +378,12 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
                           make_float4(colsum[0], colsum[1], colsum[2], colsum[3]));
         }
         __syncwarp();
+        named_bar_sync(1 + quad, 64);                                   // staging tile free for the next step
       }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(mapa_shared(smem_u32(&tempty_bar[as]), 0));
-      if (++as == 2) { as = 0; aphase ^= 1; }
     }
   }
 
-  tc_fence_before_sync();
   __syncthreads();
-  cluster_sync_all();
-  if (warp == W_ALLOC) {
-    tc_fence_after_sync();
-    tmem_dealloc_2sm(tmem_base, 2 * BN);
-  }
 }
 
 bool map2d_box(EncodeTiledFn enc, CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
@@ -431,19 +404,17 @@ cudaError_t launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorM
                    const CUtensorMap& b1, const CUtensorMap& b2, const BwdParams& p, int num_sms, cudaStream_t st) {
   static SmemOptIn optin;
   if (cudaError_t e = optin.ensure(bwd_gemm_kernel<MODE>, SMEM_BYTES)) return e;
-  const int max_clusters = num_sms / 2;
-  const int clusters = p.num_tiles < max_clusters ? p.num_tiles : max_clusters;
+  const int max_pairs = num_sms / 2;
+  const int pairs = p.num_tiles < max_pairs ? p.num_tiles : max_pairs;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * clusters);
+  cfg.gridDim = dim3(2 * pairs);
   cfg.blockDim = dim3(THREADS);
   cfg.dynamicSmemBytes = SMEM_BYTES;
   cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 2;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, bwd_gemm_kernel<MODE>, a0, a1, a2, b0, b1, b2, p);
 }
 

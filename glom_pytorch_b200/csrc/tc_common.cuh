@@ -1,5 +1,5 @@
 // Pieces shared by the tensor-core kernels (tc_kernels.cu: K1 / K2 / K3, mlp_kernel.cu: the merged persistent MLP
-// kernel): tile constants, the K1 / K2 epilogue chunk bodies and the tensor-map helpers.
+// kernel): tile constants, the accumulator hand-off, the K1 / K2 epilogue chunk bodies and the tensor-map helpers.
 #pragma once
 #include "engine.h"
 #include "ptx.cuh"
@@ -8,9 +8,58 @@
 
 namespace glom {
 
-constexpr int BM = 128;            // UMMA M (rows of the state per tile)
+constexpr int BM = 128;            // rows of the state per CTA tile (two warpgroups of wgmma M = 64)
 constexpr int BK = 64;             // bf16 elements per 128-byte swizzle row
 constexpr uint32_t A_STAGE_BYTES = BM * BK * 2;   // 16 KB
+
+// ---- hand-off of a warpgroup's wgmma accumulator to the row-per-thread epilogue chunks
+// Warps 2h and 2h + 1 of a warpgroup hold rows [32 h, 32 h + 32) of its 64 accumulator rows, 16 each.  For the 64-column
+// step s of the tile they write those 32 rows x 64 columns into the pair's staging tile (fp32, row pitch STG_PITCH
+// floats: 16-byte row reads of 8 consecutive rows hit distinct banks); after a pair barrier warp 2h + x reads row `lane`,
+// columns [32 x, 32 x + 32): the 32 x 32 chunk the epilogue functions below take, one row per thread.
+constexpr int STG_PITCH = 68;
+constexpr uint32_t STG_BYTES = 32 * STG_PITCH * 4;    // per warp pair
+template <int S, int R>
+__device__ __forceinline__ void stage_write_step(const float (&acc)[R], float* stg, int warp_in_wg, int lane) {
+  const int r = 16 * (warp_in_wg & 1) + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(stg + (r + 8 * h) * STG_PITCH + 8 * j + c) =
+          make_float2(acc[4 * (8 * S + j) + 2 * h], acc[4 * (8 * S + j) + 2 * h + 1]);
+  }
+}
+// runtime step index, accumulator indices stay compile-time (registers, no local-memory copy)
+template <int R>
+__device__ __forceinline__ void stage_write(const float (&acc)[R], float* stg, int s, int warp_in_wg, int lane) {
+  static_assert(R % 32 == 0 && R <= 128, "m64 x N fragment, N in {64, 128, 256}");
+  if (s == 0) stage_write_step<0>(acc, stg, warp_in_wg, lane);
+  if constexpr (R >= 64) { if (s == 1) stage_write_step<1>(acc, stg, warp_in_wg, lane); }
+  if constexpr (R >= 128) {
+    if (s == 2) stage_write_step<2>(acc, stg, warp_in_wg, lane);
+    if (s == 3) stage_write_step<3>(acc, stg, warp_in_wg, lane);
+  }
+}
+__device__ __forceinline__ void stage_read(const float* stg, int x, int lane, uint32_t (&v)[32]) {
+  const float4* src = reinterpret_cast<const float4*>(stg + lane * STG_PITCH + 32 * x);
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float4 f = src[q];
+    v[4 * q] = __float_as_uint(f.x); v[4 * q + 1] = __float_as_uint(f.y);
+    v[4 * q + 2] = __float_as_uint(f.z); v[4 * q + 3] = __float_as_uint(f.w);
+  }
+}
+
+// One k-block (64 of K) of a 128-row tile for warpgroup `wg`: A rows [64 wg, 64 wg + 64) of the stage's K-major A tile,
+// B = N rows (K-major, TB = 0) or 64 k-rows x N columns in 64-wide boxes 8 KB apart (MN-major, TB = 1).
+template <int N, int TB>
+__device__ __forceinline__ void wgmma_kblock(float (&acc)[N / 2], uint32_t a_smem, uint32_t b_smem) {
+  const uint64_t ad = wgmma_desc_sw128(a_smem, 16, 1024);
+  const uint64_t bd = TB ? wgmma_desc_sw128(b_smem, 8192, 1024) : wgmma_desc_sw128(b_smem, 16, 1024);
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) wgmma_bf16<N, 0, TB>(acc, ad + 2 * k, bd + (TB ? (2048 >> 4) : 2) * k);
+}
 
 // Sum of squares of a 32-column chunk row, in the canonical order shared with prep_state_kernel:
 // 8 lanes hold 4 consecutive columns each (sequential fmaf), then an xor tree over the 8 lanes.
@@ -29,7 +78,7 @@ __device__ __forceinline__ float row_chunk_sumsq(float a, float b, float c, floa
 // through the warp's 2 KB patch (16-byte chunk c of row r stored at chunk c ^ ((r >> 1) & 3)), then 64-byte
 // row segments out (8 rows x 64 B per store instruction).
 // HPOL: 0 = streaming stores (two-kernel step: H is consumed by the NEXT launch, keep it out of L2's way),
-//       1 = L2 evict-last policy `pol` (merged MLP kernel: H is consumed ~10 us later by GEMM2 tiles of the same launch
+//       1 = L2 evict-last policy `pol` (merged MLP kernel: H is consumed a few row blocks later by GEMM2 tiles of the same launch
 //           and must survive the rest of the traffic until then; the consumer's evict-first loads demote it again)
 template <bool FULL, int HPOL = 0>
 __device__ __forceinline__ void k1_chunk(const uint32_t (&v)[32], const float* bias, uint8_t* patch,
@@ -55,7 +104,7 @@ __device__ __forceinline__ void k1_chunk(const uint32_t (&v)[32], const float* b
     const int r = i * 8 + (lane >> 2);
     const uint4 val = *reinterpret_cast<const uint4*>(patch + r * 64 + ((c ^ ((r >> 1) & 3)) << 4));
     // streaming (evict-first) stores: H (369 MB per step) never fits L2, and letting it through the normal policy
-    // evicts the state shadows and weights the GEMMs and the consensus kernel re-read (measured: K1 -4 %)
+    // would evict the state shadows and weights the GEMMs and the consensus kernel re-read
     if (FULL || r < rows_left) {
       if (HPOL == 0) __stcs(reinterpret_cast<uint4*>(hdst + (size_t)r * pitch + c * 8), val);
       else st_global_v4_hint(hdst + (size_t)r * pitch + c * 8, val, pol);

@@ -1,9 +1,9 @@
-"""Data-parallel training plumbing (SURVEY 8e / 8f-2): the only collective the GLOM path ever needs.
+"""Data-parallel training plumbing: the only collective the GLOM path ever needs.
 
 The forward shards along the batch with no exchange step (``sharding.py``).  When a loss is attached
 (README.md:58-90), each rank's backward (``glom_b200_backward``) produces gradients of the replicated parameters for
-its own images; they are averaged over the ranks with a bucketed all-reduce (NCCL over NVLink / NVSwitch on the
-B200 box, gloo in the CPU tests).
+its own images; they are averaged over the ranks with a bucketed all-reduce (NCCL over NVLink / NVSwitch between
+GPUs, gloo in the CPU tests).
 
 Why this is a plain collective and not a kernel fused with the backward: the engine's backward walks the T
 iterations in reverse and ACCUMULATES every weight gradient over all of them (the MLP weights are shared by all

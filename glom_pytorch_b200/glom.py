@@ -1,4 +1,4 @@
-"""Drop-in `Glom` for lucidrains/glom-pytorch whose column-update loop runs on the B200 engine.
+"""Drop-in `Glom` for lucidrains/glom-pytorch whose column-update loop runs on the H100 (sm_90a) engine.
 
 Mirrors the reference's public surface (glom_pytorch/glom_pytorch.py):
   * ``Glom.__init__(*, dim, levels, image_size, patch_size, consensus_self,
@@ -10,9 +10,9 @@ Mirrors the reference's public surface (glom_pytorch/glom_pytorch.py):
     ``iters=0`` returns S_0, output ``(B, n, L, d)`` or ``(T+1, B, n, L, d)`` fp32.
 
 What differs: the loop body (:131-145) plus GroupedFeedForward.forward / ConsensusAttention.forward is
-one call into ``libglom_b200.so`` (C ABI in include/glom_b200.h).  CUDA sm_100 only; there is no CPU / eager
+one call into ``libglom_b200.so`` (C ABI in include/glom_b200.h).  CUDA sm_90a (H100) only; there is no CPU / eager
 fallback -- inputs on other devices raise.  Under autograd the loop is a ``torch.autograd.Function`` whose backward
-is ``glom_b200_backward`` (bf16 engine: the MLP and consensus GEMMs of the reverse pass on tcgen05 tensor cores, the
+is ``glom_b200_backward`` (bf16 engine: the MLP and consensus GEMMs of the reverse pass on wgmma tensor cores, the
 softmax / normalisation / bias reductions in fp32 on CUDA cores; fp32 engine: everything fp32 on CUDA cores): the
 forward keeps S_0..S_T and the reverse pass recomputes each step's intermediates (README.md:58-90 training use).
 The backward is once-differentiable and accumulates with ``red.add`` atomics, so gradients are reproducible only up
@@ -23,7 +23,7 @@ the packed copy is cached and keyed on each parameter's ``(data_ptr, _version)``
 ``.to()`` / ``.cuda()`` / ``.half()``-style ``_apply`` calls and ``invalidate_packed()``.  In-place edits through
 ``param.data`` do not bump ``_version``: call ``invalidate_packed()`` after them in eval mode.
 
-Engine-only knob (keyword-only, additive): ``precision`` = ``"bf16"`` (default; tcgen05 tensor cores,
+Engine-only knob (keyword-only, additive): ``precision`` = ``"bf16"`` (default; wgmma tensor cores,
 bf16 operands, fp32 accumulate and fp32 state -- the arithmetic of the reference under
 ``torch.autocast(dtype=torch.bfloat16)``) or ``"fp32"`` (CUDA-core path matching the reference's fp32
 forward to ~1e-5).
@@ -77,7 +77,7 @@ class GroupedFeedForward(nn.Module):
         )
 
     def forward(self, *_):
-        raise RuntimeError("GroupedFeedForward runs inside the fused B200 column update; call Glom.forward")
+        raise RuntimeError("GroupedFeedForward runs inside the fused column update engine; call Glom.forward")
 
 
 class ConsensusAttention(nn.Module):
@@ -96,7 +96,7 @@ class ConsensusAttention(nn.Module):
             self.register_buffer("non_local_mask", (dist > local_consensus_radius)[None])
 
     def forward(self, *_):
-        raise RuntimeError("ConsensusAttention runs inside the fused B200 column update; call Glom.forward")
+        raise RuntimeError("ConsensusAttention runs inside the fused column update engine; call Glom.forward")
 
     def mask_params(self, n):
         """(mask_side, mask_d2_max) for the engine's analytic mask, derived from the buffer so a
@@ -335,7 +335,7 @@ class Glom(nn.Module):
                                 precision or self.precision)
 
     def tokens(self, img):
-        """image_to_tokens (:114): fp32 CUDA-core kernel (precision fp32) or bf16 gather + tcgen05 GEMM (bf16)."""
+        """image_to_tokens (:114): fp32 CUDA-core kernel (precision fp32) or bf16 gather + wgmma GEMM (bf16)."""
         lin = self.image_to_tokens[1]
         b, c, h, w = img.shape
         p = self.patch_size
@@ -355,7 +355,7 @@ class Glom(nn.Module):
         self._tok_launches = _native.last_launch_count()
         return out
 
-    # ------------------------------------------------------------------ cross-call persistence (SURVEY 8 row f3)
+    # ------------------------------------------------------------------ cross-call persistence
     def stage_tokens(self, img):
         """Video / multi-frame use (README.md:94-112): compute image_to_tokens of the NEXT frame now, on a side stream, so
         that it overlaps the tail of the forward call already enqueued for the current frame.  The following
@@ -395,7 +395,7 @@ class Glom(nn.Module):
         """tokens (B,n,d), pos (n,d), state_in (B,n,L,d) or None, init (L,d): fp32 contiguous CUDA tensors.
         allow_resume (eval, no autograd): when `state_in` IS the tensor the previous call returned, unmodified, and the
         workspace is the same, the engine still holds that state's bf16 shadows / norm partials: the state prologue is
-        skipped (glom_b200_forward_resume, SURVEY 8 row f3)."""
+        skipped (glom_b200_forward_resume)."""
         device = tokens.device
         b, n = tokens.shape[0], tokens.shape[1]
         resume, self._resume = self._resume, None
@@ -435,8 +435,8 @@ class Glom(nn.Module):
     # ------------------------------------------------------------------ the reference's forward (:110)
     def forward(self, img, iters=None, levels=None, return_all=False):
         if not img.is_cuda:
-            raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_100 only (no CPU fallback); "
-                               "move the module and inputs to a B200")
+            raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
+                               "move the module and inputs to an H100")
         b = img.shape[0]
         iters = self.levels * 2 if iters is None else int(iters)             # (:112)
         needs_grad = torch.is_grad_enabled() and (

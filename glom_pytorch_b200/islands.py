@@ -1,4 +1,4 @@
-"""Island analytics on the column states (SURVEY 8 row f4).
+"""Island analytics on the column states.
 
 The reference's README (README.md:34-36) names the use: ``return_all=True`` "gives you access to all the level data
 across iterations for clustering, from which one can inspect for the theorized islands in the paper" -- islands of
@@ -22,7 +22,7 @@ def islands(states, *, grid=None, threshold=0.9):
     (..., L, n) -- ``cos_right``, ``cos_down``, ``agreement`` fp32, ``labels`` int32 (island id = smallest patch index
     of the 4-connected component of neighbour pairs with cosine similarity >= threshold) -- and ``num_islands`` (..., L)."""
     if not states.is_cuda:
-        raise RuntimeError("glom_pytorch_b200.islands runs on CUDA sm_100 only (no CPU fallback)")
+        raise RuntimeError("glom_pytorch_b200.islands runs on CUDA sm_90a (H100) only (no CPU fallback)")
     if states.dim() < 3:
         raise RuntimeError("states must be (..., n, L, d)")
     *lead, n, L, d = states.shape

@@ -1,4 +1,4 @@
-"""Batch-axis partitioning of the column update across ranks (SURVEY 8e): every term of the
+"""Batch-axis partitioning of the column update across ranks: every term of the
 update is per-image, so rank r owns a contiguous slice of images and no collective is needed."""
 
 

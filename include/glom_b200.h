@@ -1,5 +1,5 @@
 /*
- * glom_b200.h -- C ABI of the B200-native GLOM column-update engine (libglom_b200.so).
+ * glom_b200.h -- C ABI of the H100-native (sm_90a) GLOM column-update engine (libglom_b200.so).
  *
  * The reference (lucidrains/glom-pytorch) has no FFI: its hot path is the Python loop
  * glom_pytorch/glom_pytorch.py:131-145 calling GroupedFeedForward (:23-36) and
@@ -39,12 +39,12 @@ typedef enum glom_b200_status {
   GLOM_B200_ERR_INVALID = -1,     /* bad argument / unsupported shape              */
   GLOM_B200_ERR_WORKSPACE = -2,   /* workspace or packed buffer too small          */
   GLOM_B200_ERR_CUDA = -3,        /* a CUDA runtime/driver call failed             */
-  GLOM_B200_ERR_DEVICE = -4       /* device is not sm_100 (no CPU / other-arch fallback) */
+  GLOM_B200_ERR_DEVICE = -4       /* device is not compute capability 9.x, sm_90a (no CPU / other-arch fallback) */
 } glom_b200_status;
 
 typedef enum glom_b200_precision {
   GLOM_B200_FP32 = 0,  /* CUDA-core fp32 path: matches the reference's fp32 forward     */
-  GLOM_B200_BF16 = 1   /* tcgen05 path: bf16 operands, fp32 accumulate, fp32 state --
+  GLOM_B200_BF16 = 1   /* wgmma tensor-core path: bf16 operands, fp32 accumulate, fp32 state --
                           the arithmetic of the reference under torch.autocast(bf16)     */
 } glom_b200_precision;
 
@@ -106,7 +106,7 @@ GLOM_B200_API int glom_b200_forward(const glom_b200_cfg* cfg, const void* packed
                       const float* init_levels, float* state_out, int batch, int iters,
                       int return_all, void* workspace, size_t workspace_bytes, void* stream);
 
-/* Cross-call persistence (SURVEY 8 row f3, README.md:94-112: levels carried from frame to frame).  Same as
+/* Cross-call persistence.  Same as
  * glom_b200_forward with a carried-in state, for the case that `state_in` is bit for bit the FINAL state the previous
  * glom_b200_forward / _forward_resume call on this workspace wrote (same cfg, batch, and `pos`): the workspace then still
  * holds that state's bf16 shadows and norm partials in shadow buffer `shadow_parity` (0 after a plain forward with an even
@@ -119,12 +119,12 @@ GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void*
                                            int return_all, void* workspace, size_t workspace_bytes, void* stream,
                                            int shadow_parity, int* out_shadow_parity);
 
-/* Tokeniser, the step before the loop (SURVEY 8f-1): replaces image_to_tokens
+/* Tokeniser, the step before the loop: replaces image_to_tokens
  * (glom_pytorch.py:94-97, call :114): patchify 'b c (h p1) (w p2) -> b (h w) (p1 p2 c)'
  * fused with the Linear(3*p*p -> d).
  *   img (B, 3, H, W) fp32;  weight (d, 3*p*p) fp32;  bias (d) fp32;  tokens (B, n, d) fp32
  * precision GLOM_B200_FP32: one CUDA-core fp32 kernel, no workspace.
- * precision GLOM_B200_BF16: gather + cast to a zero-padded bf16 operand, then a tcgen05 GEMM with
+ * precision GLOM_B200_BF16: gather + cast to a zero-padded bf16 operand, then a wgmma GEMM with
  *   fp32 accumulation (what autocast does to this Linear); needs the workspace below, 1024-aligned. */
 GLOM_B200_API int glom_b200_tokenize_workspace_bytes(int batch, int height, int width, int patch,
                                                      int dim, int precision, size_t* out_bytes);
@@ -145,10 +145,10 @@ GLOM_B200_API int glom_b200_last_launch_count(void);
 GLOM_B200_API int glom_b200_workspace_offset(const glom_b200_cfg* cfg, int batch, int iters, int return_all,
                                int which, size_t* out_offset, size_t* out_bytes);
 
-/* Backward of the column update (SURVEY 8 row f2): gradients of glom_b200_forward's loop
+/* Backward of the column update: gradients of glom_b200_forward's loop
  * (glom_pytorch.py:123-148) with respect to tokens, pos, the initial state (or init_levels) and the
  * eight MLP tensors, given dL/d(output).  Per-step intermediates are recomputed from the saved states.  precision
- * GLOM_B200_BF16 with dim % 256 == 0: the MLP and consensus GEMMs of the reverse pass run on tcgen05 tensor cores (bf16
+ * GLOM_B200_BF16 with dim % 256 == 0: the MLP and consensus GEMMs of the reverse pass run on wgmma tensor cores (bf16
  * operands, fp32 accumulation), softmax / normalisation / bias reductions in fp32 on CUDA cores; otherwise everything
  * is fp32 on CUDA cores.  All d_* buffers are ACCUMULATED into (zero them first); weights and their
  * gradients use the reference's state_dict layout.
@@ -190,9 +190,7 @@ GLOM_B200_API int glom_b200_tokenize_backward(const float* img, const float* wei
 GLOM_B200_API int glom_b200_profile_begin(void);
 GLOM_B200_API int glom_b200_profile_end(double* ms_by_kind, int* launches_by_kind, int kinds);
 
-/* Island analytics on column states (SURVEY 8 row f4; the consumer of return_all the reference's README.md:34-36
- * describes: "all the level data across iterations for clustering, from which one can inspect for the theorized
- * islands").  states: `slabs` contiguous (side_h * side_w, levels, dim) fp32 state slabs, e.g. the (iters+1) * B slabs of
+/* Island analytics on column states.  states: `slabs` contiguous (side_h * side_w, levels, dim) fp32 state slabs, e.g. the (iters+1) * B slabs of
  * glom_b200_forward(return_all = 1).  Per (slab, level), on the patch grid (patch i = h * side_w + w):
  *   cos_right / cos_down (slabs, levels, n)  cosine similarity with the right / lower neighbour (0 where there is none)
  *   agreement            (slabs, levels, n)  mean cosine similarity with the existing 4-neighbours
@@ -219,13 +217,14 @@ GLOM_B200_API int glom_b200_mlp_schedule(const glom_b200_cfg* cfg, int batch, in
 GLOM_B200_API int glom_b200_clock_probe(uint64_t* out_cycles_ns, int spin_us, void* stream);
 
 /* Measurement aid (bench.py): the SM clock the tensor-core kernels ACTUALLY ran at.  One thread of block 0 of every
- * tcgen05 kernel brackets the kernel's working phase with (clock64, %globaltimer); the deltas accumulate per kernel kind
+ * tensor-core kernel brackets the kernel's working phase with (clock64, %globaltimer); the deltas accumulate per kernel kind
  * (indices as in glom_b200_profile_end: 0 consensus, 1 GEMM1+GELU, 2 GEMM2+combine, 4 tokeniser GEMM, 5 merged MLP kernel).
  * Writes MHz (cycles per microsecond of in-kernel time) and the in-kernel milliseconds per kind since the last reset;
  * kinds without samples report 0.  wait_frac (may be NULL, else 6 doubles per kind): fractions of block 0's in-kernel
- * cycles that {the MMA lane waited for operands, the MMA lane waited for a free accumulator stage (consensus: TMEM buffer
- * or P), the TMA lane waited for a free ring slot, epilogue / softmax warp 0 waited for an accumulator, that warp was
- * busy (consensus: softmax work), consensus only: its output work}; filled by the diagnostic instantiations only
+ * cycles in slots {0: GEMMs: consumer warp 0 waited for operands, 1: unused (0), 2: the TMA lane waited for a free ring
+ * slot, 3: consensus: consumer warp 0 waited for operands, 4: GEMMs: consumer warp 0's epilogue work; consensus: its
+ * softmax work, 5: consensus: its output work}; the accumulators live in the consumers' registers, so there is no
+ * accumulator wait.  Filled by the diagnostic instantiations only
  * (environment variable GLOM_B200_WAIT_COUNTERS=1).
  * Synchronises the device; `reset` != 0 clears the accumulators. */
 GLOM_B200_API int glom_b200_kernel_clocks(double* mhz_by_kind, double* ms_by_kind, double* wait_frac, int kinds, int reset);

@@ -18,14 +18,14 @@ What it restates (all citations relative to the reference checkout,
 * ``glom_forward``    <- Glom.forward (:110-150): S_0 (:123-124), contributions 4..4,3
                          (:128-129), the Jacobi loop (:131-145), return_all (:147-148).
 
-Parity pinning: the reference ships NO tests or golden vectors (SURVEY.md section 4), so
+Parity pinning: the reference ships NO tests or golden vectors, so
 this oracle is pinned against outputs of the live reference itself: the fixtures in
 ``tests/golden/*.npz`` were produced by ``tests/golden/make_golden.py`` importing
 ``/root/reference`` in the build container; ``tests/test_oracle_golden.py`` checks
 this file against every one of them (fp64 oracle vs fp32 reference <= 2e-5 max-abs).
 
 Arithmetic is numpy; ``dtype`` selects float32/float64.  ``emulate='bf16'`` rounds the
-tensor-core operands to bfloat16 (round-to-nearest-even) exactly where the B200 engine
+tensor-core operands to bfloat16 (round-to-nearest-even) exactly where the bf16 engine
 does, to give a tight prediction of the engine's own output for diagnostics.
 """
 from __future__ import annotations
@@ -83,7 +83,7 @@ def gelu_erf(x: np.ndarray) -> np.ndarray:
 
 def synth_params(dim, levels, image_size, patch_size, seed=0, dtype=np.float32):
     """Deterministic synthetic parameters with the reference's shapes and default-init
-    scales (SURVEY.md 3.4), keyed exactly like ``Glom.state_dict()`` (SURVEY.md section 0).
+    scales (SURVEY.md 3.4), keyed exactly like ``Glom.state_dict()``.
     Uses numpy's PCG64 so fixtures do not depend on torch's RNG stream."""
     rng = np.random.default_rng(seed)
     L, d = levels, dim

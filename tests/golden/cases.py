@@ -3,12 +3,12 @@ the reference) and the tests (any box; no reference needed).  numpy PCG64 only."
 import numpy as np
 
 CASES = {
-    # BASELINE.json configs[0]: dim=64 levels=3 image_size=28 patch_size=7 iters=2 batch=1 fp32
+    # configs[0]: dim=64 levels=3 image_size=28 patch_size=7 iters=2 batch=1 fp32
     "c1_return_all": dict(dim=64, levels=3, image_size=28, patch_size=7, batch=1, iters=2,
                           return_all=True),
     "c1_default_iters": dict(dim=64, levels=3, image_size=28, patch_size=7, batch=2,
                              iters=None, return_all=False),
-    # mid case (SURVEY 7.1): d=128 L=4 N=64
+    # mid case: d=128 L=4 N=64
     "mid_return_all": dict(dim=128, levels=4, image_size=32, patch_size=4, batch=2, iters=5,
                            return_all=True),
     "mid_consensus_self": dict(dim=128, levels=4, image_size=32, patch_size=4, batch=2,
@@ -20,10 +20,10 @@ CASES = {
     # peaky attention: carried-in state scaled x20 (softmax far from uniform)
     "mid_peaky": dict(dim=128, levels=4, image_size=32, patch_size=4, batch=2, iters=3,
                       return_all=True, levels_scale=20.0),
-    # non-square image, n < num_patches (SURVEY 8b): 16x32 with patch 4 -> n = 32 of 64
+    # non-square image, n < num_patches: 16x32 with patch 4 -> n = 32 of 64
     "mid_nonsquare": dict(dim=128, levels=4, image_size=32, patch_size=4, batch=2, iters=3,
                           return_all=False, img_hw=(16, 32)),
-    # 3-frame continuation (README.md:105-111; BASELINE config 5 shape, small dims)
+    # 3-frame continuation (README.md:105-111; configs[4] shape, small dims)
     "mid_continuation": dict(dim=128, levels=4, image_size=32, patch_size=4, batch=2,
                              iters=[4, 3, 2], return_all=False, frames=3),
     # two levels (smallest legal L: top_down has L-1 = 1 group)
@@ -50,7 +50,7 @@ def inputs(case, frame=0):
 
 # ----------------------------------------------------------------------------- gradient fixtures (f2)
 GRAD_CASES = {
-    # BASELINE configs[0] shapes, default attention (diag fill), init_levels start, loss on every time step
+    # configs[0] shapes, default attention (diag fill), init_levels start, loss on every time step
     "grad_c1_all": dict(dim=64, levels=3, image_size=28, patch_size=7, batch=2, iters=2, return_all=True,
                         param_seed=11),
     # carried-in levels (gradient w.r.t. the input state), radius mask + consensus_self, loss on the last step only

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: `pytest -m gpu`).  Everything goes through the C ABI
+"""GPU parity tests (run on an H100: `pytest -m gpu`).  Everything goes through the C ABI
 (glom_pytorch_b200._native -> libglom_b200.so).  /root/reference does not exist on the box: the
 checkers are the committed golden vectors (outputs of the live reference) and the CPU oracle.
 
@@ -6,8 +6,7 @@ Tolerances
   fp32 engine vs reference fp32 golden : max-abs <= 1e-4 * max(1, |ref|max)   (summation order only)
   bf16 engine vs reference fp32 golden : per time step rel-Frobenius <= 1e-2 and
                                          max-abs <= 3e-2 * max(1, |ref|max)
-      (SURVEY 8c: anchored on the reference's own autocast-bf16-vs-fp32 gap of 1.7e-3..3.8e-3 rel-Fro,
-       6.3e-3 max-abs, with 2-3x head-room as hard caps)
+     
   bf16 engine vs bf16-emulating oracle : rel-Frobenius <= 2e-3 (same roundings, different sum order)
 """
 import os
@@ -160,7 +159,7 @@ def test_native_tokenizer_matches_oracle():
 
 
 def test_tensor_core_tokenizer_matches_oracle():
-    """bf16 precision: patchify + cast + tcgen05 GEMM vs the bf16-operand oracle (and the exact one)."""
+    """bf16 precision: patchify + cast + wgmma GEMM vs the bf16-operand oracle (and the exact one)."""
     for name in ("mid_nonsquare", "c1_return_all"):
         case, params, _ = load(name)
         m = make_model(case, params, "bf16")
@@ -194,7 +193,7 @@ EDGE = [
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 @pytest.mark.parametrize("spec", EDGE, ids=[f"d{e[0]}_L{e[1]}_hw{e[4][0]}x{e[4][1]}_p{e[3]}" for e in EDGE])
 def test_shape_edge_cases_against_oracle(spec, precision):
-    """Ragged / extreme shapes the reference accepts (SURVEY 8b): checked against the fp64 CPU oracle."""
+    """Ragged / extreme shapes the reference accepts: checked against the fp64 CPU oracle."""
     dim, L, isz, p, hw, B, T, kw = spec
     params = O.synth_params(dim, L, isz, p, seed=3)
     m = G.Glom(dim=dim, levels=L, image_size=isz, patch_size=p, precision=precision, **kw)
@@ -268,7 +267,7 @@ def test_large_magnitude_state_takes_the_exact_maximum_softmax(consensus_self):
 
 
 def test_cached_workspaces_side_streams_and_cuda_graph_replay_are_bit_stable():
-    """Cross-call persistence (SURVEY 8 f3): packed weights and workspaces are cached per module; interleaving two
+    """Cross-call persistence: packed weights and workspaces are cached per module; interleaving two
     models, changing the batch size, running on a side stream and replaying a captured CUDA graph of `forward`
     (the library never allocates or synchronises) must all reproduce the first results bit for bit."""
     torch.manual_seed(0)
@@ -313,7 +312,7 @@ def full_model(precision, seed=0, **kw):
 
 
 def test_config2_dims_against_cpu_oracle():
-    """BASELINE configs[1] dims (d=512 L=6 N=256), B=2, 3 iterations: engine vs the fp32 CPU oracle."""
+    """configs[1] dims (d=512 L=6 N=256), B=2, 3 iterations: engine vs the fp32 CPU oracle."""
     m = full_model("bf16")
     g = torch.Generator().manual_seed(1)
     img = torch.randn(2, 3, 224, 224, generator=g)
@@ -332,7 +331,7 @@ def _oracle_params(m):
 
 
 def test_config2_dims_all_12_iterations_against_cpu_oracle():
-    """BASELINE configs[1] dims and iteration count (d=512 L=6 N=256, iters=12), B=2, return_all: every one of the 12
+    """configs[1] dims and iteration count (d=512 L=6 N=256, iters=12), B=2, return_all: every one of the 12
     time steps of the bf16 engine against the fp32 CPU oracle (existing bf16 tolerance per step)."""
     m = full_model("bf16")
     img = torch.randn(2, 3, 224, 224, generator=torch.Generator().manual_seed(11))
@@ -344,7 +343,7 @@ def test_config2_dims_all_12_iterations_against_cpu_oracle():
 
 
 def test_config5_chain_12_10_6_against_cpu_oracle():
-    """BASELINE configs[4] (README.md:105-111): three frames, iters 12 -> 10 -> 6 with the state carried, d=512 L=6
+    """configs[4] (README.md:105-111): three frames, iters 12 -> 10 -> 6 with the state carried, d=512 L=6
     N=256, B=2: 28 chained iterations.  The engine carries ITS OWN state between the calls, the oracle its own; every
     time step of every call is compared (drift over the whole chain stays inside the per-step bf16 tolerance)."""
     m = full_model("bf16")
@@ -361,7 +360,7 @@ def test_config5_chain_12_10_6_against_cpu_oracle():
 
 
 def test_config4_dims_against_cpu_oracle():
-    """BASELINE configs[3] dims (d=1024 L=8 384/16 -> N=576, the lean consensus variant), B=1, 3 iterations, against the
+    """configs[3] dims (d=1024 L=8 384/16 -> N=576, the lean consensus variant), B=1, 3 iterations, against the
     fp32 CPU oracle (not the engine's own fp32 path)."""
     torch.manual_seed(0)
     kw = dict(dim=1024, levels=8, image_size=384, patch_size=16)
@@ -475,7 +474,7 @@ def test_hidden_of_mlp_group_0_is_reused_across_the_steps_of_a_call(monkeypatch)
 
 
 def test_resumed_chain_and_staged_tokens_are_bit_identical_to_the_plain_calls():
-    """SURVEY 8 row f3 (README.md:94-112, three frames, levels carried).  Passing the very tensor the previous call
+    """(README.md:94-112, three frames, levels carried).  Passing the very tensor the previous call
     returned lets the engine resume from the bf16 shadows / norm partials it still holds (no state prologue), and
     `stage_tokens` computes the next frame's tokens on a side stream; both must give bit-identical states to plain calls
     on cloned inputs (which take the ordinary prologue), for even and odd step counts, and a modified carried tensor must
@@ -549,7 +548,7 @@ def test_clock_probe_reports_a_plausible_sm_clock():
 
 
 def test_config2_full_size_properties():
-    """Size-independent properties at BASELINE configs[1] (B=32, iters=12):
+    """Size-independent properties at configs[1] (B=32, iters=12):
     (1) continuation additivity 12 == 6 + 6 bit-exactly (README.md:105-111);
     (2) batch independence: images 3..5 run alone give bit-identical columns;
     (3) bf16 tensor-core path vs fp32 CUDA-core path of the same engine: rel-Fro <= 1e-2;
@@ -573,7 +572,7 @@ def test_config2_full_size_properties():
 
 
 def test_config4_dims_small_batch():
-    """BASELINE configs[3] dims (d=1024 L=8 384/16 -> N=576): bf16 engine vs its own fp32 path, B=1."""
+    """configs[3] dims (d=1024 L=8 384/16 -> N=576): bf16 engine vs its own fp32 path, B=1."""
     torch.manual_seed(0)
     kw = dict(dim=1024, levels=8, image_size=384, patch_size=16)
     m = G.Glom(**kw, precision="bf16").to(DEV).eval()
@@ -624,7 +623,7 @@ def test_errors_are_reported_not_swallowed():
         m(torch.randn(1, 3, 56, 56, device=DEV))
 
 
-# ----------------------------------------------------------------------------- backward (SURVEY 8 f2)
+# ----------------------------------------------------------------------------- backward
 from cases import GRAD_CASES, grad_inputs  # noqa: E402
 
 
@@ -690,7 +689,7 @@ def test_readme_denoising_training_step_runs():
 @pytest.mark.parametrize("spec", [(256, 3, 32, 4, 3, 3), (512, 6, 224, 14, 2, 3)],
                          ids=["d256_L3_n64_rows192", "config2_dims_B2"])
 def test_tensor_core_backward_matches_fp32_backward(spec):
-    """bf16 engine (dim % 256 == 0): the MLP GEMMs of the backward run on tcgen05.  Checked against the engine's own fp32
+    """bf16 engine (dim % 256 == 0): the MLP GEMMs of the backward run on tensor cores (wgmma).  Checked against the engine's own fp32
     CUDA-core backward (itself pinned on the reference's autograd above): rel-Frobenius <= 3e-2 per gradient tensor."""
     dim, L, isz, p, B, T = spec
     torch.manual_seed(4)

@@ -190,7 +190,7 @@ def _dp_worker(rank, world, port, q):
 
 
 def test_data_parallel_gradient_allreduce_two_ranks_gloo():
-    """SURVEY 8e / 8f-2: the only collective of the path -- bucketed gradient averaging over the ranks (NCCL on the
+    """the only collective of the path -- bucketed gradient averaging over the ranks (NCCL on the
     box, gloo here), incl. a parameter that has no gradient on one rank, and the setup-time parameter broadcast."""
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")

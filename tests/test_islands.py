@@ -1,4 +1,4 @@
-"""Island analytics (SURVEY 8 row f4): the numpy oracle on constructed cases (CPU), and the CUDA kernels
+"""Island analytics: the numpy oracle on constructed cases (CPU), and the CUDA kernels
 (glom_b200_islands through the C ABI) against the oracle (GPU)."""
 import numpy as np
 import pytest

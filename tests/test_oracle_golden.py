@@ -71,7 +71,7 @@ def test_bf16_round_is_rne():
 
 
 def test_continuation_additivity():
-    """2+2 iterations with the state carried == 4 iterations (SURVEY section 0 [measured])."""
+    """2+2 iterations with the state carried == 4 iterations."""
     case, params, _ = load("mid_return_all")
     img, _ = inputs(case)
     kw = dict(patch_size=case["patch_size"], image_size=case["image_size"])

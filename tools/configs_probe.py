@@ -1,4 +1,4 @@
-"""Device-time the other BASELINE configs on one GPU (informative; bench.py's line is configs[1])."""
+"""Device-time the other configs on one GPU (informative; bench.py's line is configs[1])."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import glom_pytorch_b200 as G

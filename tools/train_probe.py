@@ -1,4 +1,4 @@
-"""Training-step timing at BASELINE configs[1] shapes (forward on tensor cores + fp32 CUDA-core backward)."""
+"""Training-step timing at configs[1] shapes (forward on tensor cores + fp32 CUDA-core backward)."""
 import os, sys, time
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
