@@ -165,6 +165,13 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t adesc, ui
   else wgmma_n64<TA, TB>(d, adesc, bdesc);
 }
 
+// Per-warpgroup register reallocation (every thread of the warpgroup executes it): `dec` returns registers to the
+// CTA's pool, `inc` blocks until the pool can grant the new count.  ptxas allocates the code after it within N.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -225,6 +232,16 @@ __device__ __forceinline__ void tma_load_2d_hint(uint32_t dst_smem, const CUtens
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint "
       "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst_smem),
       "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
+      : "memory");
+}
+// same box multicast to every CTA of the cluster in `cta_mask`: it lands at offset `dst_smem` of each of them and is
+// accounted on the mbarrier at `bar`'s offset in each
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst_smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster "
+      "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst_smem),
+      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(uint32_t dst_smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {

@@ -134,8 +134,11 @@ __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b
   const int c = lane & 7, rsub = lane >> 3;
   const bool top = (k.l == k.L - 1);                  // 3 contributions on the top level, 4 elsewhere (:128-129)
   const bool has_td = (k.l >= 1);
-  const size_t ld = (size_t)k.L * k.d;
+  // row offsets r * ld and r * ldp (r < 32) in 32 bits: the compiler hoists them out of the caller's column loop, and
+  // as 64-bit values they would cost twice the registers
+  const int ld = k.L * k.d, ldp = (k.L - 1) * k.d;
   const size_t base = ((size_t)k.row0 * k.L + k.l) * k.d + col + c * 4;
+  const size_t pbase = ((size_t)k.row0 * (k.L - 1) + (k.l - 1)) * k.d + col + c * 4;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     // global loads of four rows first (independent, all in flight), then combine + store
@@ -147,8 +150,8 @@ __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b
       sv[j] = make_float4(0.f, 0.f, 0.f, 0.f); pp[j] = sv[j]; cw[j] = make_uint2(0u, 0u);
       if (FULL || r < rows_left) {
         sv[j] = k.s_bcast ? __ldg(reinterpret_cast<const float4*>(k.s32_in + (size_t)k.l * k.d + col + c * 4))
-                          : __ldcs(reinterpret_cast<const float4*>(k.s32_in + base + (size_t)r * ld));
-        cw[j] = __ldcs(reinterpret_cast<const uint2*>(k.c_in + base + (size_t)r * ld));
+                          : __ldcs(reinterpret_cast<const float4*>(k.s32_in + base + (unsigned)(r * ld)));
+        cw[j] = __ldcs(reinterpret_cast<const uint2*>(k.c_in + base + (unsigned)(r * ld)));
         if (has_td) {
           int pr = k.prow0 + r;                       // (row0 + r) % n without a division per row (r < 32)
           if (k.n >= 32) { if (pr >= k.n) pr -= k.n; } else pr %= k.n;
@@ -168,11 +171,11 @@ __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b
       if (top) { o0 = o0 / 3.0f; o1 = o1 / 3.0f; o2 = o2 / 3.0f; o3 = o3 / 3.0f; }          // (:142) IEEE division
       else { o0 *= 0.25f; o1 *= 0.25f; o2 *= 0.25f; o3 *= 0.25f; }                          // x/4 == x*0.25 exactly
       if (FULL || r < rows_left) {
-        const size_t o = base + (size_t)r * ld;
+        const size_t o = base + (unsigned)(r * ld);
         __stcs(reinterpret_cast<float4*>(k.s32_out + o), make_float4(o0, o1, o2, o3));
         *reinterpret_cast<uint2*>(k.sb_out + o) = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));
         if (has_td)
-          *reinterpret_cast<uint2*>(k.sp_out + ((size_t)(k.row0 + r) * (k.L - 1) + (k.l - 1)) * k.d + col + c * 4) =
+          *reinterpret_cast<uint2*>(k.sp_out + pbase + (unsigned)(r * ldp)) =
               make_uint2(pack_bf16x2(o0 + pp[j].x, o1 + pp[j].y), pack_bf16x2(o2 + pp[j].z, o3 + pp[j].w));
       } else {
         o0 = o1 = o2 = o3 = 0.f;

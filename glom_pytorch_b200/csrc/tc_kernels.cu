@@ -19,19 +19,25 @@ namespace glom {
 
 // =====================================================================================
 // K1 / K2: persistent grouped GEMM, fused epilogues
-//   The schedule deals 256 x BN output tiles to "pairs" of CTAs; CTA 2c + r of pair c owns rows [128 r, 128 r + 128) of
-//   each tile of pair c and computes them on its own.  One TMA producer warp fills a ring of (A 128 x 64, B BN x 64)
-//   stages; two consumer warpgroups each run wgmma m64 x BN x 16 on 64 of the rows with the accumulator in registers.
+//   The schedule deals 256 x BN output tiles to pairs of CTAs, launched as two-CTA clusters; CTA 2c + r of pair c owns
+//   rows [128 r, 128 r + 128) of each tile of pair c.  Both CTAs need the same B (weight) k-blocks in the same order, so
+//   each loads one BN/2-row half and multicasts it to both.  Warpgroup 0 is the producer: its first warp fills a ring of
+//   (A 128 x 64, B BN x 64) stages, and the warpgroup gives up registers (setmaxnreg) to the two consumer warpgroups,
+//   which each run wgmma m64 x BN x 16 on 64 of the rows with the accumulator in registers.
 //   After the tile's K loop the accumulator goes, 64 columns at a time, through per-warp-pair staging tiles into
 //   row-per-thread 32 x 32 chunks, and each chunk through a private transpose patch so that every global load / store
 //   instruction covers whole cache lines (the reference's 4-way combine / residual write, glom_pytorch.py:141-142).
 // =====================================================================================
 constexpr int GEMM_CONSUMER_WARPS = 8;
-constexpr int GEMM_THREADS = 32 * (GEMM_CONSUMER_WARPS + 1);
+constexpr int GEMM_THREADS = 128 + 32 * GEMM_CONSUMER_WARPS;
+// 40 x 128 + 232 x 256 = 64,512 of the SM's 65,536 registers: the 64 x 256 fp32 accumulator (128 registers) and the
+// epilogue fit the consumers without spilling
+constexpr uint32_t GEMM_PRODUCER_REGS = 40;
+constexpr uint32_t GEMM_CONSUMER_REGS = 232;
 
 // in-kernel clock samples (see clock_sample_begin): [kind][cycles, ns], kinds = ProfKind
-// + wait-cycle counters of block 0: [2] consumer warp 0 waiting for operands, [4] TMA lane waiting for a free ring slot,
-// [6] consumer warp 0 busy in the epilogue ([3] and [5] stay 0: the accumulator lives in the consumers' registers)
+// + wait-cycle counters of block 0: [2] first consumer warp waiting for operands, [4] TMA lane waiting for a free ring
+// slot, [6] first consumer warp busy in the epilogue ([3] and [5] stay 0: the accumulator lives in the consumers' registers)
 __device__ unsigned long long g_kernel_clk[PROF_KINDS][8];
 
 
@@ -163,10 +169,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(xch + 4 * 32);
   uint64_t* empty_bar = full_bar + STAGES;
 
-  // consumer warps first (ids 0-7: warpgroups 0 and 1), the TMA producer warp last
+  // warpgroup 0 = producer (its warp 0 issues the TMA loads), warpgroups 1 and 2 = consumers
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  constexpr int W_TMA = GEMM_CONSUMER_WARPS;
+  constexpr int W_TMA = 0;
+  constexpr int W_CONSUMER0 = 4;
   const int cta_rank = (int)(blockIdx.x & 1);
   const int cluster_id = blockIdx.x >> 1;
   const int num_clusters = gridDim.x >> 1;
@@ -175,108 +182,120 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
     tma_prefetch_desc(&map_a0);
     tma_prefetch_desc(&map_b);
     if (MODE == 0) { tma_prefetch_desc(&map_a1); tma_prefetch_desc(&map_a2); }
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], GEMM_CONSUMER_WARPS); }
+    // a slot is free once the consumers of BOTH CTAs are done with it: the peer's producer writes half of its B tile
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2 * GEMM_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  __syncthreads();
+  cluster_sync_all();          // both CTAs' barriers initialised before any multicast load or remote arrive
   pdl_launch_dependents();     // the next kernel may start its own set-up on SMs we vacate
   pdl_wait();                  // ... and we touch global memory only after the previous kernel has finished
   const bool clk_thread = blockIdx.x == 0 && warp == W_TMA && lane == 0;
-  ClockSample clk_s{};
-  if (clk_thread) clk_s = clock_sample_begin();
+  // the sample's start waits in shared memory: held in a register it would be live across the consumers' code
+  ClockSample* clk_s = reinterpret_cast<ClockSample*>(empty_bar + STAGES);
+  if (clk_thread) *clk_s = clock_sample_begin();
   const bool cnt_cta = CNT && blockIdx.x == 0;          // wait-cycle counters (diagnostic instantiation): block 0 only
   unsigned long long* const cnt = g_kernel_clk[MODE == 0 ? PROF_GEMM1 : MODE == 1 ? PROF_GEMM2 : PROF_TOKENIZE];
   unsigned long long w0 = 0, w1 = 0;
 #define GLOM_CNT_WAIT(acc, stmt) do { if (cnt_cta) { const long long t_ = clock64(); stmt; acc += (unsigned long long)(clock64() - t_); } else { stmt; } } while (0)
 
-  if (warp == W_TMA) {
-    // ------------------------------------------------------------------ TMA producer
-    // warp-converged: all lanes walk the schedule and poll the barriers, the elected lane issues (see elect_one)
-    const uint32_t elected = elect_one();
-    int stage = 0; uint32_t phase = 0;
-    const uint32_t smem0 = smem_u32(smem);
-    const uint64_t pol_first = l2_policy_evict_first();
-    const int kbg_n = 4 * p.d / BK;
-    const int blk_skip = (p.m128 - 1) * kbg_n;
-    // K2: H comes from HBM (written by the previous launch) and the ring is consumed in order.  A cursor running
-    // h_prefetch k-blocks ahead of the loads (across tile boundaries) can pull the 16 KB blocks into L2 first.
-    int pf_it = 0, pf_kb = 0, pf_nkb = 0, pf_blk0 = 0;
-    bool pf_valid = false;
-    auto pf_tile = [&](int it_) {
-      pf_it = it_; pf_kb = 0;
-      const int tl = sched_tile<MODE>(p, cluster_id, num_clusters, it_);
-      pf_valid = tl >= 0;
-      if (pf_valid) {
-        const TileInfo tt = decode_tile<MODE>(p, tl);
-        pf_nkb = tt.num_kb;
-        pf_blk0 = (2 * tt.z * p.m128 + ((tt.m_blk * 256 + cta_rank * BM) >> 7)) * kbg_n;
-      }
-    };
-    auto pf_step = [&]() {
-      if (!pf_valid) return;
-      const int blk = pf_blk0 + pf_kb + (pf_kb >= kbg_n ? blk_skip : 0);
-      if (elected) tma_prefetch_2d(&map_a0, 0, blk * BM);
-      if (++pf_kb == pf_nkb) pf_tile(pf_it + 1);
-    };
-    for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
-      const TileInfo t = decode_tile<MODE>(p, tile);
-      const CUtensorMap* amap;
-      int a_col, b_row;
-      if (MODE == 0) {
-        const int l = t.z >> 1;
-        if (t.z == 0) { amap = &map_a0; a_col = 0; }                        // bottom-up level 0 reads the tokens (:132)
-        else if (t.z & 1) { amap = &map_a2; a_col = l * p.d; }              // top-down l reads S[l+1]+pos (:136)
-        else { amap = &map_a1; a_col = (l - 1) * p.d; }                     // bottom-up l reads S[l-1]   (:134)
-        b_row = t.z * 4 * p.d + t.n_blk * BN;
-      } else if (MODE == 1) {
-        amap = &map_a0; a_col = 0;             // H is stored as contiguous 16 KB (128 x 64) blocks, see below
-        b_row = t.z * p.d + t.n_blk * BN;
-      } else {
-        amap = &map_a0; a_col = 0;               // patches (rows, Kp) x Wtok (d, Kp)
-        b_row = t.n_blk * BN;
-      }
-      const int a_row = t.m_blk * 256 + cta_rank * BM;
-      // K2: block (group g, 128-row block, 64-wide k block); [H_bu,l | H_td,l] are groups 2l and 2l+1, so k block kb
-      // of the concatenation is block blk0 + kb of group 2l and, from kb = kbg_n on, of the group behind it
-      const int blk0 = (2 * t.z * p.m128 + (a_row >> 7)) * kbg_n;
-      if (MODE == 1 && it == 0 && p.h_prefetch > 0) {            // prime the prefetch cursor
-        pf_tile(0);
-        for (int i = 0; i < p.h_prefetch; ++i) pf_step();
-      }
-      for (int kb = 0; kb < t.num_kb; ++kb) {
-        if (MODE == 1 && p.h_prefetch > 0) pf_step();
-        GLOM_CNT_WAIT(w0, mbar_wait(&empty_bar[stage], phase ^ 1));
-        if (elected) {
-          const uint32_t sa = smem0 + (uint32_t)stage * Cfg::STAGE_BYTES;
-          uint64_t* bar = &full_bar[stage];
-          mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
-          if (MODE == 1) {
-            const int blk = blk0 + kb + (kb >= kbg_n ? blk_skip : 0);
-            // H streams through once per pair of column tiles: evict-first keeps it from displacing weights / state
-            // (h_load_policy, diagnostics: 1 = only the row block's last column tile marks it evict-first, 2 = no hint)
-            if (p.h_load_policy == 0 || (p.h_load_policy == 1 && t.n_blk == p.num_n - 1)) tma_load_2d_hint(sa, amap, bar, 0, blk * BM, pol_first);
-            else tma_load_2d(sa, amap, bar, 0, blk * BM);
-          } else {
-            tma_load_2d(sa, amap, bar, a_col + kb * BK, a_row);
-          }
-          // the B tile as two boxes of BN/2 rows
-          tma_load_2d(sa + A_STAGE_BYTES, &map_b, bar, kb * BK, b_row);
-          tma_load_2d(sa + A_STAGE_BYTES + (BN / 2) * BK * 2, &map_b, bar, kb * BK, b_row + BN / 2);
+  if (warp < W_CONSUMER0) {
+    setmaxnreg_dec<GEMM_PRODUCER_REGS>();
+    if (warp == W_TMA) {
+      // ------------------------------------------------------------------ TMA producer
+      // warp-converged: all lanes walk the schedule and poll the barriers, the elected lane issues (see elect_one)
+      const uint32_t elected = elect_one();
+      int stage = 0; uint32_t phase = 0;
+      const uint32_t smem0 = smem_u32(smem);
+      const uint64_t pol_first = l2_policy_evict_first();
+      const int kbg_n = 4 * p.d / BK;
+      const int blk_skip = (p.m128 - 1) * kbg_n;
+      // K2: H comes from HBM (written by the previous launch) and the ring is consumed in order.  A cursor running
+      // h_prefetch k-blocks ahead of the loads (across tile boundaries) can pull the 16 KB blocks into L2 first.
+      int pf_it = 0, pf_kb = 0, pf_nkb = 0, pf_blk0 = 0;
+      bool pf_valid = false;
+      auto pf_tile = [&](int it_) {
+        pf_it = it_; pf_kb = 0;
+        const int tl = sched_tile<MODE>(p, cluster_id, num_clusters, it_);
+        pf_valid = tl >= 0;
+        if (pf_valid) {
+          const TileInfo tt = decode_tile<MODE>(p, tl);
+          pf_nkb = tt.num_kb;
+          pf_blk0 = (2 * tt.z * p.m128 + ((tt.m_blk * 256 + cta_rank * BM) >> 7)) * kbg_n;
         }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      };
+      auto pf_step = [&]() {
+        if (!pf_valid) return;
+        const int blk = pf_blk0 + pf_kb + (pf_kb >= kbg_n ? blk_skip : 0);
+        if (elected) tma_prefetch_2d(&map_a0, 0, blk * BM);
+        if (++pf_kb == pf_nkb) pf_tile(pf_it + 1);
+      };
+      for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
+        const TileInfo t = decode_tile<MODE>(p, tile);
+        const CUtensorMap* amap;
+        int a_col, b_row;
+        if (MODE == 0) {
+          const int l = t.z >> 1;
+          if (t.z == 0) { amap = &map_a0; a_col = 0; }                        // bottom-up level 0 reads the tokens (:132)
+          else if (t.z & 1) { amap = &map_a2; a_col = l * p.d; }              // top-down l reads S[l+1]+pos (:136)
+          else { amap = &map_a1; a_col = (l - 1) * p.d; }                     // bottom-up l reads S[l-1]   (:134)
+          b_row = t.z * 4 * p.d + t.n_blk * BN;
+        } else if (MODE == 1) {
+          amap = &map_a0; a_col = 0;             // H is stored as contiguous 16 KB (128 x 64) blocks, see below
+          b_row = t.z * p.d + t.n_blk * BN;
+        } else {
+          amap = &map_a0; a_col = 0;               // patches (rows, Kp) x Wtok (d, Kp)
+          b_row = t.n_blk * BN;
+        }
+        const int a_row = t.m_blk * 256 + cta_rank * BM;
+        // K2: block (group g, 128-row block, 64-wide k block); [H_bu,l | H_td,l] are groups 2l and 2l+1, so k block kb
+        // of the concatenation is block blk0 + kb of group 2l and, from kb = kbg_n on, of the group behind it
+        const int blk0 = (2 * t.z * p.m128 + (a_row >> 7)) * kbg_n;
+        if (MODE == 1 && it == 0 && p.h_prefetch > 0) {            // prime the prefetch cursor
+          pf_tile(0);
+          for (int i = 0; i < p.h_prefetch; ++i) pf_step();
+        }
+        for (int kb = 0; kb < t.num_kb; ++kb) {
+          if (MODE == 1 && p.h_prefetch > 0) pf_step();
+          GLOM_CNT_WAIT(w0, mbar_wait(&empty_bar[stage], phase ^ 1));
+          if (elected) {
+            const uint32_t sa = smem0 + (uint32_t)stage * Cfg::STAGE_BYTES;
+            uint64_t* bar = &full_bar[stage];
+            mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
+            if (MODE == 1) {
+              const int blk = blk0 + kb + (kb >= kbg_n ? blk_skip : 0);
+              // H streams through once per pair of column tiles: evict-first keeps it from displacing weights / state
+              // (h_load_policy, diagnostics: 1 = only the row block's last column tile marks it evict-first, 2 = no hint)
+              if (p.h_load_policy == 0 || (p.h_load_policy == 1 && t.n_blk == p.num_n - 1)) tma_load_2d_hint(sa, amap, bar, 0, blk * BM, pol_first);
+              else tma_load_2d(sa, amap, bar, 0, blk * BM);
+            } else {
+              tma_load_2d(sa, amap, bar, a_col + kb * BK, a_row);
+            }
+            // the B tile is the same in both CTAs of the pair: each loads one box of BN/2 rows and multicasts it to both
+            const uint32_t b_half = (uint32_t)cta_rank * (BN / 2);
+            tma_load_2d_multicast(sa + A_STAGE_BYTES + b_half * BK * 2, &map_b, bar, kb * BK, b_row + (int)b_half, 0x3);
+          }
+          __syncwarp();
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
       }
+      if (cnt_cta && elected) atomicAdd(&cnt[4], w0);
     }
-    if (cnt_cta && elected) atomicAdd(&cnt[4], w0);
-  } else if (warp < W_TMA) {
+  } else {
     // ------------------------------------------------------------------ consumers: wgmma main loop + epilogue
-    const int wg = warp >> 2, wi = warp & 3;
-    const int pair = warp >> 1, x = warp & 1;  // warp pair = 32-row band `pair` of the CTA's 128 rows; x = its 32-column half
+    setmaxnreg_inc<GEMM_CONSUMER_REGS>();
+    const int cw = warp - W_CONSUMER0;       // consumer warp 0-7
+    const int wg = cw >> 2, wi = cw & 3;
+    const int pair = cw >> 1, x = cw & 1;    // warp pair = 32-row band `pair` of the CTA's 128 rows; x = its 32-column half
     float* stg = stg_all + pair * (STG_BYTES / 4);
-    uint8_t* patch = patches + (size_t)warp * Cfg::PATCH_BYTES;
+    uint8_t* patch = patches + (size_t)cw * Cfg::PATCH_BYTES;
     float* xch_p = xch + pair * 32;
     const uint32_t smem0 = smem_u32(smem);
     const uint64_t pol_keep = l2_policy_evict_normal();
+    const uint32_t empty_peer = mapa_shared(smem_u32(empty_bar), (uint32_t)cta_rank ^ 1u);
+    auto release = [&](int slot) {     // this warp is done reading `slot`: free it for both CTAs' producers
+      __syncwarp();
+      if (lane == 0) { mbar_arrive(&empty_bar[slot]); mbar_arrive_cluster(empty_peer + 8u * (uint32_t)slot); }
+    };
     int stage = 0; uint32_t phase = 0;
     float acc[BN / 2];
     for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
@@ -305,14 +324,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
         wgmma_commit();
         wgmma_wait<1>();                  // the previous k-block's MMAs are complete: release its slot
         wgmma_fence_regs(acc);
-        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+        if (prev >= 0) release(prev);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      release(prev);
       const long long busy_t0 = cnt_cta ? clock64() : 0;
 #pragma unroll 1
       for (int s = 0; s < BN / 64; ++s) {
@@ -364,11 +382,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
             writer = x == 0;
           }
           if (writer && (lane & 7) == 0) {
+            float* nsq = p.nsq_out + ((size_t)row0 * p.L + t.z) * p.nparts + t.n_blk * Cfg::PARTS + part;
+            const int ldn = p.L * p.nparts;   // row offsets r * ldn (r < 32) in 32 bits: half the registers once hoisted
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               const int r = i * 4 + (lane >> 3);
-              if (r < rows_left)
-                p.nsq_out[((size_t)(row0 + r) * p.L + t.z) * p.nparts + t.n_blk * Cfg::PARTS + part] = rowsq[i];
+              if (r < rows_left) nsq[(unsigned)(r * ldn)] = rowsq[i];
             }
           }
         }
@@ -376,12 +395,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
       }
       if (cnt_cta) w1 += (unsigned long long)(clock64() - busy_t0);
     }
-    if (cnt_cta && warp == 0 && lane == 0) { atomicAdd(&cnt[2], w0); atomicAdd(&cnt[6], w1); }
+    if (cnt_cta && cw == 0 && lane == 0) { atomicAdd(&cnt[2], w0); atomicAdd(&cnt[6], w1); }
   }
 #undef GLOM_CNT_WAIT
 
-  __syncthreads();
-  if (clk_thread) clock_sample_end(clk_s, g_kernel_clk[MODE == 0 ? PROF_GEMM1 : MODE == 1 ? PROF_GEMM2 : PROF_TOKENIZE]);
+  cluster_sync_all();          // no CTA exits while its peer can still multicast into it or arrive on its barriers
+  if (clk_thread) clock_sample_end(*clk_s, g_kernel_clk[MODE == 0 ? PROF_GEMM1 : MODE == 1 ? PROF_GEMM2 : PROF_TOKENIZE]);
 }
 
 // =====================================================================================
@@ -809,17 +828,29 @@ static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1
   using Cfg = GemmCfg<MODE, BN>;
   static SmemOptIn optin;
   if (cudaError_t e = optin.ensure(gemm_kernel<MODE, BN, CNT>, Cfg::SMEM_BYTES)) return e;
-  const int max_pairs = num_sms / 2;
-  const int pairs = p.num_tiles < max_pairs ? p.num_tiles : max_pairs;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pairs);
   cfg.blockDim = dim3(Cfg::THREADS);
   cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernel
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
+  attr[1].id = cudaLaunchAttributeClusterDimension;                     // the pair shares its B tiles (multicast)
+  attr[1].val.clusterDim.x = 2; attr[1].val.clusterDim.y = 1; attr[1].val.clusterDim.z = 1;
+  // Both CTAs of a cluster need an SM of the same GPC, so fewer than num_sms / 2 pairs may be co-resident; a grid beyond
+  // that would run its last clusters as a second wave.
+  static int max_pairs = 0;
+  if (max_pairs == 0) {
+    cfg.gridDim = dim3(2 * (num_sms / 2));
+    cfg.attrs = &attr[1]; cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaError_t e = cudaOccupancyMaxActiveClusters(&n, gemm_kernel<MODE, BN, CNT>, &cfg)) return e;
+    if (n < 1) return cudaErrorInvalidConfiguration;
+    max_pairs = n < num_sms / 2 ? n : num_sms / 2;
+  }
+  cfg.attrs = attr; cfg.numAttrs = 2;
+  const int pairs = p.num_tiles < max_pairs ? p.num_tiles : max_pairs;
+  cfg.gridDim = dim3(2 * pairs);
   return cudaLaunchKernelEx(&cfg, gemm_kernel<MODE, BN, CNT>, a0, a1, a2, bm, p);
 }
 
