@@ -255,6 +255,28 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst_smem, const CUtensorMap
 __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* m, int c0, int c1) {
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(m), "r"(c0), "r"(c1) : "memory");
 }
+// TMA store of a box from this CTA's shared memory (laid out as the map's swizzle expects) to global memory, with an L2
+// cache policy.  Completion is tracked per issuing thread in bulk groups: bulk_commit_group closes the group of the
+// stores issued since the last commit; bulk_wait_group_read<N> waits until at most N groups may still read their shared
+// memory source, bulk_wait_group<N> until at most N groups are incomplete (their writes done).
+__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap* m, uint32_t src_smem, int c0, int c1, uint64_t policy) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;" ::"l"(m),
+               "r"(src_smem), "r"(c0), "r"(c1), "l"(policy)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// Four 8 x 8 b16 matrices from registers to shared memory (warp-wide).  Lanes 8i .. 8i + 7 give the addresses of the 8
+// 16-byte rows of matrix i; register i of lane t holds row t / 4, columns 2 (t % 4) and 2 (t % 4) + 1 of matrix i, which
+// is the layout of a bf16x2-packed pair of wgmma accumulator elements (see wgmma_n64).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));

@@ -24,9 +24,11 @@ namespace glom {
 //   each loads one BN/2-row half and multicasts it to both.  Warpgroup 0 is the producer: its first warp fills a ring of
 //   (A 128 x 64, B BN x 64) stages, and the warpgroup gives up registers (setmaxnreg) to the two consumer warpgroups,
 //   which each run wgmma m64 x BN x 16 on 64 of the rows with the accumulator in registers.
-//   After the tile's K loop the accumulator goes, 64 columns at a time, through per-warp-pair staging tiles into
-//   row-per-thread 32 x 32 chunks, and each chunk through a private transpose patch so that every global load / store
-//   instruction covers whole cache lines (the reference's 4-way combine / residual write, glom_pytorch.py:141-142).
+//   After the tile's K loop, K1 applies bias + GELU on the accumulator fragment itself and stores H through per-warpgroup
+//   swizzled output tiles with TMA.  K2 and the tokeniser hand the accumulator, 64 columns at a time, through
+//   per-warp-pair staging tiles into row-per-thread 32 x 32 chunks, and each chunk through a private transpose patch so
+//   that every global load / store instruction covers whole cache lines (the reference's 4-way combine / residual
+//   write, glom_pytorch.py:141-142).
 // =====================================================================================
 constexpr int GEMM_CONSUMER_WARPS = 8;
 constexpr int GEMM_THREADS = 128 + 32 * GEMM_CONSUMER_WARPS;
@@ -48,8 +50,6 @@ struct GemmParams {
   int z0;                            // first MLP group (K1) / level (K2) of this launch, see level batching below
   int n_half;                        // K2: number of half-cost (top-level) tiles in this launch
   const float* bias;
-  // K1
-  __nv_bfloat16* h_out;
   // K2
   const float* s32_in;
   int s_bcast;                       // s32_in = init_levels broadcast (see K2Chunk)
@@ -65,7 +65,7 @@ struct GemmParams {
   int tok_kb;      // K blocks of 64 of the zero-padded patch dimension
   int h_prefetch;  // K2: k-blocks of H prefetched into L2 ahead of the TMA loads (0 = off)
   int z_rev;        // K1: groups walked from G - 1 down to z0 (see step_bf16)
-  int h_keep_z;     // K1: H blocks of groups <= h_keep_z are stored with the default L2 policy instead of streaming stores
+  int h_keep_z;     // K1: H blocks of groups <= h_keep_z are stored with the default L2 policy instead of evict-first
   int h_load_policy; // K2: L2 hint of the H loads (GLOM_B200_K2_HPOL, default 0 = evict-first on every load)
   int epi_prefetch; // K2: L2 prefetch of the epilogue's state / consensus lines at tile start (GLOM_B200_K2_EPI_PREFETCH, default on)
 };
@@ -78,11 +78,18 @@ struct GemmCfg {
   static constexpr int THREADS = GEMM_THREADS;
   static constexpr uint32_t B_STAGE_BYTES = BN * BK * 2;
   static constexpr uint32_t STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 3 : (BN == 128) ? 4 : 5;   // ring + staging + patches within 227 KB
-  static constexpr uint32_t PATCH_BYTES = (MODE == 0) ? 2048 : 4096; // per-warp 32x32 transpose patch (bf16 | f32)
   static_assert(MODE >= 0 && MODE <= 2, "0 = GEMM1+GELU, 1 = GEMM2+combine, 2 = tokeniser");
-  static constexpr size_t SMEM_BYTES = 1024 /*align slack*/ + (size_t)STAGES * STAGE_BYTES + 4 * (size_t)STG_BYTES +
-                                       (size_t)GEMM_CONSUMER_WARPS * PATCH_BYTES + 4 * 32 * 4 + 256;
+  // ring + epilogue buffers within 227 KB
+  static constexpr int STAGES = (BN == 256) ? 3 : (BN == 128) ? 4 : 5;
+  // K1 (MODE 0): a 64-row x BN-column bf16 output tile per consumer warpgroup, BN / 64 TMA boxes of 64 x 64, written
+  // from the accumulator fragment and stored to H by TMA.  K2 / tokeniser: per-pair staging tiles, per-warp 32 x 32 f32
+  // transpose patches and the squared-norm exchange of the warp pairs.
+  static constexpr uint32_t OUT_BOX_BYTES = 64 * BK * 2;
+  static constexpr uint32_t PATCH_BYTES = 4096;
+  static constexpr size_t EPI_BYTES = (MODE == 0) ? 2 * (BN / 64) * (size_t)OUT_BOX_BYTES
+                                                  : 4 * (size_t)STG_BYTES + (size_t)GEMM_CONSUMER_WARPS * PATCH_BYTES + 4 * 32 * 4;
+  static constexpr size_t SMEM_BYTES = 1024 /*align slack*/ + (size_t)STAGES * STAGE_BYTES + EPI_BYTES + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 232448, "over the 227 KB of shared memory a block may opt in to");
 };
 
 struct TileInfo {
@@ -156,6 +163,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
             const __grid_constant__ CUtensorMap map_a1,   // K1: state shadow Sb (rows, L*d)
             const __grid_constant__ CUtensorMap map_a2,   // K1: Sb[:,1:]+pos shadow Sp (rows, (L-1)*d)
             const __grid_constant__ CUtensorMap map_b,    // K1: W1p (G*4d, d)              K2: W2p (L*d, 8d)   box BN/2 rows
+            const __grid_constant__ CUtensorMap map_out,  // K1: H, box 64 x 64 (the TMA stores)   K2 / tokeniser: unused
             const GemmParams p) {
   using Cfg = GemmCfg<MODE, BN>;
   constexpr int STAGES = Cfg::STAGES;
@@ -163,10 +171,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
   // 1024-byte alignment (128-byte swizzle atoms) by pointer arithmetic on the __shared__ array (keeps the shared address
   // space visible to the compiler: LDS/STS instead of generic LD/ST for every staging / patch access)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* stg_all = reinterpret_cast<float*>(smem + (size_t)STAGES * Cfg::STAGE_BYTES);
-  uint8_t* patches = reinterpret_cast<uint8_t*>(stg_all) + 4 * STG_BYTES;
+  uint8_t* epi = smem + (size_t)STAGES * Cfg::STAGE_BYTES;      // K1: output tiles; K2 / tokeniser: staging, patches, exchange
+  float* stg_all = reinterpret_cast<float*>(epi);
+  uint8_t* patches = epi + 4 * STG_BYTES;
   float* xch = reinterpret_cast<float*>(patches + (size_t)GEMM_CONSUMER_WARPS * Cfg::PATCH_BYTES);   // [4 pairs][32]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(xch + 4 * 32);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi + Cfg::EPI_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   // warpgroup 0 = producer (its warp 0 issues the TMA loads), warpgroups 1 and 2 = consumers
@@ -181,7 +190,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
   if (warp == W_TMA && lane == 0) {
     tma_prefetch_desc(&map_a0);
     tma_prefetch_desc(&map_b);
-    if (MODE == 0) { tma_prefetch_desc(&map_a1); tma_prefetch_desc(&map_a2); }
+    if (MODE == 0) { tma_prefetch_desc(&map_a1); tma_prefetch_desc(&map_a2); tma_prefetch_desc(&map_out); }
     // a slot is free once the consumers of BOTH CTAs are done with it: the peer's producer writes half of its B tile
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2 * GEMM_CONSUMER_WARPS); }
     fence_barrier_init();
@@ -291,6 +300,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
     float* xch_p = xch + pair * 32;
     const uint32_t smem0 = smem_u32(smem);
     const uint64_t pol_keep = l2_policy_evict_normal();
+    const uint64_t pol_stream = l2_policy_evict_first();
+    // K1: the thread that issues the warpgroup's TMA stores (bulk groups are tracked per thread) and the lane's part of the
+    // stmatrix addresses: lanes 8i .. 8i + 7 address the rows of matrix i = (column group j & 1, row half h)
+    const bool st_issuer = (threadIdx.x & 127) == 0;
+    const uint32_t out_wg = smem_u32(epi) + (uint32_t)wg * (BN / 64) * Cfg::OUT_BOX_BYTES;
+    const uint32_t st_row = (uint32_t)(16 * wi + 8 * ((lane >> 3) & 1) + (lane & 7)) * 128;
+    const int st_jx = lane >> 4, st_sw = lane & 7;     // tile row r of this lane: r & 7 == st_sw
     const uint32_t empty_peer = mapa_shared(smem_u32(empty_bar), (uint32_t)cta_rank ^ 1u);
     auto release = [&](int slot) {     // this warp is done reading `slot`: free it for both CTAs' producers
       __syncwarp();
@@ -332,70 +348,108 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
       wgmma_fence_regs(acc);
       release(prev);
       const long long busy_t0 = cnt_cta ? clock64() : 0;
-#pragma unroll 1
-      for (int s = 0; s < BN / 64; ++s) {
-        stage_write(acc, stg, s, wi, lane);
-        named_bar_sync(1 + pair, 64);
-        uint32_t v[32];
-        stage_read(stg, x, lane, v);
-        const int cc = 64 * s + 32 * x;                               // column of this chunk inside the tile
-        if (MODE == 0) {
-          // H block (group, 128-row block, k block = this 64-column step): 16 KB contiguous, row pitch 64
-          const int hblk = (t.z * p.m128 + (t.m_blk * 2 + cta_rank)) * (4 * p.d / BK) + t.n_blk * (BN / BK) + s;
-          __nv_bfloat16* hrow = p.h_out + ((size_t)hblk * BM + pair * 32) * BK + 32 * x;
-          const float* bias = p.bias + (size_t)t.z * 4 * p.d + t.n_blk * BN + cc;
-          if (t.z <= p.h_keep_z) {       // read first by the GEMM2 launch that follows: keep it in L2 if it fits
-            if (rows_left >= 32) k1_chunk<true, 1>(v, bias, patch, hrow, (size_t)BK, lane, 32, pol_keep);
-            else k1_chunk<false, 1>(v, bias, patch, hrow, (size_t)BK, lane, rows_left, pol_keep);
-          } else if (rows_left >= 32) k1_chunk<true>(v, bias, patch, hrow, (size_t)BK, lane, 32);
-          else k1_chunk<false>(v, bias, patch, hrow, (size_t)BK, lane, rows_left);
-        } else if (MODE == 2) {
-          float* trow = p.tok_out + (size_t)row0 * p.d + t.n_blk * BN + cc;
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + t.n_blk * BN + cc + (lane & 7) * 4));
-          tok_chunk(v, b4, patch, trow, (size_t)p.d, lane, rows_left);
-        } else {
-          K2Chunk kc;
-          kc.l = t.z; kc.L = p.L; kc.d = p.d; kc.n = p.n; kc.row0 = row0; kc.prow0 = row0 % p.n; kc.s_bcast = p.s_bcast;
-          kc.s32_in = p.s32_in; kc.c_in = p.c_in; kc.pos = p.pos;
-          kc.s32_out = p.s32_out; kc.sb_out = p.sb_out; kc.sp_out = p.sp_out;
-          const int col = t.n_blk * BN + cc;
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + (size_t)t.z * p.d + col + (lane & 7) * 4));
-          float rowsq[8];
+      if constexpr (MODE == 0) {
+        // K1 epilogue on the accumulator fragment: bias + GELU per column pair, bf16x2 words into the warpgroup's output
+        // tile by stmatrix, then one TMA store per 64-column box s into H block (group, 128-row block, k block s of the
+        // tile): 16 KB contiguous, row pitch 64.  Each box is 64 x 64 in the 128-byte swizzle (16-byte chunk c of row r at
+        // c ^ (r & 7)).  The stores drain during the next tile's main loop, so one tile per warpgroup suffices.
+        // Whole 64-row boxes are stored, so in the last, padded 128-row block the rows past p.rows receive gelu(b1) (their
+        // A rows are zero-filled by the TMA loads).  Only GEMM2 rows >= p.rows read them, and k2_chunk discards those
+        // results and zeroes their squared-norm contribution.  A box that starts at or past p.rows is not stored: it may
+        // lie in a 128-row block H does not have.
+        const int wrow0 = t.m_blk * 256 + cta_rank * BM + 64 * wg;     // first row of this warpgroup's 64
+        if (wrow0 < p.rows) {                                           // warpgroup-uniform
+          const int hblk0 = (t.z * p.m128 + (t.m_blk * 2 + cta_rank)) * (4 * p.d / BK) + t.n_blk * (BN / BK);
+          const float* bias = p.bias + (size_t)t.z * 4 * p.d + t.n_blk * BN + 2 * (lane & 3);
+          // groups read first by the GEMM2 launch that follows keep the default policy (stay in L2 if they fit)
+          const uint64_t pol = t.z <= p.h_keep_z ? pol_keep : pol_stream;
+          // all of the tile's GELU work first, with no barrier in between: pk[16 s + 2 j + h] holds columns
+          // 64 s + 8 j + 2 (lane & 3) + {0, 1} of row half h
+          uint32_t pk[BN / 4];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) rowsq[i] = 0.f;
-          if (rows_left >= 32) k2_chunk<true>(v, b4, patch, kc, col, lane, 32, rowsq);
-          else k2_chunk<false>(v, b4, patch, kc, col, lane, rows_left, rowsq);
-          // one squared-norm partial per PART_COLS columns: with 64-column parts the two warps of the pair hold the two
-          // 32-column halves, summed in chunk order (0 + first) + second as in prep_state_kernel
-          int part = cc / Cfg::PART_COLS;
-          bool writer = true;
-          if (Cfg::PART_COLS == 64) {
-            if (x == 1 && (lane & 7) == 0) {
+          for (int s = 0; s < BN / 64; ++s) {
 #pragma unroll
-              for (int i = 0; i < 8; ++i) xch_p[i * 4 + (lane >> 3)] = rowsq[i];
+            for (int j = 0; j < 8; ++j) {
+              const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 64 * s + 8 * j));
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                pk[16 * s + 2 * j + h] = gelu_pair_bf16(acc[4 * (8 * s + j) + 2 * h], acc[4 * (8 * s + j) + 2 * h + 1], b.x, b.y);
             }
-            named_bar_sync(1 + pair, 64);
-            if (x == 0) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) rowsq[i] += xch_p[i * 4 + (lane >> 3)];
-            }
-            writer = x == 0;
           }
-          if (writer && (lane & 7) == 0) {
-            float* nsq = p.nsq_out + ((size_t)row0 * p.L + t.z) * p.nparts + t.n_blk * Cfg::PARTS + part;
-            const int ldn = p.L * p.nparts;   // row offsets r * ldn (r < 32) in 32 bits: half the registers once hoisted
+          if (st_issuer) bulk_wait_group_read<0>();       // the previous tile's stores have read the output tile
+          named_bar_sync(1 + wg, 128);
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int r = i * 4 + (lane >> 3);
-              if (r < rows_left) nsq[(unsigned)(r * ldn)] = rowsq[i];
-            }
+          for (int s = 0; s < BN / 64; ++s)
+#pragma unroll
+            for (int q = 0; q < 4; ++q)                   // column groups 2q, 2q + 1 of box s
+              stmatrix_x4(out_wg + (uint32_t)s * Cfg::OUT_BOX_BYTES + st_row + ((uint32_t)((2 * q + st_jx) ^ st_sw) << 4),
+                          pk[16 * s + 4 * q], pk[16 * s + 4 * q + 1], pk[16 * s + 4 * q + 2], pk[16 * s + 4 * q + 3]);
+          fence_proxy_async_smem();                       // the tile -> visible to the TMA stores
+          named_bar_sync(1 + wg, 128);
+          if (st_issuer) {
+#pragma unroll
+            for (int s = 0; s < BN / 64; ++s)
+              tma_store_2d_hint(&map_out, out_wg + (uint32_t)s * Cfg::OUT_BOX_BYTES, 0, (hblk0 + s) * BM + 64 * wg, pol);
+            bulk_commit_group();
           }
         }
-        named_bar_sync(1 + pair, 64);                                   // staging tile free for the next step
+      } else {
+#pragma unroll 1
+        for (int s = 0; s < BN / 64; ++s) {
+          stage_write(acc, stg, s, wi, lane);
+          named_bar_sync(1 + pair, 64);
+          uint32_t v[32];
+          stage_read(stg, x, lane, v);
+          const int cc = 64 * s + 32 * x;                               // column of this chunk inside the tile
+          if (MODE == 2) {
+            float* trow = p.tok_out + (size_t)row0 * p.d + t.n_blk * BN + cc;
+            const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + t.n_blk * BN + cc + (lane & 7) * 4));
+            tok_chunk(v, b4, patch, trow, (size_t)p.d, lane, rows_left);
+          } else {
+            K2Chunk kc;
+            kc.l = t.z; kc.L = p.L; kc.d = p.d; kc.n = p.n; kc.row0 = row0; kc.prow0 = row0 % p.n; kc.s_bcast = p.s_bcast;
+            kc.s32_in = p.s32_in; kc.c_in = p.c_in; kc.pos = p.pos;
+            kc.s32_out = p.s32_out; kc.sb_out = p.sb_out; kc.sp_out = p.sp_out;
+            const int col = t.n_blk * BN + cc;
+            const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + (size_t)t.z * p.d + col + (lane & 7) * 4));
+            float rowsq[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) rowsq[i] = 0.f;
+            if (rows_left >= 32) k2_chunk<true>(v, b4, patch, kc, col, lane, 32, rowsq);
+            else k2_chunk<false>(v, b4, patch, kc, col, lane, rows_left, rowsq);
+            // one squared-norm partial per PART_COLS columns: with 64-column parts the two warps of the pair hold the two
+            // 32-column halves, summed in chunk order (0 + first) + second as in prep_state_kernel
+            int part = cc / Cfg::PART_COLS;
+            bool writer = true;
+            if (Cfg::PART_COLS == 64) {
+              if (x == 1 && (lane & 7) == 0) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) xch_p[i * 4 + (lane >> 3)] = rowsq[i];
+              }
+              named_bar_sync(1 + pair, 64);
+              if (x == 0) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) rowsq[i] += xch_p[i * 4 + (lane >> 3)];
+              }
+              writer = x == 0;
+            }
+            if (writer && (lane & 7) == 0) {
+              float* nsq = p.nsq_out + ((size_t)row0 * p.L + t.z) * p.nparts + t.n_blk * Cfg::PARTS + part;
+              const int ldn = p.L * p.nparts;   // row offsets r * ldn (r < 32) in 32 bits: half the registers once hoisted
+#pragma unroll
+              for (int i = 0; i < 8; ++i) {
+                const int r = i * 4 + (lane >> 3);
+                if (r < rows_left) nsq[(unsigned)(r * ldn)] = rowsq[i];
+              }
+            }
+          }
+          named_bar_sync(1 + pair, 64);                                   // staging tile free for the next step
+        }
       }
       if (cnt_cta) w1 += (unsigned long long)(clock64() - busy_t0);
     }
     if (cnt_cta && cw == 0 && lane == 0) { atomicAdd(&cnt[2], w0); atomicAdd(&cnt[6], w1); }
+    if (MODE == 0 && st_issuer) bulk_wait_group<0>();   // the output tiles stay allocated until the last stores are done
   }
 #undef GLOM_CNT_WAIT
 
@@ -810,21 +864,21 @@ cudaError_t tc_kernel_clocks(unsigned long long* out /* [PROF_KINDS][8] */, bool
 // =====================================================================================
 template <int MODE, int BN, bool CNT>
 static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& bm,
-                                    const GemmParams& p, int num_sms, cudaStream_t st);
+                                    const CUtensorMap& out, const GemmParams& p, int num_sms, cudaStream_t st);
 
 template <int MODE, int BN>
 static cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& bm,
-                               const GemmParams& p, int num_sms, cudaStream_t st) {
+                               const CUtensorMap& out, const GemmParams& p, int num_sms, cudaStream_t st) {
   // GLOM_B200_WAIT_COUNTERS=1 (diagnostics): the instantiation whose block 0 accumulates its roles' wait cycles
   static int count_waits = -1;
   if (count_waits < 0) { const char* ev = getenv("GLOM_B200_WAIT_COUNTERS"); count_waits = (ev && ev[0] == '1') ? 1 : 0; }
-  if (count_waits) return launch_gemm_impl<MODE, BN, true>(a0, a1, a2, bm, p, num_sms, st);
-  return launch_gemm_impl<MODE, BN, false>(a0, a1, a2, bm, p, num_sms, st);
+  if (count_waits) return launch_gemm_impl<MODE, BN, true>(a0, a1, a2, bm, out, p, num_sms, st);
+  return launch_gemm_impl<MODE, BN, false>(a0, a1, a2, bm, out, p, num_sms, st);
 }
 
 template <int MODE, int BN, bool CNT>
 static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& bm,
-                                    const GemmParams& p, int num_sms, cudaStream_t st) {
+                                    const CUtensorMap& out, const GemmParams& p, int num_sms, cudaStream_t st) {
   using Cfg = GemmCfg<MODE, BN>;
   static SmemOptIn optin;
   if (cudaError_t e = optin.ensure(gemm_kernel<MODE, BN, CNT>, Cfg::SMEM_BYTES)) return e;
@@ -851,7 +905,7 @@ static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1
   cfg.attrs = attr; cfg.numAttrs = 2;
   const int pairs = p.num_tiles < max_pairs ? p.num_tiles : max_pairs;
   cfg.gridDim = dim3(2 * pairs);
-  return cudaLaunchKernelEx(&cfg, gemm_kernel<MODE, BN, CNT>, a0, a1, a2, bm, p);
+  return cudaLaunchKernelEx(&cfg, gemm_kernel<MODE, BN, CNT>, a0, a1, a2, bm, out, p);
 }
 
 // K3: consensus attention -> C
@@ -934,9 +988,13 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int* sched, int step_inde
     return step_bf16_mlp_fused(g, b, sched, enc, num_sms, st, launches, err, errlen, prof);
   }
   // One launch each of K1 (all groups), K3, K2 (all levels).
-  CUtensorMap mh;
+  // H: (group, 128-row block, 64-column k block) blocks of 128 x 64, read by K2 a block at a time (mh) and written by
+  // K1 a warpgroup's 64 rows at a time (mh_out)
+  CUtensorMap mh, mh_out;
   const int m128 = (rows + BM - 1) / BM;
-  if (!map2d(enc, &mh, b.h, (uint64_t)g.G * m128 * (4 * d / BK) * BM, BK, BM, err, errlen, "H")) return -3;
+  const uint64_t h_rows = (uint64_t)g.G * m128 * (4 * d / BK) * BM;
+  if (!map2d(enc, &mh, b.h, h_rows, BK, BM, err, errlen, "H")) return -3;
+  if (!map2d(enc, &mh_out, b.h, h_rows, BK, 64, err, errlen, "H out")) return -3;
   CUtensorMap mx, msb, msp, mw1, mw2;
   if (!map2d(enc, &mx, b.xb, rows, d, BM, err, errlen, "Xb")) return -3;
   if (!map2d(enc, &msb, b.sb_in, rows, (uint64_t)L * d, BM, err, errlen, "Sb")) return -3;
@@ -955,15 +1013,15 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int* sched, int step_inde
     // Group order: GEMM2 of the previous step wrote the shadows level 0 first, the top level last, and this step's GEMM2
     // reads H level 0 first.  Walking the groups from the top down reads the most recently written shadows first (L2
     // hits) and leaves the groups GEMM2 starts with (levels 0, 1) as the last ones written; those are stored with the
-    // default L2 policy instead of streaming stores.  (GLOM_B200_K1_ORDER: bit 0 = reverse walk, bits 1.. = keep groups)
+    // default L2 policy instead of evict-first.  (GLOM_B200_K1_ORDER: bit 0 = reverse walk, bits 1.. = keep groups)
     static int k1_order = -1;
     if (k1_order < 0) { const char* ev = getenv("GLOM_B200_K1_ORDER"); k1_order = ev ? atoi(ev) : 0; }
     p.z_rev = k1_order & 1;
     p.h_keep_z = (k1_order >> 1) - 1;
     p.num_m = (rows + 255) / 256; p.num_n = 4 * d / 256; p.num_tiles = (g.G - p.z0) * p.num_m * p.num_n;
-    p.bias = b.b1; p.h_out = b.h; p.m128 = m128;
+    p.bias = b.b1; p.m128 = m128;
     ProfScope scope(prof, PROF_GEMM1, st);
-    cudaError_t e = launch_gemm<0, 256>(mx, msb, msp, mw1, p, num_sms, st);
+    cudaError_t e = launch_gemm<0, 256>(mx, msb, msp, mw1, mh_out, p, num_sms, st);
     if (launches) ++*launches;
     if (e != cudaSuccess) { snprintf(err, errlen, "gemm1 launch: %s", cudaGetErrorString(e)); return -3; }
   }
@@ -989,9 +1047,9 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int* sched, int step_inde
     p.h_load_policy = k2_hpol;
     cudaError_t e;
     ProfScope scope(prof, PROF_GEMM2, st);
-    if (g.bn2 == 256) e = launch_gemm<1, 256>(mh, mh, mh, mw2, p, num_sms, st);
-    else if (g.bn2 == 128) e = launch_gemm<1, 128>(mh, mh, mh, mw2, p, num_sms, st);
-    else e = launch_gemm<1, 64>(mh, mh, mh, mw2, p, num_sms, st);
+    if (g.bn2 == 256) e = launch_gemm<1, 256>(mh, mh, mh, mw2, mh, p, num_sms, st);
+    else if (g.bn2 == 128) e = launch_gemm<1, 128>(mh, mh, mh, mw2, mh, p, num_sms, st);
+    else e = launch_gemm<1, 64>(mh, mh, mh, mw2, mh, p, num_sms, st);
     if (launches) ++*launches;
     if (e != cudaSuccess) { snprintf(err, errlen, "gemm2 launch: %s", cudaGetErrorString(e)); return -3; }
   }
@@ -1011,9 +1069,9 @@ int tokenize_tc(const __nv_bfloat16* patches, const __nv_bfloat16* wtok, const f
   p.num_m = (rows + 255) / 256; p.num_n = d / bn; p.num_tiles = p.num_m * p.num_n;
   p.bias = bias; p.tok_out = tokens; p.tok_kb = kp / BK;
   cudaError_t e;
-  if (bn == 256) e = launch_gemm<2, 256>(ma, ma, ma, mb, p, num_sms, st);
-  else if (bn == 128) e = launch_gemm<2, 128>(ma, ma, ma, mb, p, num_sms, st);
-  else e = launch_gemm<2, 64>(ma, ma, ma, mb, p, num_sms, st);
+  if (bn == 256) e = launch_gemm<2, 256>(ma, ma, ma, mb, ma, p, num_sms, st);
+  else if (bn == 128) e = launch_gemm<2, 128>(ma, ma, ma, mb, ma, p, num_sms, st);
+  else e = launch_gemm<2, 64>(ma, ma, ma, mb, ma, p, num_sms, st);
   if (launches) ++*launches;
   if (e != cudaSuccess) { snprintf(err, errlen, "tokeniser gemm launch: %s", cudaGetErrorString(e)); return -3; }
   return 0;
