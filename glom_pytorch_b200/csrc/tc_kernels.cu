@@ -15,6 +15,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <type_traits>
+
 namespace glom {
 
 // =====================================================================================
@@ -459,29 +461,45 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
 
 // =====================================================================================
 // K3: consensus attention.  Persistent CTAs; a work item is (128-query tile, level l, image b).
-//   phase 1: S = Q K^T per key block of 128 keys over d: one TMA producer warp streams (Q, K) 64-column chunks through a
-//            ring, two consumer warpgroups run wgmma m64n128k16 on 64 query rows each with S in registers and turn it in
-//            place into unnormalised bf16 probabilities P in shared memory (wgmma A-operand layout, 128-byte swizzle).
+//   Warpgroup 0 is the producer and gives up registers (setmaxnreg) to the two consumer warpgroups.  Its warp 0 streams
+//   the operands through a ring of shared-memory slots with TMA; its warps 1-3 compute the next item's per-key scales
+//   into one of two scale buffers (mbarrier hand-off), so the consumers never wait on the squared-norm loads.
+//   phase 1: S = Q K^T per key block of KEYS keys over d: each slot holds a (Q, K) 64-column chunk; the two consumer
+//            warpgroups run wgmma m64 x KEYS x 16 on 64 query rows each with S in registers and turn it in place into
+//            unnormalised bf16 probabilities P in shared memory (wgmma A-operand layout, 128-byte swizzle).
+//            KEYS = 256 when all keys fit one block (n <= 256): S is a single pass over d and Q is loaded once per item.
 //   phase 2: O = P V in 256-wide slices of d (V read MN-major straight from the state shadow, 64 keys per ring slot),
-//            O in registers, scaled by 1/rowsum and written as bf16 C.
+//            O in registers, scaled by 1/rowsum and written as bf16 C: the four lanes of a row exchange their words so
+//            that each stores 16 contiguous bytes (a row's quad covers 64 contiguous bytes).
 // Softmax stabiliser: every key is unit-normalised, so |logit_ij| <= |S_i| d^-1/2 (Cauchy-Schwarz); that bound
 // replaces the row maximum (softmax is shift-invariant) and S needs one pass.  The diagonal is never masked (its logit
 // is -5e-4 or, with attend_self, ~ the bound itself), so the row sum cannot underflow while the bound stays below
 // 2^BOUND_MAX; warps with a row beyond that take the exact-maximum path.
 // =====================================================================================
 constexpr int ATTN_CONSUMER_WARPS = 8;
-constexpr int ATTN_THREADS = 32 * (ATTN_CONSUMER_WARPS + 1);
-constexpr int ATTN_KEYS = 128;                    // keys per S block (wgmma N)
-constexpr int ATTN_MAX_KB = 5;
-constexpr uint32_t ATTN_SLOT_BYTES = 32768;       // ring slot: Q + K chunk (16 + 16 KB), or 64 keys x 256 columns of V
+constexpr int ATTN_THREADS = 128 + 32 * ATTN_CONSUMER_WARPS;
+// 56 x 128 + 224 x 256 = 64,512 of the SM's 65,536 registers: the 64 x 256 fp32 S or O fragment (128 registers) and the
+// softmax / output work fit the consumers, and the scale warps' loads fit the producers, without spilling
+constexpr uint32_t ATTN_PRODUCER_REGS = 56;
+constexpr uint32_t ATTN_CONSUMER_REGS = 224;
+constexpr int ATTN_SCALE_WARPS = 3;               // producer warps 1-3: per-key scales of the next item
 constexpr float ATTN_BOUND_MAX = 96.f;            // log2 units
 constexpr int ATTN_SINGLE_PASS_MAX = 576;         // columns whose probabilities (128 queries x all keys) fit in shared memory
 constexpr int ATTN_PASS_KEYS = 512;               // keys per pass beyond that
 
+template <int KEYS>
+struct AttnCfg {
+  static_assert(KEYS == 128 || KEYS == 256, "S block = one wgmma N");
+  static constexpr int MAX_KB = (KEYS == 256) ? 1 : 5;                  // key blocks per pass (<= 576 keys)
+  // ring slot: Q chunk (128 x 64) + K chunk (KEYS x 64), or 64 keys x 256 columns of V (4 boxes of 64 x 64)
+  static constexpr uint32_t SLOT_BYTES = A_STAGE_BYTES + (uint32_t)KEYS * BK * 2;
+  static_assert(SLOT_BYTES >= 4 * 8192, "a slot holds a V chunk");
+};
+
 struct AttnParams {
   int n, L, d;
   int attend_self, mask_side, mask_d2_max;
-  int n_pad16, n_pad64, nkb, nchunk;   // key padding, key blocks (<= 128), 64-key chunks
+  int n_pad16, n_pad64, nkb, nchunk;   // key padding, key blocks of KEYS, 64-key chunks
   int num_stages;
   int ntiles, num_items;               // 128-query tiles per (l, b); ntiles * L * B
   int nparts;
@@ -497,110 +515,177 @@ struct AttnParams {
   float* ml_acc;                       // (rows, L, 2) fp32: stabiliser (log2 units), row sum
 };
 
-template <bool CNT>
+// shared-memory bytes of a pass: P (nchunk x [128 x 64] bf16), the ring, two scale buffers (rs, bnd) + key coordinates,
+// barriers and the clock sample
+constexpr size_t attn_fixed_smem(int nchunk, int n_pad16) {
+  return 1024 /*align slack*/ + (size_t)nchunk * A_STAGE_BYTES + (size_t)n_pad16 * (2 * 2 * 4 + 4) + 256;
+}
+static_assert(attn_fixed_smem(4, 256) + 3 * AttnCfg<256>::SLOT_BYTES <= 232448, "n = 256: three 48 KB slots");
+static_assert(attn_fixed_smem(9, 576) + 2 * AttnCfg<128>::SLOT_BYTES <= 232448, "n = 576: two 32 KB slots");
+
+// sum of a row's squared-norm partials, in order
+__device__ __forceinline__ float attn_row_norm(const float* ns, int nparts) {
+  float ss = 0.f;
+  if ((nparts & 3) == 0 && nparts <= 16) {      // one round trip: all partials in flight, then summed in order
+    float4 q[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      q[i] = 4 * i < nparts ? __ldg(reinterpret_cast<const float4*>(ns) + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) ss = (((ss + q[i].x) + q[i].y) + q[i].z) + q[i].w;
+  } else {
+    for (int i = 0; i < nparts; ++i) ss += ns[i];
+  }
+  return sqrtf(ss);
+}
+
+template <int KEYS, bool CNT>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64, 128, 1)
-            const __grid_constant__ CUtensorMap map_k,    // box (64, 128, 1)
+            const __grid_constant__ CUtensorMap map_k,    // box (64, KEYS, 1)
             const __grid_constant__ CUtensorMap map_v,    // box (64, 64, 1)
             const AttnParams p) {
+  using Cfg = AttnCfg<KEYS>;
+  constexpr uint32_t SLOT = Cfg::SLOT_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* p_smem = smem;                                                  // nchunk x [128 x 64] bf16, SW128
   uint8_t* stages = p_smem + (size_t)p.nchunk * A_STAGE_BYTES;
-  float* rs = reinterpret_cast<float*>(stages + (size_t)p.num_stages * ATTN_SLOT_BYTES);   // [n_pad16] per-key scales
-  float* bnd = rs + p.n_pad16;                                             // [n_pad16] per-row logit bounds
-  uint32_t* key_hw = reinterpret_cast<uint32_t*>(bnd + p.n_pad16);         // [n_pad16] (grid row << 16) | grid column
+  // scale buffer b: rs = sc + 2 b n_pad16 [n_pad16] per-key scales, bnd = rs + n_pad16 [n_pad16] per-row logit bounds
+  float* sc = reinterpret_cast<float*>(stages + (size_t)p.num_stages * SLOT);
+  uint32_t* key_hw = reinterpret_cast<uint32_t*>(sc + 4 * p.n_pad16);      // [n_pad16] (grid row << 16) | grid column
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(key_hw + p.n_pad16);
   uint64_t* empty_bar = full_bar + p.num_stages;
+  uint64_t* sc_full = empty_bar + p.num_stages;                           // [2] scale buffer filled (3 scale warps)
+  uint64_t* sc_empty = sc_full + 2;                                       // [2] scale buffer released (8 consumer warps)
+  ClockSample* clk_s = reinterpret_cast<ClockSample*>(sc_empty + 2);
 
+  // warpgroup 0 = producer (warp 0: TMA, warps 1-3: scales), warpgroups 1 and 2 = consumers
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  constexpr int W_TMA = ATTN_CONSUMER_WARPS;
+  constexpr int W_TMA = 0;
+  constexpr int W_CONSUMER0 = 4;
   const int nsub = (p.d + 255) / 256;                  // O slices per item
   const int per_img = p.ntiles * p.L;
+  const int nkb = (KEYS == 256) ? 1 : p.nkb;           // compile-time single key block on the 256-key path
+  constexpr float LOG2E = 1.4426950408889634f;
 
   if (warp == W_TMA && lane == 0) {
     tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v);
     for (int i = 0; i < p.num_stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], ATTN_CONSUMER_WARPS); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&sc_full[i], ATTN_SCALE_WARPS); mbar_init(&sc_empty[i], ATTN_CONSUMER_WARPS); }
     fence_barrier_init();
   }
   __syncthreads();
   pdl_launch_dependents();
   pdl_wait();
   const bool clk_thread = blockIdx.x == 0 && warp == W_TMA && lane == 0;
-  ClockSample clk_s{};
-  if (clk_thread) clk_s = clock_sample_begin();
+  // the sample's start waits in shared memory: held in a register it would be live across the consumers' code
+  if (clk_thread) *clk_s = clock_sample_begin();
   // diagnostic instantiation (GLOM_B200_WAIT_COUNTERS=1): block 0's wait / busy cycles per role, in g_kernel_clk[PROF_ATTN]:
-  // [4] TMA lane waiting for a free slot, [5] consumer warp 0 waiting for operands, [6] its softmax work, [7] its output work
+  // [4] TMA lane waiting for a free slot, [5] consumer warp 0 waiting for operands (ring slots and scale buffers),
+  // [6] its softmax work, [7] its output work
   const bool cnt_cta = CNT && blockIdx.x == 0;
   unsigned long long* const cnt = g_kernel_clk[PROF_ATTN];
   unsigned long long w0 = 0, w1 = 0, w2 = 0;
 #define GLOM_CNT_WAIT(acc, stmt) do { if (cnt_cta) { const long long t_ = clock64(); stmt; acc += (unsigned long long)(clock64() - t_); } else { stmt; } } while (0)
 
-  if (warp == W_TMA) {
-    // ------------------------------------------------------------------ TMA producer, warp-converged
-    const uint32_t elected = elect_one();
-    int stage = 0; uint32_t phase = 0;
-    const uint32_t stages0 = smem_u32(stages);
-    for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
-      const int b = it / per_img, l = (it % per_img) / p.ntiles;
-      const int q0 = (it % p.ntiles) * BM;
-      for (int kb = 0; kb < p.nkb; ++kb) {
-        for (int dc = 0; dc < p.d / BK; ++dc) {
-          GLOM_CNT_WAIT(w0, mbar_wait(&empty_bar[stage], phase ^ 1));
-          if (elected) {
-            const uint32_t s = stages0 + (uint32_t)stage * ATTN_SLOT_BYTES;
-            mbar_arrive_expect_tx(&full_bar[stage], 2u * A_STAGE_BYTES);
-            tma_load_3d(s, &map_q, &full_bar[stage], l * p.d + dc * BK, q0, b);
-            tma_load_3d(s + A_STAGE_BYTES, &map_k, &full_bar[stage], l * p.d + dc * BK, p.key0 + kb * ATTN_KEYS, b);
+  if (warp < W_CONSUMER0) {
+    setmaxnreg_dec<ATTN_PRODUCER_REGS>();
+    if (warp == W_TMA) {
+      // ---------------------------------------------------------------- TMA producer, warp-converged
+      const uint32_t elected = elect_one();
+      int stage = 0; uint32_t phase = 0;
+      const uint32_t stages0 = smem_u32(stages);
+      for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
+        const int b = it / per_img, l = (it % per_img) / p.ntiles;
+        const int q0 = (it % p.ntiles) * BM;
+        for (int kb = 0; kb < nkb; ++kb) {
+          for (int dc = 0; dc < p.d / BK; ++dc) {
+            GLOM_CNT_WAIT(w0, mbar_wait(&empty_bar[stage], phase ^ 1));
+            if (elected) {
+              const uint32_t s = stages0 + (uint32_t)stage * SLOT;
+              mbar_arrive_expect_tx(&full_bar[stage], SLOT);
+              tma_load_3d(s, &map_q, &full_bar[stage], l * p.d + dc * BK, q0, b);
+              tma_load_3d(s + A_STAGE_BYTES, &map_k, &full_bar[stage], l * p.d + dc * BK, p.key0 + kb * KEYS, b);
+            }
+            __syncwarp();
+            if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
           }
-          __syncwarp();
-          if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
+        }
+        for (int sp = 0; sp < nsub; ++sp) {
+          for (int kc = 0; kc < p.nchunk; ++kc) {
+            GLOM_CNT_WAIT(w0, mbar_wait(&empty_bar[stage], phase ^ 1));
+            if (elected) {
+              const uint32_t s = stages0 + (uint32_t)stage * SLOT;
+              mbar_arrive_expect_tx(&full_bar[stage], 4u * 8192u);
+              for (int i = 0; i < 4; ++i) {
+                const int dcol = sp * 256 + i * 64;
+                tma_load_3d(s + i * 8192, &map_v, &full_bar[stage], dcol < p.d ? l * p.d + dcol : p.L * p.d,
+                            p.key0 + kc * 64, b);                              // past d: out of bounds -> zeros
+              }
+            }
+            __syncwarp();
+            if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
+          }
         }
       }
-      for (int sp = 0; sp < nsub; ++sp) {
-        for (int kc = 0; kc < p.nchunk; ++kc) {
-          GLOM_CNT_WAIT(w0, mbar_wait(&empty_bar[stage], phase ^ 1));
-          if (elected) {
-            const uint32_t s = stages0 + (uint32_t)stage * ATTN_SLOT_BYTES;
-            mbar_arrive_expect_tx(&full_bar[stage], 4u * 8192u);
-            for (int i = 0; i < 4; ++i) {
-              const int dcol = sp * 256 + i * 64;
-              tma_load_3d(s + i * 8192, &map_v, &full_bar[stage], dcol < p.d ? l * p.d + dcol : p.L * p.d,
-                          p.key0 + kc * 64, b);                              // past d: out of bounds -> zeros
-            }
+      if (cnt_cta && elected) atomicAdd(&cnt[4], w0);
+    } else {
+      // ---------------------------------------------------------------- scale warps: per-key scales, one item ahead
+      const int t = threadIdx.x - 32;
+      // key coordinates for the careful path, written once: padding keys sit 20000 rows away, so one distance test masks
+      // them as well (:67-69; without a radius every real key is at (0, 0), the query at (0, 0) and the threshold 1).
+      // The consumers read them only after their first scale-buffer wait, which orders them after these writes.
+      const bool use_mask = p.mask_side > 0;
+      for (int j = t; j < p.n_pad16; j += 32 * ATTN_SCALE_WARPS)
+        key_hw[j] = j >= p.nk ? (20000u << 16)
+                              : use_mask ? ((uint32_t)((p.key0 + j) / p.mask_side) << 16) | (uint32_t)((p.key0 + j) % p.mask_side) : 0u;
+      int k = 0;
+      for (int it = blockIdx.x; it < p.num_items; it += gridDim.x, ++k) {
+        const int b = it / per_img, l = (it % per_img) / p.ntiles;
+        const size_t img_row0 = (size_t)b * p.n;
+        const int buf = k & 1;
+        mbar_wait(&sc_empty[buf], ((k >> 1) & 1) ^ 1);
+        float* rs = sc + 2 * buf * p.n_pad16;
+        float* bnd = rs + p.n_pad16;
+        // per-key scale  log2(e) d^-1/2 / max(|S_j|, 1e-12)  (F.normalize eps, :58; logits are kept in log2 units)
+        // and per-row bound  log2(e) d^-1/2 |S_j|  on the magnitude of row j's logits
+        for (int j = t; j < p.n_pad16; j += 32 * ATTN_SCALE_WARPS) {
+          float v = 0.f, bd = 0.f;
+          if (j < p.nk) {
+            const float nrm = attn_row_norm(p.nsq + ((img_row0 + p.key0 + j) * p.L + l) * p.nparts, p.nparts);
+            v = p.scale * LOG2E / fmaxf(nrm, 1e-12f);
+            bd = p.scale * LOG2E * nrm;
           }
-          __syncwarp();
-          if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
+          rs[j] = v;
+          bnd[j] = bd;
         }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&sc_full[buf]);
       }
     }
-    if (cnt_cta && elected) atomicAdd(&cnt[4], w0);
-  } else if (warp < W_TMA) {
-    // ------------------------------------------------------------------ consumers: 2 warpgroups x 64 query rows
+  } else {
+    // ---------------------------------------------------------------- consumers: 2 warpgroups x 64 query rows
+    setmaxnreg_inc<ATTN_CONSUMER_REGS>();
     // thread rows (fragment layout of wgmma, see ptx.cuh): tile rows r_h = 64 wg + 16 wi + lane / 4 + 8 h, h = 0, 1;
     // fragment element i holds column 8 (i / 4) + 2 (lane % 4) + (i % 2) of row r_{(i / 2) % 2}
-    const int wg = warp >> 2, wi = warp & 3;
-    const int ctid = threadIdx.x;
+    const int cw = warp - W_CONSUMER0;
+    const int wg = cw >> 2, wi = cw & 3;
     const int rbase = 64 * wg + 16 * wi + (lane >> 2);
     const int cq = 2 * (lane & 3);
-    constexpr float LOG2E = 1.4426950408889634f;
     const float NEG_INF = __int_as_float(0xff800000);
     const bool use_mask = p.mask_side > 0;
     const uint32_t stages0 = smem_u32(stages);
     const uint32_t p0 = smem_u32(p_smem);
     int stage = 0; uint32_t phase = 0;
 
-    // key coordinates for the careful path: padding keys sit 20000 rows away, so one distance test masks them as well
-    // (:67-69; without a radius every real key is at (0, 0), the query at (0, 0) and the threshold 1)
-    for (int j = ctid; j < p.n_pad16; j += 256)
-      key_hw[j] = j >= p.nk ? (20000u << 16)
-                            : use_mask ? ((uint32_t)((p.key0 + j) / p.mask_side) << 16) | (uint32_t)((p.key0 + j) % p.mask_side) : 0u;
     const int d2_max = use_mask ? p.mask_d2_max : 1;
-    // K-padding keys of the last 64-key chunk: P = 0, never written again
+    // K-padding keys of the last 64-key chunk, this warpgroup's rows: P = 0, never written again (visible to the
+    // warpgroup's wgmma reads through the fence + barrier before its first P V)
     const int npadk = (p.n_pad64 - p.n_pad16) >> 3;
-    for (int idx = ctid; idx < 128 * npadk; idx += 256) {
-      const int t = idx & 127, key = p.n_pad16 + 8 * (idx >> 7);
+    for (int idx = threadIdx.x & 127; idx < 64 * npadk; idx += 128) {
+      const int t = 64 * wg + (idx & 63), key = p.n_pad16 + 8 * (idx >> 6);
       *reinterpret_cast<uint4*>(p_smem + (size_t)(key >> 6) * A_STAGE_BYTES + (size_t)t * 128 + ((((key & 63) >> 3) ^ (t & 7)) << 4)) =
           make_uint4(0, 0, 0, 0);
     }
@@ -610,41 +695,18 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
       return reinterpret_cast<uint32_t*>(p_smem + (size_t)(key >> 6) * A_STAGE_BYTES + (size_t)r * 128 +
                                          ((((key & 63) >> 3) ^ (r & 7)) << 4) + (key & 7) * 2);
     };
-    auto row_norm = [&](const float* ns) -> float {     // sum of the row's squared-norm partials, in order
-      float ss = 0.f;
-      if ((p.nparts & 3) == 0 && p.nparts <= 16) {      // one round trip: all partials in flight, then summed in order
-        float4 q[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          q[i] = 4 * i < p.nparts ? __ldg(reinterpret_cast<const float4*>(ns) + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) ss = (((ss + q[i].x) + q[i].y) + q[i].z) + q[i].w;
-      } else {
-        for (int i = 0; i < p.nparts; ++i) ss += ns[i];
-      }
-      return sqrtf(ss);
-    };
 
-    for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
+    int k = 0;
+    for (int it = blockIdx.x; it < p.num_items; it += gridDim.x, ++k) {
       const int b = it / per_img, l = (it % per_img) / p.ntiles;
       const int q0 = (it % p.ntiles) * BM;
       const size_t img_row0 = (size_t)b * p.n;
       const long long cnt_t0 = cnt_cta ? clock64() : 0;
       const unsigned long long cnt_w0 = w0;
-      // per-key scale  log2(e) d^-1/2 / max(|S_j|, 1e-12)  (F.normalize eps, :58; logits are kept in log2 units)
-      // and per-row bound  log2(e) d^-1/2 |S_j|  on the magnitude of row j's logits
-      named_bar_sync(1, 256);                  // the previous item is done with the scale arrays
-      for (int j = ctid; j < p.n_pad16; j += 256) {
-        float v = 0.f, bd = 0.f;
-        if (j < p.nk) {
-          const float nrm = row_norm(p.nsq + ((img_row0 + p.key0 + j) * p.L + l) * p.nparts);
-          v = p.scale * LOG2E / fmaxf(nrm, 1e-12f);
-          bd = p.scale * LOG2E * nrm;
-        }
-        rs[j] = v;
-        bnd[j] = bd;
-      }
-      named_bar_sync(1, 256);
+      const int buf = k & 1;
+      GLOM_CNT_WAIT(w0, mbar_wait(&sc_full[buf], (k >> 1) & 1));     // this item's scales
+      const float* rs = sc + 2 * buf * p.n_pad16;
+      const float* bnd = rs + p.n_pad16;
 
       const bool multi = !(p.pass_first && p.pass_last);
       int qi[2];
@@ -655,11 +717,11 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
         row_bound[h] = 0.f;
         if (qi[h] < p.n) {
           if (!multi) row_bound[h] = bnd[qi[h]];
-          else row_bound[h] = p.scale * LOG2E * row_norm(p.nsq + ((img_row0 + qi[h]) * p.L + l) * p.nparts);
+          else row_bound[h] = p.scale * LOG2E * attn_row_norm(p.nsq + ((img_row0 + qi[h]) * p.L + l) * p.nparts, p.nparts);
         }
       }
       const bool exact_max = __any_sync(0xffffffffu, !(row_bound[0] <= ATTN_BOUND_MAX) || !(row_bound[1] <= ATTN_BOUND_MAX));
-      float m_run[2], l_run[2] = {0.f, 0.f}, m_used[ATTN_MAX_KB][2];
+      float m_run[2], l_run[2] = {0.f, 0.f}, m_used[Cfg::MAX_KB][2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) m_run[h] = exact_max ? NEG_INF : row_bound[h];
       const int qh[2] = {use_mask ? qi[0] / p.mask_side : 0, use_mask ? qi[1] / p.mask_side : 0};
@@ -667,17 +729,17 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
       const int wrow0 = q0 + 64 * wg + 16 * wi;                 // first query of this warp's 16 rows
 
 #pragma unroll 1
-      for (int kb = 0; kb < p.nkb; ++kb) {
-        float s[64];
+      for (int kb = 0; kb < nkb; ++kb) {
+        float s[KEYS / 2];
 #pragma unroll
-        for (int i = 0; i < 64; ++i) s[i] = 0.f;
+        for (int i = 0; i < KEYS / 2; ++i) s[i] = 0.f;
         int prev = -1;                    // slot of the k-block whose MMAs may still be running
         for (int dc = 0; dc < p.d / BK; ++dc) {
           GLOM_CNT_WAIT(w0, mbar_wait(&full_bar[stage], phase));
-          const uint32_t sa = stages0 + (uint32_t)stage * ATTN_SLOT_BYTES;
+          const uint32_t sa = stages0 + (uint32_t)stage * SLOT;
           wgmma_fence_regs(s);
           wgmma_fence();
-          wgmma_kblock<ATTN_KEYS, 0>(s, sa + (uint32_t)wg * (A_STAGE_BYTES / 2), sa + A_STAGE_BYTES);
+          wgmma_kblock<KEYS, 0>(s, sa + (uint32_t)wg * (A_STAGE_BYTES / 2), sa + A_STAGE_BYTES);
           wgmma_commit();
           wgmma_wait<1>();                  // the previous k-block's MMAs are complete: release its slot
           wgmma_fence_regs(s);
@@ -689,29 +751,52 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
         wgmma_fence_regs(s);
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
-        const int kbase = kb * ATTN_KEYS;                       // pass-local index of the block's first key
-        const int w = min(ATTN_KEYS, p.n_pad16 - kbase);
-        // logits (log2 units).  Plain blocks -- no padding, radius mask or diagonal of this warp's rows, a warp-uniform
-        // property -- take one multiply per key; the others the select chain of the reference's masking.
+        const int kbase = kb * KEYS;                            // pass-local index of the block's first key
+        const int w = min(KEYS, p.n_pad16 - kbase);
+        // logits (log2 units).  Blocks of real keys without a radius mask (every block of configs[1]) take one multiply
+        // and one diagonal select per key, in straight-line code: per-element branches between the variants would
+        // leave the two consumer warps of each scheduler waiting on branch and dependency latency.  The others take
+        // the select chain of the reference's masking.
         const int gk0 = p.key0 + kbase;
-        const bool plain = !use_mask && kbase + ATTN_KEYS <= p.nk &&
-                           (p.attend_self || wrow0 + 16 <= gk0 || wrow0 >= gk0 + ATTN_KEYS);
+        const bool plain_keys = !use_mask && kbase + KEYS <= p.nk;      // implies w == KEYS
+        if (plain_keys) {
+          // key 8 jj + e of this lane's columns is row h's diagonal iff 8 jj + e == dq[h]; -1 never matches
+          const bool diag = !p.attend_self && wrow0 + 16 > gk0 && wrow0 < gk0 + KEYS;
+          const int dq[2] = {diag ? qi[0] - gk0 - cq : -1, diag ? qi[1] - gk0 - cq : -1};
 #pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          const int h = (i >> 1) & 1;
-          const int col = 8 * (i >> 2) + cq + (i & 1);
-          if (col < w) {
-            const int j = kbase + col;
-            float sv = s[i] * rs[j];                                                  // (:60)
-            if (!plain) {
-              sv = (!p.attend_self && p.key0 + j == qi[h]) ? -5e-4f * LOG2E : sv;     // (:62-65)
-              const uint32_t hw = key_hw[j];
-              const int dh = qh[h] - (int)(hw >> 16), dw = qw[h] - (int)(hw & 0xFFFFu);
-              sv = (dh * dh + dw * dw > d2_max) ? NEG_INF : sv;                       // (:67-69) and key padding
+          for (int jj = 0; jj < KEYS / 8; ++jj) {
+            const float2 r2 = *reinterpret_cast<const float2*>(rs + kbase + 8 * jj + cq);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float sv = s[4 * jj + 2 * h + e] * (e ? r2.y : r2.x);                   // (:60)
+                s[4 * jj + 2 * h + e] = (8 * jj + e == dq[h]) ? -5e-4f * LOG2E : sv;         // (:62-65)
+              }
+          }
+        } else {
+#pragma unroll
+          for (int jj = 0; jj < KEYS / 8; ++jj) {
+            const int col = 8 * jj + cq;
+            if (col < w) {
+              const int j = kbase + col;
+              const float2 r2 = *reinterpret_cast<const float2*>(rs + j);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  float sv = s[4 * jj + 2 * h + e] * (e ? r2.y : r2.x);                       // (:60)
+                  sv = (!p.attend_self && p.key0 + j + e == qi[h]) ? -5e-4f * LOG2E : sv;     // (:62-65)
+                  const uint32_t hw = key_hw[j + e];
+                  const int dh = qh[h] - (int)(hw >> 16), dw = qw[h] - (int)(hw & 0xFFFFu);
+                  sv = (dh * dh + dw * dw > d2_max) ? NEG_INF : sv;                           // (:67-69) and key padding
+                  s[4 * jj + 2 * h + e] = sv;
+                }
+              }
+            } else {
+#pragma unroll
+              for (int e = 0; e < 4; ++e) s[4 * jj + e] = NEG_INF;
             }
-            s[i] = sv;
-          } else {
-            s[i] = NEG_INF;
           }
         }
         float m_safe[2] = {m_run[0], m_run[1]};
@@ -720,7 +805,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
           for (int h = 0; h < 2; ++h) {
             float bm = NEG_INF;
 #pragma unroll
-            for (int i = 0; i < 64; ++i) if (((i >> 1) & 1) == h) bm = fmaxf(bm, s[i]);
+            for (int i = 0; i < KEYS / 2; ++i) if (((i >> 1) & 1) == h) bm = fmaxf(bm, s[i]);
             bm = fmaxf(bm, __shfl_xor_sync(0xffffffffu, bm, 1));
             bm = fmaxf(bm, __shfl_xor_sync(0xffffffffu, bm, 2));
             const float m_new = fmaxf(m_run[h], bm);
@@ -729,30 +814,39 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
             m_run[h] = m_new;
           }
         }
-        // unnormalised probabilities 2^(logit - m) -> bf16 P and their running sum
+        // unnormalised probabilities 2^(logit - m) -> bf16 P and their running sum (a whole block: no column test)
+        auto probs = [&](auto full) {
 #pragma unroll
-        for (int jj = 0; jj < 16; ++jj) {
-          const int col = 8 * jj + cq;
+          for (int jj = 0; jj < KEYS / 8; ++jj) {
+            const int col = 8 * jj + cq;
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const float e0 = ex2_approx(s[4 * jj + 2 * h] - m_safe[h]), e1 = ex2_approx(s[4 * jj + 2 * h + 1] - m_safe[h]);
-            l_run[h] += e0 + e1;
-            if (col < w) *p_word(rbase + 8 * h, kbase + col) = pack_bf16x2(e0, e1);
+            for (int h = 0; h < 2; ++h) {
+              const float e0 = ex2_approx(s[4 * jj + 2 * h] - m_safe[h]), e1 = ex2_approx(s[4 * jj + 2 * h + 1] - m_safe[h]);
+              l_run[h] += e0 + e1;
+              if (decltype(full)::value || col < w) *p_word(rbase + 8 * h, kbase + col) = pack_bf16x2(e0, e1);
+            }
           }
-        }
-        m_used[kb][0] = m_safe[0]; m_used[kb][1] = m_safe[1];
+        };
+        if (w == KEYS) probs(std::true_type{});
+        else probs(std::false_type{});
+#pragma unroll
+        for (int i = 0; i < Cfg::MAX_KB; ++i)             // static indices: m_used stays in registers
+          if (i == kb) { m_used[i][0] = m_safe[0]; m_used[i][1] = m_safe[1]; }
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&sc_empty[buf]);             // done with this item's scales
       if (exact_max) {
         // bring every block's probabilities onto the final stabiliser
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const float m_fin = (m_run[h] == NEG_INF) ? 0.f : m_run[h];
-          for (int kb = 0; kb < p.nkb; ++kb) {
-            if (m_used[kb][h] == m_fin) continue;
+#pragma unroll
+          for (int kb = 0; kb < Cfg::MAX_KB; ++kb) {
+            if (kb >= nkb || m_used[kb][h] == m_fin) continue;
             const float f = ex2_approx(m_used[kb][h] - m_fin);
-            const int w = min(ATTN_KEYS, p.n_pad16 - kb * ATTN_KEYS);
+            const int w = min(KEYS, p.n_pad16 - kb * KEYS);
             for (int col = cq; col < w; col += 8) {
-              uint32_t* ptr = p_word(rbase + 8 * h, kb * ATTN_KEYS + col);
+              uint32_t* ptr = p_word(rbase + 8 * h, kb * KEYS + col);
               const uint32_t wv = *ptr;
               *ptr = pack_bf16x2(__uint_as_float(wv << 16) * f, __uint_as_float(wv & 0xFFFF0000u) * f);
             }
@@ -807,7 +901,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
         int prev = -1;                    // slot of the k-block whose MMAs may still be running
         for (int kc = 0; kc < p.nchunk; ++kc) {
           GLOM_CNT_WAIT(w0, mbar_wait(&full_bar[stage], phase));
-          const uint32_t sa = stages0 + (uint32_t)stage * ATTN_SLOT_BYTES;
+          const uint32_t sa = stages0 + (uint32_t)stage * SLOT;
           wgmma_fence_regs(o);
           wgmma_fence();
           wgmma_kblock<256, 1>(o, p0 + (uint32_t)kc * A_STAGE_BYTES + (uint32_t)wg * (A_STAGE_BYTES / 2), sa);
@@ -822,31 +916,60 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
         wgmma_fence_regs(o);
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (multi) {
 #pragma unroll
-        for (int i = 0; i < 128; i += 2) {
-          const int h = (i >> 1) & 1;
-          const int col = sp * 256 + 8 * (i >> 2) + cq;                 // columns past d hold zeros
-          if (col >= p.d || qi[h] >= p.n) continue;
-          float v0 = o[i], v1 = o[i + 1];
-          if (multi) {
+          for (int i = 0; i < 128; i += 2) {
+            const int h = (i >> 1) & 1;
+            const int col = sp * 256 + 8 * (i >> 2) + cq;               // columns past d hold zeros
+            if (col >= p.d || qi[h] >= p.n) continue;
+            float v0 = o[i], v1 = o[i + 1];
             float2* accp = reinterpret_cast<float2*>(p.o_acc + acc_row[h] * p.d + col);
             float2 prev = make_float2(0.f, 0.f);
             if (!p.pass_first) prev = *accp;
             v0 = v0 * f_new[h] + prev.x * f_old[h];
             v1 = v1 * f_new[h] + prev.y * f_old[h];
             if (!p.pass_last) { *accp = make_float2(v0, v1); continue; }
+            *reinterpret_cast<uint32_t*>(p.c_out + acc_row[h] * p.d + col) = pack_bf16x2(v0 * inv_l[h], v1 * inv_l[h]);
           }
-          *reinterpret_cast<uint32_t*>(p.c_out + acc_row[h] * p.d + col) = pack_bf16x2(v0 * inv_l[h], v1 * inv_l[h]);
+        } else {
+          // Lane q of a row's quad holds word t of every group of 4 column octets (columns 32 g + 8 t + 2 q, + 1).  A 4 x 4
+          // transpose across the quad (two xor-shuffle rounds) gives lane q all 4 words of octet q: 16 contiguous bytes.
+          const int q = lane & 3;
+          const bool b1 = q & 1, b2 = q & 2;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            __nv_bfloat16* crow = p.c_out + acc_row[h] * p.d + sp * 256 + 8 * q;
+            const bool row_ok = qi[h] < p.n;
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+              uint32_t a[4];
+#pragma unroll
+              for (int t = 0; t < 4; ++t)
+                a[t] = pack_bf16x2(o[4 * (4 * g + t) + 2 * h] * inv_l[h], o[4 * (4 * g + t) + 2 * h + 1] * inv_l[h]);
+#pragma unroll
+              for (int pr = 0; pr < 2; ++pr) {          // swap the words whose lane and word bit 0 differ
+                const uint32_t r = __shfl_xor_sync(0xffffffffu, b1 ? a[2 * pr] : a[2 * pr + 1], 1);
+                if (b1) a[2 * pr] = r; else a[2 * pr + 1] = r;
+              }
+#pragma unroll
+              for (int pr = 0; pr < 2; ++pr) {          // ... then those whose bit 1 differs
+                const uint32_t r = __shfl_xor_sync(0xffffffffu, b2 ? a[pr] : a[2 + pr], 2);
+                if (b2) a[pr] = r; else a[2 + pr] = r;
+              }
+              if (row_ok && sp * 256 + 32 * g < p.d)   // d is a multiple of 64: a 32-column group is all in or all out
+                *reinterpret_cast<uint4*>(crow + 32 * g) = make_uint4(a[0], a[1], a[2], a[3]);
+            }
+          }
         }
       }
       if (cnt_cta) w2 += (unsigned long long)(clock64() - cnt_t1) - (w0 - cnt_w1);          // output work
     }
-    if (cnt_cta && warp == 0 && lane == 0) { atomicAdd(&cnt[5], w0); atomicAdd(&cnt[6], w1); atomicAdd(&cnt[7], w2); }
+    if (cnt_cta && cw == 0 && lane == 0) { atomicAdd(&cnt[5], w0); atomicAdd(&cnt[6], w1); atomicAdd(&cnt[7], w2); }
   }
 #undef GLOM_CNT_WAIT
 
   __syncthreads();
-  if (clk_thread) clock_sample_end(clk_s, g_kernel_clk[PROF_ATTN]);
+  if (clk_thread) clock_sample_end(*clk_s, g_kernel_clk[PROF_ATTN]);
 }
 
 // cycles / ns accumulated by the kernels of this translation unit since the last call (and reset)
@@ -908,6 +1031,20 @@ static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1
   return cudaLaunchKernelEx(&cfg, gemm_kernel<MODE, BN, CNT>, a0, a1, a2, bm, out, p);
 }
 
+template <int KEYS, bool CNT>
+static cudaError_t launch_attn_impl(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& ap,
+                                    size_t smem, int ctas, cudaStream_t st) {
+  static SmemOptIn optin;
+  if (cudaError_t e = optin.ensure(attn_kernel<KEYS, CNT>, smem)) return e;
+  cudaLaunchConfig_t acfg{};
+  acfg.gridDim = dim3(ctas); acfg.blockDim = dim3(ATTN_THREADS); acfg.dynamicSmemBytes = smem; acfg.stream = st;
+  cudaLaunchAttribute aattr[1];
+  aattr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernel
+  aattr[0].val.programmaticStreamSerializationAllowed = 1;
+  acfg.attrs = aattr; acfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&acfg, attn_kernel<KEYS, CNT>, mq, mk, mv, ap);
+}
+
 // K3: consensus attention -> C
 static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiledFn enc, int num_sms, cudaStream_t st,
                             int* launches, char* err, size_t errlen, Profiler* prof) {
@@ -919,13 +1056,19 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiled
     snprintf(err, errlen, "consensus for n = %d columns needs the key-pass scratch buffer (workspace too old?)", n);
     return -3;
   }
+  // All keys of a single pass of more than 128 and at most 256 (padded) keys form one 256-key S block; every other
+  // pass uses 128-key blocks
+  const int keys = (npass == 1 && (n + 15) / 16 * 16 > 128 && (n + 15) / 16 * 16 <= 256) ? 256 : 128;
   CUtensorMap mq, mk, mv;
   const uint64_t dims[3] = {(uint64_t)L * d, (uint64_t)n, (uint64_t)g.B};
   const uint64_t strides[2] = {(uint64_t)L * d * 2, (uint64_t)n * L * d * 2};
-  const uint32_t boxq[3] = {(uint32_t)BK, (uint32_t)BM, 1}, boxv[3] = {(uint32_t)BK, 64, 1};
+  const uint32_t boxq[3] = {(uint32_t)BK, (uint32_t)BM, 1}, boxk[3] = {(uint32_t)BK, (uint32_t)keys, 1};
+  const uint32_t boxv[3] = {(uint32_t)BK, 64, 1};
   if (!encode_map(enc, &mq, b.sb_in, 3, dims, strides, boxq, err, errlen, "attn.q")) return -3;
-  if (!encode_map(enc, &mk, b.sb_in, 3, dims, strides, boxq, err, errlen, "attn.k")) return -3;
+  if (!encode_map(enc, &mk, b.sb_in, 3, dims, strides, boxk, err, errlen, "attn.k")) return -3;
   if (!encode_map(enc, &mv, b.sb_in, 3, dims, strides, boxv, err, errlen, "attn.v")) return -3;
+  static int count_waits = -1;
+  if (count_waits < 0) { const char* ev = getenv("GLOM_B200_WAIT_COUNTERS"); count_waits = (ev && ev[0] == '1') ? 1 : 0; }
   for (int pass = 0; pass < npass; ++pass) {
     AttnParams ap{};
     ap.n = n; ap.L = L; ap.d = d;
@@ -937,7 +1080,7 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiled
     ap.ml_acc = b.attn_acc ? b.attn_acc + (size_t)g.rows * L * d : nullptr;
     ap.n_pad16 = (ap.nk + 15) / 16 * 16;
     ap.n_pad64 = (ap.nk + 63) / 64 * 64;
-    ap.nkb = (ap.n_pad16 + ATTN_KEYS - 1) / ATTN_KEYS;
+    ap.nkb = (ap.n_pad16 + keys - 1) / keys;
     ap.nchunk = ap.n_pad64 / 64;
     ap.nparts = g.nparts;
     ap.nsq = b.nsq_in;
@@ -945,34 +1088,26 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiled
     ap.scale = 1.0f / sqrtf((float)d);
     ap.ntiles = (n + BM - 1) / BM;
     ap.num_items = ap.ntiles * L * g.B;
-    const size_t fixed = 1024 + (size_t)ap.nchunk * A_STAGE_BYTES + (size_t)ap.n_pad16 * 12 + 256;
-    const size_t max_smem = 227 * 1024;
+    // 256 keys: 3 slots of 48 KB next to 64 KB of P (n = 256: 219,392 B); 128 keys: 2 slots of 32 KB at 576 keys
+    const uint32_t slot = keys == 256 ? AttnCfg<256>::SLOT_BYTES : AttnCfg<128>::SLOT_BYTES;
+    const size_t fixed = attn_fixed_smem(ap.nchunk, ap.n_pad16);
+    const size_t max_smem = 232448;                       // the 227 KB of shared memory a block may opt in to
     int stages = 4;
-    while (stages > 0 && fixed + (size_t)stages * ATTN_SLOT_BYTES > max_smem) --stages;
-    if (stages < 1 || ap.nkb > ATTN_MAX_KB) {
+    while (stages > 0 && fixed + (size_t)stages * slot > max_smem) --stages;
+    // the consumers release a slot only after the next one's MMAs are issued: the ring needs two slots
+    if (stages < 2 || ap.nkb > (keys == 256 ? AttnCfg<256>::MAX_KB : AttnCfg<128>::MAX_KB)) {
       snprintf(err, errlen, "consensus pass of %d keys does not fit shared memory", ap.nk);
       return -3;
     }
     ap.num_stages = stages;
-    const size_t smem = fixed + (size_t)stages * ATTN_SLOT_BYTES;
-    static SmemOptIn optin;
-    static int count_waits = -1;
-    if (count_waits < 0) { const char* ev = getenv("GLOM_B200_WAIT_COUNTERS"); count_waits = (ev && ev[0] == '1') ? 1 : 0; }
-    static SmemOptIn optin_cnt;
-    if (cudaError_t e = count_waits ? optin_cnt.ensure(attn_kernel<true>, smem) : optin.ensure(attn_kernel<false>, smem)) {
-      snprintf(err, errlen, "cudaFuncSetAttribute(attn): %s", cudaGetErrorString(e));
-      return -3;
-    }
+    const size_t smem = fixed + (size_t)stages * slot;
     const int ctas = ap.num_items < num_sms ? ap.num_items : num_sms;
     ProfScope scope(prof, PROF_ATTN, st);
-    cudaLaunchConfig_t acfg{};
-    acfg.gridDim = dim3(ctas); acfg.blockDim = dim3(ATTN_THREADS); acfg.dynamicSmemBytes = smem; acfg.stream = st;
-    cudaLaunchAttribute aattr[1];
-    aattr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernel
-    aattr[0].val.programmaticStreamSerializationAllowed = 1;
-    acfg.attrs = aattr; acfg.numAttrs = 1;
-    const cudaError_t e = count_waits ? cudaLaunchKernelEx(&acfg, attn_kernel<true>, mq, mk, mv, ap)
-                                      : cudaLaunchKernelEx(&acfg, attn_kernel<false>, mq, mk, mv, ap);
+    cudaError_t e;
+    if (keys == 256) e = count_waits ? launch_attn_impl<256, true>(mq, mk, mv, ap, smem, ctas, st)
+                                     : launch_attn_impl<256, false>(mq, mk, mv, ap, smem, ctas, st);
+    else e = count_waits ? launch_attn_impl<128, true>(mq, mk, mv, ap, smem, ctas, st)
+                         : launch_attn_impl<128, false>(mq, mk, mv, ap, smem, ctas, st);
     if (launches) ++*launches;
     if (e != cudaSuccess) { snprintf(err, errlen, "attn_kernel launch: %s", cudaGetErrorString(e)); return -3; }
   }
