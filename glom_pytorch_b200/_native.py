@@ -18,6 +18,7 @@ EXPORTS = (
     "glom_b200_backward", "glom_b200_backward_workspace_bytes",
     "glom_b200_tokenize_backward", "glom_b200_tokenize_backward_workspace_bytes",
     "glom_b200_clock_probe", "glom_b200_mlp_schedule", "glom_b200_islands", "glom_b200_kernel_clocks",
+    "glom_b200_settle", "glom_b200_settle_workspace_bytes",
 )
 PROFILE_KINDS = ("attention", "gemm1_gelu", "gemm2_combine", "prologue", "tokenize", "mlp_fused")
 
@@ -92,6 +93,10 @@ def load():
     lib.glom_b200_clock_probe.restype = i32
     lib.glom_b200_kernel_clocks.argtypes = [vp, vp, vp, i32, i32]
     lib.glom_b200_kernel_clocks.restype = i32
+    lib.glom_b200_settle_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, i32, ctypes.POINTER(sz)]
+    lib.glom_b200_settle_workspace_bytes.restype = i32
+    lib.glom_b200_settle.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, vp, sz, vp]
+    lib.glom_b200_settle.restype = i32
     for f in ("glom_b200_packed_weight_bytes", "glom_b200_pack_weights", "glom_b200_workspace_bytes",
               "glom_b200_workspace_offset", "glom_b200_forward", "glom_b200_tokenize"):
         getattr(lib, f).restype = i32
@@ -177,6 +182,19 @@ def forward_resume(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, out_ptr, 
     check(load().glom_b200_forward_resume(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, out_ptr, batch, iters,
                                           int(bool(return_all)), ws_ptr, ws_bytes, stream, shadow_parity, ctypes.byref(out_par)))
     return out_par.value
+
+
+def settle_workspace_bytes(cfg, batch, max_iters):
+    out = ctypes.c_size_t()
+    check(load().glom_b200_settle_workspace_bytes(ctypes.byref(cfg), batch, max_iters, ctypes.byref(out)))
+    return out.value
+
+
+def settle(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, max_iters, tol, steps_ptr,
+           ws_ptr, ws_bytes, stream):
+    """glom_b200_settle: up to max_iters steps, each image stopped on the GPU; steps_ptr -> (batch,) int32 device words."""
+    check(load().glom_b200_settle(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch,
+                                  max_iters, float(tol), steps_ptr, ws_ptr, ws_bytes, stream))
 
 
 def backward_workspace_bytes(cfg, batch):

@@ -73,6 +73,20 @@ struct WorkspaceLayout {
 };
 WorkspaceLayout workspace_layout(const Geometry& g, int precision, int iters, int return_all);
 
+// Glom.settle (bf16 engine): the forward workspace for (max_iters, return_all = 0), followed by
+struct SettleLayout {
+  WorkspaceLayout fwd;
+  size_t dsq_off;          // squared-change partials            (rows, L, nparts) f32
+  size_t flags_off;        // zeroed at the start of a call:
+  size_t frozen_off;       //   [B] int            1: the image has stopped
+  size_t block_frozen_off; //   [ceil(rows/256)]   1: every row of the 256-row block belongs to a stopped image
+  size_t done_off;         //   [1] unsigned       blocks of the convergence kernel that have finished
+  size_t level_q_off;      //   [B * L] f32        the convergence kernel's per-(image, level) ratios
+  size_t flags_bytes;
+  size_t total;
+};
+SettleLayout settle_layout(const Geometry& g, int max_iters);
+
 // ---- launchers (return cudaError_t of the launch; all asynchronous on `st`) -----------------
 struct Bf16Buffers {
   const float* s32_in;  float* s32_out;              // fp32 master state of step t / t+1
@@ -85,6 +99,10 @@ struct Bf16Buffers {
   const float* nsq_in;  float* nsq_out;
   const float* pos;                                   // (n, d) fp32
   const __nv_bfloat16* w1;  const __nv_bfloat16* w2;  const float* b1;  const float* b2;
+  // Glom.settle only (NULL for a forward): the step skips stopped images (SETTLE kernel instantiations)
+  const int* frozen;                                  // [B] 1: the image has stopped
+  const int* block_frozen;                            // [ceil(rows / 256)] 1: all rows of the block belong to stopped images
+  float* dsq_out;                                     // (rows, L, nparts) squared-change partials |S_{t+1} - S_t|^2
 };
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -109,6 +127,14 @@ size_t mlp_sched_ints(const Geometry& g);
 int mlp_schedule_dump(const Geometry& g, int num_sms, int* out, int capacity, int* num_tiles, int* delay);
 int step_bf16_mlp_fused(const Geometry& g, const Bf16Buffers& b, int* sched, EncodeTiledFn enc, int num_sms,
                         cudaStream_t st, int* launches, char* err, size_t errlen, Profiler* prof);
+
+// Glom.settle (settle_kernels.cu): the stopping rule after step `step` (one launch), and the copy of the stopped images
+// whose final state is in the workspace slab into state_out (after the last step)
+cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
+                                   int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, cudaStream_t st,
+                                   int* launches);
+cudaError_t launch_settle_gather(const Geometry& g, int max_iters, const int32_t* steps, const float* slab, float* state_out,
+                                 cudaStream_t st, int* launches);
 
 struct F32Buffers {
   const float* s_in;  float* s_out;

@@ -68,6 +68,21 @@ WorkspaceLayout workspace_layout(const Geometry& g, int precision, int iters, in
   return w;
 }
 
+SettleLayout settle_layout(const Geometry& g, int max_iters) {
+  SettleLayout s{};
+  s.fwd = workspace_layout(g, GLOM_B200_BF16, max_iters, 0);
+  size_t off = s.fwd.total;
+  s.dsq_off = off; off = align_up(off + s.fwd.nsq_bytes, 1024);
+  s.flags_off = off;
+  s.frozen_off = off; off += (size_t)g.B * 4;
+  s.block_frozen_off = off; off += (size_t)(g.rows + 255) / 256 * 4;
+  s.done_off = off; off += 4;
+  s.level_q_off = off; off += (size_t)g.B * g.L * 4;
+  s.flags_bytes = off - s.flags_off;
+  s.total = align_up(off, 1024);
+  return s;
+}
+
 static int check_cfg(const glom_b200_cfg* cfg) {
   if (!cfg) return fail(GLOM_B200_ERR_INVALID, "cfg is NULL");
   if (cfg->struct_size != sizeof(glom_b200_cfg))
@@ -195,9 +210,41 @@ GLOM_B200_API int glom_b200_workspace_offset(const glom_b200_cfg* cfg, int batch
   }
 }
 
+// glom_b200_settle: a forward of max_iters steps (return_all = 0) that stops each image at the first step whose change
+// criterion is <= tol
+struct SettleRun { float tol; int32_t* steps; };
+
 static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                         const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
-                        int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity);
+                        int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity,
+                        const SettleRun* settle = nullptr);
+
+static int check_settle(const glom_b200_cfg* cfg, int batch, int max_iters) {
+  if (int r = check_cfg(cfg)) return r;
+  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "settle: bf16 engine only (precision fp32 given)");
+  if (batch < 1) return fail(GLOM_B200_ERR_INVALID, "settle: batch must be >= 1 (got %d)", batch);
+  if (max_iters < 1) return fail(GLOM_B200_ERR_INVALID, "settle: max_iters must be >= 1 (got %d)", max_iters);
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_settle_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_iters, size_t* out_bytes) {
+  if (int r = check_settle(cfg, batch, max_iters)) return r;
+  if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
+  *out_bytes = settle_layout(make_geometry(cfg, batch), max_iters).total;
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
+                                   const float* state_in, const float* init_levels, float* state_out, int batch, int max_iters,
+                                   float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int r = check_settle(cfg, batch, max_iters)) return r;
+  if (tol != tol) return fail(GLOM_B200_ERR_INVALID, "settle: tol is NaN");
+  if (!steps_out) return fail(GLOM_B200_ERR_INVALID, "settle: steps_out is NULL");
+  if (reinterpret_cast<uintptr_t>(steps_out) % 4) return fail(GLOM_B200_ERR_INVALID, "settle: steps_out must be 4-byte aligned");
+  const SettleRun run{tol, steps_out};
+  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_iters, 0, workspace,
+                      workspace_bytes, stream, -1, &run);
+}
 
 GLOM_B200_API int glom_b200_forward(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                       const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
@@ -221,7 +268,8 @@ GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void*
 
 static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                         const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
-                        int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity) {
+                        int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity,
+                        const SettleRun* settle) {
   if (int r = check_cfg(cfg)) return r;
   if (batch < 1 || iters < 0) return fail(GLOM_B200_ERR_INVALID, "batch must be >= 1 and iters >= 0");
   if (!packed_weights || !tokens || !pos || !state_out) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
@@ -236,9 +284,11 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
   DeviceInfo di{};
   if (int r = device_info(&di)) return r;
   const Geometry g = make_geometry(cfg, batch);
-  const WorkspaceLayout wl = workspace_layout(g, cfg->precision, iters, return_all);
-  if (!workspace || workspace_bytes < wl.total)
-    return fail(GLOM_B200_ERR_WORKSPACE, "workspace: need %zu bytes, got %zu", wl.total, workspace_bytes);
+  const SettleLayout sl = settle ? settle_layout(g, iters) : SettleLayout{};
+  const WorkspaceLayout wl = settle ? sl.fwd : workspace_layout(g, cfg->precision, iters, return_all);
+  const size_t ws_need = settle ? sl.total : wl.total;
+  if (!workspace || workspace_bytes < ws_need)
+    return fail(GLOM_B200_ERR_WORKSPACE, "workspace: need %zu bytes, got %zu", ws_need, workspace_bytes);
   const PackedLayout pl = packed_layout(g.d, g.L, cfg->precision);
   const char* pw = static_cast<const char*>(packed_weights);
   char* ws = static_cast<char*>(workspace);
@@ -282,12 +332,20 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
     // list heads / dependency counters for every step are zeroed once per call.  Opt-in: the three-launch step is the
     // default path.
     const char* merged_env = getenv("GLOM_B200_MERGED_MLP");     // read per call: tests toggle it in-process
-    const bool split_mlp = !(merged_env && merged_env[0] == '1');
+    const bool split_mlp = settle || !(merged_env && merged_env[0] == '1');     // settle: always the three-launch step
     int* sched = nullptr;
     if (wl.sched_bytes && !split_mlp && iters > 0) {
       sched = reinterpret_cast<int*>(ws + wl.sched_off);
       e = cudaMemsetAsync(sched, 0, wl.sched_bytes, st);
       if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "scheduler counters memset: %s", cudaGetErrorString(e));
+    }
+    // settle: no image has stopped yet
+    int* frozen = settle ? reinterpret_cast<int*>(ws + sl.frozen_off) : nullptr;
+    int* block_frozen = settle ? reinterpret_cast<int*>(ws + sl.block_frozen_off) : nullptr;
+    float* dsq = settle ? reinterpret_cast<float*>(ws + sl.dsq_off) : nullptr;
+    if (settle) {
+      e = cudaMemsetAsync(ws + sl.flags_off, 0, sl.flags_bytes, st);
+      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle flags memset: %s", cudaGetErrorString(e));
     }
     for (int t = 0; t < iters; ++t) {
       Bf16Buffers b{};
@@ -305,10 +363,22 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
       b.w2 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w2_off);
       b.b1 = reinterpret_cast<const float*>(pw + pl.b1_off);
       b.b2 = reinterpret_cast<const float*>(pw + pl.b2_off);
+      b.frozen = frozen; b.block_frozen = block_frozen; b.dsq_out = dsq;
       char msg[400] = "";
       const int r = step_bf16(g, b, sched ? sched + (size_t)t * mlp_sched_ints(g) : nullptr, t, g_encode, di.sms, st,
                               &g_launches, msg, sizeof(msg), &g_prof);
       if (r) return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "step %d: %s", t, msg);
+      if (settle) {
+        e = launch_settle_converge(g, t + 1, settle->tol, dsq, b.nsq_out, frozen, block_frozen,
+                                   reinterpret_cast<unsigned int*>(ws + sl.done_off), reinterpret_cast<float*>(ws + sl.level_q_off),
+                                   settle->steps, st, &g_launches);
+        if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle convergence launch after step %d: %s", t, cudaGetErrorString(e));
+      }
+    }
+    // settle: image b's result S_steps[b] is in loc(steps[b]); the ones in the workspace slab move to state_out
+    if (settle) {
+      e = launch_settle_gather(g, iters, settle->steps, wslab, state_out, st, &g_launches);
+      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle gather launch: %s", cudaGetErrorString(e));
     }
   } else {
     cudaError_t e = launch_broadcast_init(g, state_in, init_levels, loc(0), st, &g_launches, &g_prof);

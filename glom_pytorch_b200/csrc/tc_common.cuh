@@ -123,9 +123,13 @@ struct K2Chunk {
   const float* s32_in; const __nv_bfloat16* c_in; const float* pos;
   float* s32_out; __nv_bfloat16* sb_out; __nv_bfloat16* sp_out;
 };
-template <bool FULL>
+// SETTLE (Glom.settle): row r of the band loads and stores nothing unless bit r of `live` is set (rows of images that
+// have stopped keep their state), and rowdsq[i] accumulates the squared change |S_{t+1} - S_t|^2 of row i * 4 + rsub
+// in the same order as rowsq.
+template <bool FULL, bool SETTLE = false>
 __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b4, uint8_t* patch, const K2Chunk& k,
-                                         int col, int lane, int rows_left, float (&rowsq)[8]) {
+                                         int col, int lane, int rows_left, float (&rowsq)[8], uint32_t live = ~0u,
+                                         float* rowdsq = nullptr) {
 #pragma unroll
   for (int c = 0; c < 8; ++c)
     *reinterpret_cast<uint4*>(patch + lane * 128 + ((c ^ (lane & 7)) << 4)) =
@@ -148,7 +152,7 @@ __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b
     for (int j = 0; j < 4; ++j) {
       const int r = (h * 4 + j) * 4 + rsub;
       sv[j] = make_float4(0.f, 0.f, 0.f, 0.f); pp[j] = sv[j]; cw[j] = make_uint2(0u, 0u);
-      if (FULL || r < rows_left) {
+      if ((FULL || r < rows_left) && (!SETTLE || ((live >> r) & 1u))) {
         sv[j] = k.s_bcast ? __ldg(reinterpret_cast<const float4*>(k.s32_in + (size_t)k.l * k.d + col + c * 4))
                           : __ldcs(reinterpret_cast<const float4*>(k.s32_in + base + (unsigned)(r * ld)));
         cw[j] = __ldcs(reinterpret_cast<const uint2*>(k.c_in + base + (unsigned)(r * ld)));
@@ -170,7 +174,14 @@ __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b
       float o3 = (sv[j].w + (acc.w + b4.w)) + __uint_as_float(cw[j].y & 0xFFFF0000u);
       if (top) { o0 = o0 / 3.0f; o1 = o1 / 3.0f; o2 = o2 / 3.0f; o3 = o3 / 3.0f; }          // (:142) IEEE division
       else { o0 *= 0.25f; o1 *= 0.25f; o2 *= 0.25f; o3 *= 0.25f; }                          // x/4 == x*0.25 exactly
-      if (FULL || r < rows_left) {
+      const bool store = (FULL || r < rows_left) && (!SETTLE || ((live >> r) & 1u));
+      if constexpr (SETTLE) {
+        // rows that store nothing contribute no change (and, below, no norm)
+        const float e0 = store ? o0 - sv[j].x : 0.f, e1 = store ? o1 - sv[j].y : 0.f;
+        const float e2 = store ? o2 - sv[j].z : 0.f, e3 = store ? o3 - sv[j].w : 0.f;
+        rowdsq[i] += row_chunk_sumsq(e0, e1, e2, e3);
+      }
+      if (store) {
         const size_t o = base + (unsigned)(r * ld);
         __stcs(reinterpret_cast<float4*>(k.s32_out + o), make_float4(o0, o1, o2, o3));
         *reinterpret_cast<uint2*>(k.sb_out + o) = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));

@@ -70,6 +70,10 @@ struct GemmParams {
   int h_keep_z;     // K1: H blocks of groups <= h_keep_z are stored with the default L2 policy instead of evict-first
   int h_load_policy; // K2: L2 hint of the H loads (GLOM_B200_K2_HPOL, default 0 = evict-first on every load)
   int epi_prefetch; // K2: L2 prefetch of the epilogue's state / consensus lines at tile start (GLOM_B200_K2_EPI_PREFETCH, default on)
+  // SETTLE instantiations (Glom.settle), flags written by the convergence kernel of the previous step
+  const int* frozen;        // [B] 1: the image has stopped
+  const int* block_frozen;  // [num_m] 1: every row of the 256-row block belongs to a stopped image
+  float* dsq_out;           // K2: squared-change partials |S_{t+1} - S_t|^2, laid out like nsq_out
 };
 
 template <int MODE, int BN>
@@ -159,7 +163,10 @@ __device__ __forceinline__ void tok_chunk(const uint32_t (&v)[32], const float4 
   __syncwarp();
 }
 
-template <int MODE, int BN, bool CNT>
+// SETTLE (K1 / K2 of Glom.settle): tiles of 256-row blocks whose images have all stopped are skipped by every warp role
+// of both CTAs (the same flag, written by an earlier launch and read after pdl_wait, keeps the multicast and empty-barrier
+// protocol in step); K2 stores nothing for rows of stopped images and also writes the squared-change partials.
+template <int MODE, int BN, bool CNT, bool SETTLE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows, d)        K2: H (rows, G*4d)
             const __grid_constant__ CUtensorMap map_a1,   // K1: state shadow Sb (rows, L*d)
@@ -242,6 +249,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
       };
       for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
         const TileInfo t = decode_tile<MODE>(p, tile);
+        if constexpr (SETTLE) { if (p.block_frozen[t.m_blk]) continue; }
         const CUtensorMap* amap;
         int a_col, b_row;
         if (MODE == 0) {
@@ -318,8 +326,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
     float acc[BN / 2];
     for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
       const TileInfo t = decode_tile<MODE>(p, tile);
+      if constexpr (SETTLE) { if (p.block_frozen[t.m_blk]) continue; }
       const int row0 = t.m_blk * 256 + cta_rank * BM + pair * 32;     // first row of this warp pair's 32-row band
       const int rows_left = p.rows - row0;                              // >= 32: whole band valid (warp-uniform)
+      uint32_t live = ~0u;                                              // SETTLE, K2: bit r = row row0 + r is stored
+      if constexpr (SETTLE && MODE == 1)
+        live = __ballot_sync(0xffffffffu, row0 + lane < p.rows && !p.frozen[(row0 + lane) / p.n]);
       if (MODE == 1 && p.epi_prefetch && lane < rows_left) {
         // The combine reads this band's fp32 state and C lines: pull them into L2 before the main loop, so the epilogue's
         // dependent global loads hit L2 instead of paying the HBM latency
@@ -414,34 +426,49 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
             kc.s32_out = p.s32_out; kc.sb_out = p.sb_out; kc.sp_out = p.sp_out;
             const int col = t.n_blk * BN + cc;
             const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + (size_t)t.z * p.d + col + (lane & 7) * 4));
-            float rowsq[8];
+            float rowsq[8], rowdsq[8];
 #pragma unroll
-            for (int i = 0; i < 8; ++i) rowsq[i] = 0.f;
-            if (rows_left >= 32) k2_chunk<true>(v, b4, patch, kc, col, lane, 32, rowsq);
-            else k2_chunk<false>(v, b4, patch, kc, col, lane, rows_left, rowsq);
+            for (int i = 0; i < 8; ++i) rowsq[i] = rowdsq[i] = 0.f;
+            if (rows_left >= 32) k2_chunk<true, SETTLE>(v, b4, patch, kc, col, lane, 32, rowsq, live, rowdsq);
+            else k2_chunk<false, SETTLE>(v, b4, patch, kc, col, lane, rows_left, rowsq, live, rowdsq);
             // one squared-norm partial per PART_COLS columns: with 64-column parts the two warps of the pair hold the two
-            // 32-column halves, summed in chunk order (0 + first) + second as in prep_state_kernel
+            // 32-column halves, summed in chunk order (0 + first) + second as in prep_state_kernel.  SETTLE: the
+            // squared changes take the same exchange through the second warp's transpose patch, which k2_chunk no
+            // longer reads and which the pair barrier at the end of the step frees again
             int part = cc / Cfg::PART_COLS;
             bool writer = true;
             if (Cfg::PART_COLS == 64) {
+              float* dxch = reinterpret_cast<float*>(patches + (size_t)(cw | 1) * Cfg::PATCH_BYTES);
               if (x == 1 && (lane & 7) == 0) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i) xch_p[i * 4 + (lane >> 3)] = rowsq[i];
+                if constexpr (SETTLE) {
+#pragma unroll
+                  for (int i = 0; i < 8; ++i) dxch[i * 4 + (lane >> 3)] = rowdsq[i];
+                }
               }
               named_bar_sync(1 + pair, 64);
               if (x == 0) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i) rowsq[i] += xch_p[i * 4 + (lane >> 3)];
+                if constexpr (SETTLE) {
+#pragma unroll
+                  for (int i = 0; i < 8; ++i) rowdsq[i] += dxch[i * 4 + (lane >> 3)];
+                }
               }
               writer = x == 0;
             }
             if (writer && (lane & 7) == 0) {
-              float* nsq = p.nsq_out + ((size_t)row0 * p.L + t.z) * p.nparts + t.n_blk * Cfg::PARTS + part;
+              const size_t po = ((size_t)row0 * p.L + t.z) * p.nparts + t.n_blk * Cfg::PARTS + part;
+              float* nsq = p.nsq_out + po;
               const int ldn = p.L * p.nparts;   // row offsets r * ldn (r < 32) in 32 bits: half the registers once hoisted
 #pragma unroll
               for (int i = 0; i < 8; ++i) {
                 const int r = i * 4 + (lane >> 3);
-                if (r < rows_left) nsq[(unsigned)(r * ldn)] = rowsq[i];
+                if (r < rows_left && (!SETTLE || ((live >> r) & 1u))) {
+                  nsq[(unsigned)(r * ldn)] = rowsq[i];
+                  if constexpr (SETTLE) p.dsq_out[po + (unsigned)(r * ldn)] = rowdsq[i];
+                }
               }
             }
           }
@@ -513,6 +540,7 @@ struct AttnParams {
   int key0, nk, pass_first, pass_last;
   float* o_acc;                        // (rows, L, d) fp32
   float* ml_acc;                       // (rows, L, 2) fp32: stabiliser (log2 units), row sum
+  const int* frozen;                   // SETTLE: [B] 1 = the image has stopped, its items are skipped
 };
 
 // shared-memory bytes of a pass: P (nchunk x [128 x 64] bf16), the ring, two scale buffers (rs, bnd) + key coordinates,
@@ -539,7 +567,9 @@ __device__ __forceinline__ float attn_row_norm(const float* ns, int nparts) {
   return sqrtf(ss);
 }
 
-template <int KEYS, bool CNT>
+// SETTLE (Glom.settle): the items of stopped images are skipped by all three roles (TMA warp, scale warps, consumers),
+// which read the same flag after pdl_wait; the scale-buffer sequence number k counts processed items only.
+template <int KEYS, bool CNT, bool SETTLE = false>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64, 128, 1)
             const __grid_constant__ CUtensorMap map_k,    // box (64, KEYS, 1)
@@ -599,6 +629,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
       const uint32_t stages0 = smem_u32(stages);
       for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
         const int b = it / per_img, l = (it % per_img) / p.ntiles;
+        if constexpr (SETTLE) { if (p.frozen[b]) continue; }
         const int q0 = (it % p.ntiles) * BM;
         for (int kb = 0; kb < nkb; ++kb) {
           for (int dc = 0; dc < p.d / BK; ++dc) {
@@ -642,8 +673,9 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
         key_hw[j] = j >= p.nk ? (20000u << 16)
                               : use_mask ? ((uint32_t)((p.key0 + j) / p.mask_side) << 16) | (uint32_t)((p.key0 + j) % p.mask_side) : 0u;
       int k = 0;
-      for (int it = blockIdx.x; it < p.num_items; it += gridDim.x, ++k) {
+      for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
         const int b = it / per_img, l = (it % per_img) / p.ntiles;
+        if constexpr (SETTLE) { if (p.frozen[b]) continue; }
         const size_t img_row0 = (size_t)b * p.n;
         const int buf = k & 1;
         mbar_wait(&sc_empty[buf], ((k >> 1) & 1) ^ 1);
@@ -663,6 +695,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&sc_full[buf]);
+        ++k;
       }
     }
   } else {
@@ -697,8 +730,9 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
     };
 
     int k = 0;
-    for (int it = blockIdx.x; it < p.num_items; it += gridDim.x, ++k) {
+    for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
       const int b = it / per_img, l = (it % per_img) / p.ntiles;
+      if constexpr (SETTLE) { if (p.frozen[b]) continue; }
       const int q0 = (it % p.ntiles) * BM;
       const size_t img_row0 = (size_t)b * p.n;
       const long long cnt_t0 = cnt_cta ? clock64() : 0;
@@ -963,6 +997,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
         }
       }
       if (cnt_cta) w2 += (unsigned long long)(clock64() - cnt_t1) - (w0 - cnt_w1);          // output work
+      ++k;
     }
     if (cnt_cta && cw == 0 && lane == 0) { atomicAdd(&cnt[5], w0); atomicAdd(&cnt[6], w1); atomicAdd(&cnt[7], w2); }
   }
@@ -985,13 +1020,17 @@ cudaError_t tc_kernel_clocks(unsigned long long* out /* [PROF_KINDS][8] */, bool
 // =====================================================================================
 // Host side: tensor maps + launches for one Jacobi step
 // =====================================================================================
-template <int MODE, int BN, bool CNT>
+template <int MODE, int BN, bool CNT, bool SETTLE = false>
 static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& bm,
                                     const CUtensorMap& out, const GemmParams& p, int num_sms, cudaStream_t st);
 
 template <int MODE, int BN>
 static cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& bm,
                                const CUtensorMap& out, const GemmParams& p, int num_sms, cudaStream_t st) {
+  // Glom.settle: the instantiation that skips stopped images (no wait-counting variant)
+  if constexpr (MODE != 2) {
+    if (p.block_frozen) return launch_gemm_impl<MODE, BN, false, true>(a0, a1, a2, bm, out, p, num_sms, st);
+  }
   // GLOM_B200_WAIT_COUNTERS=1 (diagnostics): the instantiation whose block 0 accumulates its roles' wait cycles
   static int count_waits = -1;
   if (count_waits < 0) { const char* ev = getenv("GLOM_B200_WAIT_COUNTERS"); count_waits = (ev && ev[0] == '1') ? 1 : 0; }
@@ -999,12 +1038,12 @@ static cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, con
   return launch_gemm_impl<MODE, BN, false>(a0, a1, a2, bm, out, p, num_sms, st);
 }
 
-template <int MODE, int BN, bool CNT>
+template <int MODE, int BN, bool CNT, bool SETTLE>
 static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& bm,
                                     const CUtensorMap& out, const GemmParams& p, int num_sms, cudaStream_t st) {
   using Cfg = GemmCfg<MODE, BN>;
   static SmemOptIn optin;
-  if (cudaError_t e = optin.ensure(gemm_kernel<MODE, BN, CNT>, Cfg::SMEM_BYTES)) return e;
+  if (cudaError_t e = optin.ensure(gemm_kernel<MODE, BN, CNT, SETTLE>, Cfg::SMEM_BYTES)) return e;
   cudaLaunchConfig_t cfg{};
   cfg.blockDim = dim3(Cfg::THREADS);
   cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
@@ -1021,28 +1060,28 @@ static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1
     cfg.gridDim = dim3(2 * (num_sms / 2));
     cfg.attrs = &attr[1]; cfg.numAttrs = 1;
     int n = 0;
-    if (cudaError_t e = cudaOccupancyMaxActiveClusters(&n, gemm_kernel<MODE, BN, CNT>, &cfg)) return e;
+    if (cudaError_t e = cudaOccupancyMaxActiveClusters(&n, gemm_kernel<MODE, BN, CNT, SETTLE>, &cfg)) return e;
     if (n < 1) return cudaErrorInvalidConfiguration;
     max_pairs = n < num_sms / 2 ? n : num_sms / 2;
   }
   cfg.attrs = attr; cfg.numAttrs = 2;
   const int pairs = p.num_tiles < max_pairs ? p.num_tiles : max_pairs;
   cfg.gridDim = dim3(2 * pairs);
-  return cudaLaunchKernelEx(&cfg, gemm_kernel<MODE, BN, CNT>, a0, a1, a2, bm, out, p);
+  return cudaLaunchKernelEx(&cfg, gemm_kernel<MODE, BN, CNT, SETTLE>, a0, a1, a2, bm, out, p);
 }
 
-template <int KEYS, bool CNT>
+template <int KEYS, bool CNT, bool SETTLE = false>
 static cudaError_t launch_attn_impl(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& ap,
                                     size_t smem, int ctas, cudaStream_t st) {
   static SmemOptIn optin;
-  if (cudaError_t e = optin.ensure(attn_kernel<KEYS, CNT>, smem)) return e;
+  if (cudaError_t e = optin.ensure(attn_kernel<KEYS, CNT, SETTLE>, smem)) return e;
   cudaLaunchConfig_t acfg{};
   acfg.gridDim = dim3(ctas); acfg.blockDim = dim3(ATTN_THREADS); acfg.dynamicSmemBytes = smem; acfg.stream = st;
   cudaLaunchAttribute aattr[1];
   aattr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernel
   aattr[0].val.programmaticStreamSerializationAllowed = 1;
   acfg.attrs = aattr; acfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&acfg, attn_kernel<KEYS, CNT>, mq, mk, mv, ap);
+  return cudaLaunchKernelEx(&acfg, attn_kernel<KEYS, CNT, SETTLE>, mq, mk, mv, ap);
 }
 
 // K3: consensus attention -> C
@@ -1088,6 +1127,7 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiled
     ap.scale = 1.0f / sqrtf((float)d);
     ap.ntiles = (n + BM - 1) / BM;
     ap.num_items = ap.ntiles * L * g.B;
+    ap.frozen = b.frozen;
     // 256 keys: 3 slots of 48 KB next to 64 KB of P (n = 256: 219,392 B); 128 keys: 2 slots of 32 KB at 576 keys
     const uint32_t slot = keys == 256 ? AttnCfg<256>::SLOT_BYTES : AttnCfg<128>::SLOT_BYTES;
     const size_t fixed = attn_fixed_smem(ap.nchunk, ap.n_pad16);
@@ -1104,8 +1144,10 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiled
     const int ctas = ap.num_items < num_sms ? ap.num_items : num_sms;
     ProfScope scope(prof, PROF_ATTN, st);
     cudaError_t e;
-    if (keys == 256) e = count_waits ? launch_attn_impl<256, true>(mq, mk, mv, ap, smem, ctas, st)
-                                     : launch_attn_impl<256, false>(mq, mk, mv, ap, smem, ctas, st);
+    if (b.frozen) e = keys == 256 ? launch_attn_impl<256, false, true>(mq, mk, mv, ap, smem, ctas, st)
+                                  : launch_attn_impl<128, false, true>(mq, mk, mv, ap, smem, ctas, st);
+    else if (keys == 256) e = count_waits ? launch_attn_impl<256, true>(mq, mk, mv, ap, smem, ctas, st)
+                                          : launch_attn_impl<256, false>(mq, mk, mv, ap, smem, ctas, st);
     else e = count_waits ? launch_attn_impl<128, true>(mq, mk, mv, ap, smem, ctas, st)
                          : launch_attn_impl<128, false>(mq, mk, mv, ap, smem, ctas, st);
     if (launches) ++*launches;
@@ -1155,6 +1197,7 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int* sched, int step_inde
     p.h_keep_z = (k1_order >> 1) - 1;
     p.num_m = (rows + 255) / 256; p.num_n = 4 * d / 256; p.num_tiles = (g.G - p.z0) * p.num_m * p.num_n;
     p.bias = b.b1; p.m128 = m128;
+    p.frozen = b.frozen; p.block_frozen = b.block_frozen;
     ProfScope scope(prof, PROF_GEMM1, st);
     cudaError_t e = launch_gemm<0, 256>(mx, msb, msp, mw1, mh_out, p, num_sms, st);
     if (launches) ++*launches;
@@ -1171,6 +1214,7 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int* sched, int step_inde
     p.m128 = m128;
     p.bias = b.b2; p.s32_in = b.s32_in; p.s_bcast = b.s32_in_bcast; p.c_in = b.c; p.pos = b.pos;
     p.s32_out = b.s32_out; p.sb_out = b.sb_out; p.sp_out = b.sp_out; p.nsq_out = b.nsq_out; p.nparts = g.nparts;
+    p.frozen = b.frozen; p.block_frozen = b.block_frozen; p.dsq_out = b.dsq_out;
     static int h_pf = -1;
     if (h_pf < 0) { const char* ev = getenv("GLOM_B200_K2_PREFETCH"); h_pf = ev ? atoi(ev) : 0; }
     p.h_prefetch = h_pf;

@@ -467,3 +467,59 @@ class Glom(nn.Module):
         pos = self.pos_emb.weight[:n]                                                            # (:117)
         state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
         return _ColumnUpdate.apply(self, iters, return_all, tokens, pos, state0, self.init_levels, *self._mlp_params())
+
+    # ------------------------------------------------------------------ inference until the columns settle
+    def settle(self, img, tol, max_iters=None, levels=None):
+        """Run each image's column update until its levels stop changing -> ``(levels, steps)``.
+
+        After step k the change of image b is ``max_l sqrt(sum_i |S_k[b,i,l] - S_{k-1}[b,i,l]|^2 / sum_i |S_k[b,i,l]|^2)``
+        (sums over the image's columns, fp32); the first k where it is ``<= tol`` stops the image.  ``levels[b]`` is then
+        S_k, bit-identical to ``forward(img, iters=k, levels=same_start)[b]`` on the same batch, and ``steps[b] = k``.
+        Images that never meet the rule run ``max_iters`` steps (``None`` = 2L as in ``forward``).  The stopping decisions
+        are taken on the GPU inside the call: ``steps`` is a (B,) int32 CUDA tensor the host never reads, so the call does
+        not synchronise.  Inference only (raises if autograd would be needed), bf16 engine only."""
+        if self.precision != "bf16":
+            raise RuntimeError("Glom.settle needs precision='bf16' (the fp32 engine has no early stopping)")
+        if not img.is_cuda:
+            raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
+                               "move the module and inputs to an H100")
+        if torch.is_grad_enabled() and (img.requires_grad or (levels is not None and levels.requires_grad)
+                                        or any(p.requires_grad for p in self.parameters())):
+            raise RuntimeError("Glom.settle is inference only: call it under torch.no_grad() / torch.inference_mode() "
+                               "or with parameters and inputs that do not require grad")
+        max_iters = self.levels * 2 if max_iters is None else int(max_iters)
+        if max_iters < 1:
+            raise ValueError(f"max_iters must be >= 1, got {max_iters}")
+        tol = float(tol)
+        if tol != tol:
+            raise ValueError("tol is NaN")
+        b, p = img.shape[0], self.patch_size
+        if img.dim() != 4 or img.shape[1] != 3 or img.shape[2] % p or img.shape[3] % p:
+            raise RuntimeError(f"image {tuple(img.shape)} is not (B, 3, H, W) with H, W multiples of {p}")
+        n = (img.shape[2] // p) * (img.shape[3] // p)
+        if n > self.pos_emb.num_embeddings:
+            raise IndexError(f"{n} patches exceed pos_emb size {self.pos_emb.num_embeddings}")
+        if levels is not None and tuple(levels.shape) != (b, n, self.levels, self.dim):
+            raise RuntimeError(f"levels must have shape {(b, n, self.levels, self.dim)}, got {tuple(levels.shape)}")
+        tokens = self._take_staged(img)
+        if tokens is None:
+            tokens = self.tokens(img)
+        device = tokens.device
+        # the workspace shadows of stopped images are stale: the next forward must take the ordinary state prologue
+        self._resume = None
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            tokens = tokens.detach().to(torch.float32).contiguous()
+            pos = self.pos_emb.weight[:n].detach().to(torch.float32).contiguous()
+            init = self.init_levels.detach().to(torch.float32).contiguous()
+            state_in = None if levels is None else levels.detach().to(device=device, dtype=torch.float32).contiguous()
+            cfg = self.engine_cfg(n)
+            packed = self._packed_weights(cfg, device, stream)
+            out = torch.empty((b, n, self.levels, self.dim), dtype=torch.float32, device=device)
+            steps = torch.empty(b, dtype=torch.int32, device=device)
+            ws = self._get_workspace(_native.settle_workspace_bytes(cfg, b, max_iters), device)
+            _native.settle(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(),
+                           None if state_in is None else state_in.data_ptr(), init.data_ptr(), out.data_ptr(), b,
+                           max_iters, tol, steps.data_ptr(), ws.data_ptr(), ws.numel(), stream)
+            self.last_launches = _native.last_launch_count() + getattr(self, "_tok_launches", 0)
+        return out, steps

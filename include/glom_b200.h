@@ -119,6 +119,24 @@ GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void*
                                            int return_all, void* workspace, size_t workspace_bytes, void* stream,
                                            int shadow_parity, int* out_shadow_parity);
 
+/* Inference until the columns settle (Glom.settle).  bf16 engine only.  Runs up to `max_iters` (>= 1) steps from the same
+ * start as glom_b200_forward (state_in, or init_levels broadcast) and stops each image on its own, on the GPU and without
+ * a host synchronisation.  After step k (k >= 1) image b has
+ *   r_b(k) = max_l sqrt( sum_i |S_k[b,i,l] - S_{k-1}[b,i,l]|^2 / sum_i |S_k[b,i,l]|^2 )
+ * (sums over the image's n columns, fp32, fixed order; 0/0 counts as 0, x/0 with x > 0 as inf).  The first k with
+ * r_b(k) <= tol stops image b: state_out[b] = S_k and steps_out[b] = k.  An image that never meets it gets S_max_iters and
+ * steps_out[b] = max_iters; a negative tol never stops an image.  state_out[b] is bit-identical to
+ * glom_b200_forward(iters = steps_out[b]) on the same batch.
+ *   state_out (B, n, L, d) fp32, must not alias state_in;  steps_out (B) int32, device memory, written on `stream`.
+ * Later steps skip the stopped images' work (their launches stay enqueued).  NaN tol, max_iters < 1, precision fp32 and a
+ * NULL steps_out are errors.  The workspace (1024-byte aligned) is the forward workspace for (batch, max_iters) plus the
+ * stopping rule's partials and flags; a following glom_b200_forward_resume on it is not valid. */
+GLOM_B200_API int glom_b200_settle_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_iters, size_t* out_bytes);
+GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
+                                   const float* state_in, const float* init_levels, float* state_out, int batch,
+                                   int max_iters, float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes,
+                                   void* stream);
+
 /* Tokeniser, the step before the loop: replaces image_to_tokens
  * (glom_pytorch.py:94-97, call :114): patchify 'b c (h p1) (w p2) -> b (h w) (p1 p2 c)'
  * fused with the Linear(3*p*p -> d).
