@@ -19,6 +19,7 @@ EXPORTS = (
     "glom_b200_tokenize_backward", "glom_b200_tokenize_backward_workspace_bytes",
     "glom_b200_clock_probe", "glom_b200_mlp_schedule", "glom_b200_islands", "glom_b200_kernel_clocks",
     "glom_b200_settle", "glom_b200_settle_workspace_bytes",
+    "glom_b200_forward_steps", "glom_b200_forward_steps_workspace_bytes", "glom_b200_backward_steps",
 )
 PROFILE_KINDS = ("attention", "gemm1_gelu", "gemm2_combine", "prologue", "tokenize", "mlp_fused")
 
@@ -97,6 +98,13 @@ def load():
     lib.glom_b200_settle_workspace_bytes.restype = i32
     lib.glom_b200_settle.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, vp, sz, vp]
     lib.glom_b200_settle.restype = i32
+    lib.glom_b200_forward_steps_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, i32, i32, ctypes.POINTER(sz)]
+    lib.glom_b200_forward_steps_workspace_bytes.restype = i32
+    lib.glom_b200_forward_steps.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, vp, i32, i32, vp, sz, vp]
+    lib.glom_b200_forward_steps.restype = i32
+    lib.glom_b200_backward_steps.argtypes = [ctypes.POINTER(Cfg), ctypes.POINTER(WeightsRef), vp, vp, vp, vp,
+                                             ctypes.POINTER(Grads), i32, vp, i32, i32, vp, sz, vp]
+    lib.glom_b200_backward_steps.restype = i32
     for f in ("glom_b200_packed_weight_bytes", "glom_b200_pack_weights", "glom_b200_workspace_bytes",
               "glom_b200_workspace_offset", "glom_b200_forward", "glom_b200_tokenize"):
         getattr(lib, f).restype = i32
@@ -195,6 +203,31 @@ def settle(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr
     """glom_b200_settle: up to max_iters steps, each image stopped on the GPU; steps_ptr -> (batch,) int32 device words."""
     check(load().glom_b200_settle(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch,
                                   max_iters, float(tol), steps_ptr, ws_ptr, ws_bytes, stream))
+
+
+def forward_steps_workspace_bytes(cfg, batch, max_steps, return_all):
+    out = ctypes.c_size_t()
+    check(load().glom_b200_forward_steps_workspace_bytes(ctypes.byref(cfg), batch, max_steps, int(bool(return_all)),
+                                                         ctypes.byref(out)))
+    return out.value
+
+
+def forward_steps(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, steps_ptr, max_steps,
+                  return_all, ws_ptr, ws_bytes, stream):
+    """glom_b200_forward_steps: image b runs steps[b] steps (steps_ptr -> (batch,) int32 device words, clamped on the
+    device to [0, max_steps])."""
+    check(load().glom_b200_forward_steps(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr,
+                                         batch, steps_ptr, max_steps, int(bool(return_all)), ws_ptr, ws_bytes, stream))
+
+
+def backward_steps(cfg, weight_ptrs, tokens_ptr, pos_ptr, states_ptr, grad_out_ptr, grad_ptrs, batch, steps_ptr, max_steps,
+                   grad_all, ws_ptr, ws_bytes, stream):
+    """glom_b200_backward_steps: the backward of forward_steps(return_all=1); arguments as for backward()."""
+    w = WeightsRef(ctypes.sizeof(WeightsRef), *weight_ptrs)
+    g = Grads(ctypes.sizeof(Grads), *[grad_ptrs.get(k) for k, _ in Grads._fields_[1:]])
+    check(load().glom_b200_backward_steps(ctypes.byref(cfg), ctypes.byref(w), tokens_ptr, pos_ptr, states_ptr,
+                                          grad_out_ptr, ctypes.byref(g), batch, steps_ptr, max_steps, int(grad_all),
+                                          ws_ptr, ws_bytes, stream))
 
 
 def backward_workspace_bytes(cfg, batch):

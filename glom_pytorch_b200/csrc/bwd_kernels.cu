@@ -100,14 +100,22 @@ static cudaError_t gemm_f32(const GemmF32& q, int batches, cudaStream_t st, int*
 // =====================================================================================
 // g (R, L, d)  <-  (gin + extra) (R, L, d) / c_l   (:142);   ds (R, L, d) <- g (residual term of the sum, :141)
 // `extra` (nullable) is the upstream gradient of this time step's own output when every step is returned (:147-148)
+// steps (nullable): per-image step counts; an image with steps[b] <= t is the identity at step t, so its rows get
+// g = 0 (every later contribution of theirs is an exact zero) and ds = gin + extra unscaled
 __global__ void scale_by_contrib_kernel(size_t total, int L, int d, const float* __restrict__ gin,
-                                        const float* __restrict__ extra, float* __restrict__ g, float* __restrict__ ds) {
+                                        const float* __restrict__ extra, float* __restrict__ g, float* __restrict__ ds,
+                                        const int32_t* __restrict__ steps, int t, size_t img4) {
   const size_t total4 = total / 4;
   const unsigned d4 = (unsigned)d / 4;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (size_t)gridDim.x * blockDim.x) {
     const unsigned l = (unsigned)((i / d4) % (unsigned)L);
     float4 v = reinterpret_cast<const float4*>(gin)[i];
     if (extra) { const float4 e = reinterpret_cast<const float4*>(extra)[i]; v.x += e.x; v.y += e.y; v.z += e.z; v.w += e.w; }
+    if (steps && __ldg(steps + i / img4) <= t) {
+      reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      reinterpret_cast<float4*>(ds)[i] = v;
+      continue;
+    }
     if (l == (unsigned)L - 1) { v.x /= 3.0f; v.y /= 3.0f; v.z /= 3.0f; v.w /= 3.0f; }
     else { v.x *= 0.25f; v.y *= 0.25f; v.z *= 0.25f; v.w *= 0.25f; }
     reinterpret_cast<float4*>(g)[i] = v;
@@ -403,7 +411,7 @@ BackwardLayout backward_layout(const Geometry& g, int precision) {
 // accumulate parameter / token / pos gradients.
 static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const float* s_t, const float* gin,
                                  const float* gextra, float* ds, char* ws, const BackwardLayout& wl, bool mlp_on_tc,
-                                 bool attn_on_tc, cudaStream_t st, int* launches) {
+                                 bool attn_on_tc, const int32_t* steps, int t, cudaStream_t st, int* launches) {
   const int R = g.rows, L = g.L, d = g.d, n = g.n, h4 = 4 * g.d;
   const long long ld = (long long)L * d;
   float* gs = reinterpret_cast<float*>(ws + wl.gs_off);       // (gin + gextra) / c
@@ -413,7 +421,7 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
   float* xp = reinterpret_cast<float*>(ws + wl.xp_off);
   float* dx = reinterpret_cast<float*>(ws + wl.dx_off);
   const size_t state = (size_t)R * L * d;
-  scale_by_contrib_kernel<<<nblk(state), 256, 0, st>>>(state, L, d, gin, gextra, gs, ds);
+  scale_by_contrib_kernel<<<nblk(state), 256, 0, st>>>(state, L, d, gin, gextra, gs, ds, steps, t, (size_t)n * ld / 4);
   CKL();
 
   // ---- the two grouped MLPs (:23-36), one group at a time (fp32 path; the bf16 engine runs them on tensor cores)
@@ -566,8 +574,8 @@ __global__ void bwd_shadows_kernel(int rows, int n, int L, int d, const float* _
   }
 }
 
-int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int iters, int grad_all, void* workspace,
-                 EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen) {
+int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int iters, int grad_all, const int32_t* steps,
+                 void* workspace, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen) {
 #define CKI(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { snprintf(err, errlen, "backward: %s", cudaGetErrorString(e_)); return -3; } } while (0)
 #define CKLI() do { if (launches) ++*launches; CKI(cudaGetLastError()); } while (0)
   const BackwardLayout wl = backward_layout(g, precision);
@@ -613,7 +621,7 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
   for (int t = iters - 1, k = 0; t >= 0; --t, ++k) {
     const float* s_t = a.states + (size_t)t * state;
     float* ds = slab[k & 1];
-    CKI(backward_step(g, a, s_t, gin, gextra, ds, ws, wl, tc, attn_tc, st, launches));   // scale (+ the fp32 MLP / attention backward)
+    CKI(backward_step(g, a, s_t, gin, gextra, ds, ws, wl, tc, attn_tc, steps, t, st, launches));   // scale (+ the fp32 MLP / attention backward)
     if (tc) {
       bwd_shadows_kernel<<<nblk(state / 4), 256, 0, st>>>(g.rows, g.n, g.L, g.d, s_t, gs, a.pos,
                                                           const_cast<__nv_bfloat16*>(m.sb), const_cast<__nv_bfloat16*>(m.sp),
@@ -649,6 +657,7 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
         CKLI();
       }
       m.ds = ds;
+      m.steps = steps; m.t = t;
       if (int r = mlp_backward_tc(g, m, enc, num_sms, st, launches, err, errlen)) return r;
       colsum_acc_kernel<<<dim3((g.L * g.d + 31) / 32, 16), 256, 0, st>>>(g.rows, g.L * g.d, (long long)g.L * g.d, gs, a.d_bu_b2,
                                                                          a.d_td_b2, (g.L - 1) * g.d);

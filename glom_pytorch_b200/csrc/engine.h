@@ -73,7 +73,8 @@ struct WorkspaceLayout {
 };
 WorkspaceLayout workspace_layout(const Geometry& g, int precision, int iters, int return_all);
 
-// Glom.settle (bf16 engine): the forward workspace for (max_iters, return_all = 0), followed by
+// Glom.settle and the per-image step counts of glom_b200_forward_steps (bf16 engine): the forward workspace for
+// (max_iters, return_all; settle: return_all = 0), followed by
 struct SettleLayout {
   WorkspaceLayout fwd;
   size_t dsq_off;          // squared-change partials            (rows, L, nparts) f32
@@ -85,7 +86,7 @@ struct SettleLayout {
   size_t flags_bytes;
   size_t total;
 };
-SettleLayout settle_layout(const Geometry& g, int max_iters);
+SettleLayout settle_layout(const Geometry& g, int max_iters, int return_all = 0);
 
 // ---- launchers (return cudaError_t of the launch; all asynchronous on `st`) -----------------
 struct Bf16Buffers {
@@ -133,8 +134,17 @@ int step_bf16_mlp_fused(const Geometry& g, const Bf16Buffers& b, int* sched, Enc
 cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
                                    int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, cudaStream_t st,
                                    int* launches);
+// s0 (nullable): where S_0 is when no step materialised it (the carried state, or init_levels broadcast if s0_bcast);
+// images with steps[b] == 0 are copied from there
 cudaError_t launch_settle_gather(const Geometry& g, int max_iters, const int32_t* steps, const float* slab, float* state_out,
-                                 cudaStream_t st, int* launches);
+                                 const float* s0, int s0_bcast, cudaStream_t st, int* launches);
+// glom_b200_forward_steps (settle_kernels.cu): the flags of step t from the given step counts (clamped to [0, max_steps]),
+// one launch before every step; and, for return_all, the copy of slab steps[b] of each image into its slabs
+// steps[b]+1 .. max_steps (after the last step)
+cudaError_t launch_steps_schedule(const Geometry& g, int t, int max_steps, const int32_t* steps, int* frozen, int* block_frozen,
+                                  cudaStream_t st, int* launches);
+cudaError_t launch_steps_fill(const Geometry& g, int max_steps, const int32_t* steps, float* states, cudaStream_t st,
+                              int* launches);
 
 struct F32Buffers {
   const float* s_in;  float* s_out;
@@ -199,6 +209,10 @@ struct MlpBwdTc {
                                                // dL/dS_t (R, L, d), dL/dtokens (R, d), dL/dpos (n, d)
   float *d_bu_w1, *d_bu_w2, *d_td_w1, *d_td_w2;
   float *d_bu_b1, *d_td_b1;                    // first-layer bias gradients, reduced in the DH epilogue
+  // per-image step counts (glom_b200_backward_steps; NULL = every image runs every step): rows of images with
+  // steps[b] <= t have gs = 0 at reverse step t, so row blocks made only of such rows are skipped
+  const int32_t* steps;
+  int t;
 };
 int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches,
                     char* err, size_t errlen);
@@ -214,8 +228,9 @@ BackwardLayout backward_layout(const Geometry& g, int precision);
 size_t tokenize_backward_workspace_bytes(int B, int H, int W, int p, int need_dimg);
 cudaError_t tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight, float* d_bias,
                               float* d_img, int B, int H, int W, int p, int d, void* workspace, cudaStream_t st, int* launches);
-int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int iters, int grad_all, void* workspace,
-                 EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen);
+// steps (nullable, device memory): per-image step counts; image b is the identity at every reverse step t >= steps[b]
+int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int iters, int grad_all, const int32_t* steps,
+                 void* workspace, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen);
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per device and per function: remember, per device, the
 // largest size already configured for one kernel (one instance of this per kernel template instantiation).

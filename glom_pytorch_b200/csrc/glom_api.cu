@@ -68,9 +68,9 @@ WorkspaceLayout workspace_layout(const Geometry& g, int precision, int iters, in
   return w;
 }
 
-SettleLayout settle_layout(const Geometry& g, int max_iters) {
+SettleLayout settle_layout(const Geometry& g, int max_iters, int return_all) {
   SettleLayout s{};
-  s.fwd = workspace_layout(g, GLOM_B200_BF16, max_iters, 0);
+  s.fwd = workspace_layout(g, GLOM_B200_BF16, max_iters, return_all);
   size_t off = s.fwd.total;
   s.dsq_off = off; off = align_up(off + s.fwd.nsq_bytes, 1024);
   s.flags_off = off;
@@ -217,7 +217,7 @@ struct SettleRun { float tol; int32_t* steps; };
 static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                         const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
                         int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity,
-                        const SettleRun* settle = nullptr);
+                        const SettleRun* settle = nullptr, const int32_t* steps = nullptr);
 
 static int check_settle(const glom_b200_cfg* cfg, int batch, int max_iters) {
   if (int r = check_cfg(cfg)) return r;
@@ -246,6 +246,34 @@ GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_
                       workspace_bytes, stream, -1, &run);
 }
 
+// glom_b200_forward_steps: a forward of max_steps steps in which image b stops after steps[b] (read on the device only)
+static int check_forward_steps(const glom_b200_cfg* cfg, int batch, int max_steps) {
+  if (int r = check_cfg(cfg)) return r;
+  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "forward_steps: bf16 engine only (precision fp32 given)");
+  if (batch < 1) return fail(GLOM_B200_ERR_INVALID, "forward_steps: batch must be >= 1 (got %d)", batch);
+  if (max_steps < 0) return fail(GLOM_B200_ERR_INVALID, "forward_steps: max_steps must be >= 0 (got %d)", max_steps);
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_forward_steps_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_steps, int return_all,
+                                                          size_t* out_bytes) {
+  if (int r = check_forward_steps(cfg, batch, max_steps)) return r;
+  if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
+  *out_bytes = settle_layout(make_geometry(cfg, batch), max_steps, return_all ? 1 : 0).total;
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_forward_steps(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
+                                          const float* pos, const float* state_in, const float* init_levels, float* state_out,
+                                          int batch, const int32_t* steps, int max_steps, int return_all, void* workspace,
+                                          size_t workspace_bytes, void* stream) {
+  if (int r = check_forward_steps(cfg, batch, max_steps)) return r;
+  if (!steps) return fail(GLOM_B200_ERR_INVALID, "forward_steps: steps is NULL");
+  if (reinterpret_cast<uintptr_t>(steps) % 4) return fail(GLOM_B200_ERR_INVALID, "forward_steps: steps must be 4-byte aligned");
+  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_steps, return_all ? 1 : 0,
+                      workspace, workspace_bytes, stream, -1, nullptr, steps);
+}
+
 GLOM_B200_API int glom_b200_forward(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                       const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
                       int return_all, void* workspace, size_t workspace_bytes, void* stream) {
@@ -269,7 +297,7 @@ GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void*
 static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                         const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
                         int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity,
-                        const SettleRun* settle) {
+                        const SettleRun* settle, const int32_t* steps) {
   if (int r = check_cfg(cfg)) return r;
   if (batch < 1 || iters < 0) return fail(GLOM_B200_ERR_INVALID, "batch must be >= 1 and iters >= 0");
   if (!packed_weights || !tokens || !pos || !state_out) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
@@ -284,9 +312,11 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
   DeviceInfo di{};
   if (int r = device_info(&di)) return r;
   const Geometry g = make_geometry(cfg, batch);
-  const SettleLayout sl = settle ? settle_layout(g, iters) : SettleLayout{};
-  const WorkspaceLayout wl = settle ? sl.fwd : workspace_layout(g, cfg->precision, iters, return_all);
-  const size_t ws_need = settle ? sl.total : wl.total;
+  // settle and forward_steps freeze images: the SETTLE instantiations of the step kernels, driven by per-image flags
+  const bool freeze = settle || steps;
+  const SettleLayout sl = freeze ? settle_layout(g, iters, return_all) : SettleLayout{};
+  const WorkspaceLayout wl = freeze ? sl.fwd : workspace_layout(g, cfg->precision, iters, return_all);
+  const size_t ws_need = freeze ? sl.total : wl.total;
   if (!workspace || workspace_bytes < ws_need)
     return fail(GLOM_B200_ERR_WORKSPACE, "workspace: need %zu bytes, got %zu", ws_need, workspace_bytes);
   const PackedLayout pl = packed_layout(g.d, g.L, cfg->precision);
@@ -332,22 +362,26 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
     // list heads / dependency counters for every step are zeroed once per call.  Opt-in: the three-launch step is the
     // default path.
     const char* merged_env = getenv("GLOM_B200_MERGED_MLP");     // read per call: tests toggle it in-process
-    const bool split_mlp = settle || !(merged_env && merged_env[0] == '1');     // settle: always the three-launch step
+    const bool split_mlp = freeze || !(merged_env && merged_env[0] == '1');     // freezing: always the three-launch step
     int* sched = nullptr;
     if (wl.sched_bytes && !split_mlp && iters > 0) {
       sched = reinterpret_cast<int*>(ws + wl.sched_off);
       e = cudaMemsetAsync(sched, 0, wl.sched_bytes, st);
       if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "scheduler counters memset: %s", cudaGetErrorString(e));
     }
-    // settle: no image has stopped yet
-    int* frozen = settle ? reinterpret_cast<int*>(ws + sl.frozen_off) : nullptr;
-    int* block_frozen = settle ? reinterpret_cast<int*>(ws + sl.block_frozen_off) : nullptr;
-    float* dsq = settle ? reinterpret_cast<float*>(ws + sl.dsq_off) : nullptr;
+    // settle: no image has stopped yet.  forward_steps: the schedule kernel writes every flag before each step
+    int* frozen = freeze ? reinterpret_cast<int*>(ws + sl.frozen_off) : nullptr;
+    int* block_frozen = freeze ? reinterpret_cast<int*>(ws + sl.block_frozen_off) : nullptr;
+    float* dsq = settle ? reinterpret_cast<float*>(ws + sl.dsq_off) : nullptr;     // NULL: K2 sums no squared change
     if (settle) {
       e = cudaMemsetAsync(ws + sl.flags_off, 0, sl.flags_bytes, st);
       if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle flags memset: %s", cudaGetErrorString(e));
     }
     for (int t = 0; t < iters; ++t) {
+      if (steps) {         // images with steps[b] <= t are frozen from step t on (from the start when steps[b] == 0)
+        e = launch_steps_schedule(g, t, iters, steps, frozen, block_frozen, st, &g_launches);
+        if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "step schedule launch before step %d: %s", t, cudaGetErrorString(e));
+      }
       Bf16Buffers b{};
       b.s32_in = (s0_direct && t == 0) ? (state_in ? state_in : init_levels) : loc(t); b.s32_out = loc(t + 1);
       b.s32_in_bcast = (s0_direct && t == 0 && !state_in) ? 1 : 0;
@@ -377,8 +411,18 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
     }
     // settle: image b's result S_steps[b] is in loc(steps[b]); the ones in the workspace slab move to state_out
     if (settle) {
-      e = launch_settle_gather(g, iters, settle->steps, wslab, state_out, st, &g_launches);
+      e = launch_settle_gather(g, iters, settle->steps, wslab, state_out, nullptr, 0, st, &g_launches);
       if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle gather launch: %s", cudaGetErrorString(e));
+    }
+    // forward_steps: return_all slab t of image b must be S_min(t, steps[b]); without return_all the result of an image
+    // with steps[b] == 0 is S_0, which step 0 read straight from state_in / init_levels when it ran
+    if (steps && return_all) {
+      e = launch_steps_fill(g, iters, steps, state_out, st, &g_launches);
+      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "return_all fill launch: %s", cudaGetErrorString(e));
+    } else if (steps && iters > 0) {
+      e = launch_settle_gather(g, iters, steps, wslab, state_out, s0_direct ? (state_in ? state_in : init_levels) : nullptr,
+                               state_in ? 0 : 1, st, &g_launches);
+      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "step gather launch: %s", cudaGetErrorString(e));
     }
   } else {
     cudaError_t e = launch_broadcast_init(g, state_in, init_levels, loc(0), st, &g_launches, &g_prof);
@@ -482,10 +526,10 @@ GLOM_B200_API int glom_b200_backward_workspace_bytes(const glom_b200_cfg* cfg, i
   return 0;
 }
 
-GLOM_B200_API int glom_b200_backward(const glom_b200_cfg* cfg, const glom_b200_weights_ref* w, const float* tokens,
-                                     const float* pos, const float* states, const float* grad_out,
-                                     const glom_b200_grads* gr, int batch, int iters, int grad_all, void* workspace,
-                                     size_t workspace_bytes, void* stream) {
+// glom_b200_backward (steps == NULL) and glom_b200_backward_steps (per-image step counts, iters = max_steps)
+static int backward_impl(const glom_b200_cfg* cfg, const glom_b200_weights_ref* w, const float* tokens, const float* pos,
+                         const float* states, const float* grad_out, const glom_b200_grads* gr, int batch, int iters,
+                         const int32_t* steps, int grad_all, void* workspace, size_t workspace_bytes, void* stream) {
   if (int r = check_cfg(cfg)) return r;
   if (batch < 1 || iters < 0) return fail(GLOM_B200_ERR_INVALID, "batch must be >= 1 and iters >= 0");
   if (!w || w->struct_size != sizeof(glom_b200_weights_ref) || !gr || gr->struct_size != sizeof(glom_b200_grads))
@@ -510,11 +554,30 @@ GLOM_B200_API int glom_b200_backward(const glom_b200_cfg* cfg, const glom_b200_w
   a.d_td_w1 = gr->d_td_w1; a.d_td_b1 = gr->d_td_b1; a.d_td_w2 = gr->d_td_w2; a.d_td_b2 = gr->d_td_b2;
   g_launches = 0;
   char msg[400] = "";
-  if (int r = backward_run(g, a, cfg->precision, iters, grad_all, workspace, g_encode, di.sms,
+  if (int r = backward_run(g, a, cfg->precision, iters, grad_all, steps, workspace, g_encode, di.sms,
                            static_cast<cudaStream_t>(stream), &g_launches, msg, sizeof(msg)))
     return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "%s", msg);
   g_err[0] = 0;
   return 0;
+}
+
+GLOM_B200_API int glom_b200_backward(const glom_b200_cfg* cfg, const glom_b200_weights_ref* w, const float* tokens,
+                                     const float* pos, const float* states, const float* grad_out,
+                                     const glom_b200_grads* gr, int batch, int iters, int grad_all, void* workspace,
+                                     size_t workspace_bytes, void* stream) {
+  return backward_impl(cfg, w, tokens, pos, states, grad_out, gr, batch, iters, nullptr, grad_all, workspace,
+                       workspace_bytes, stream);
+}
+
+GLOM_B200_API int glom_b200_backward_steps(const glom_b200_cfg* cfg, const glom_b200_weights_ref* w, const float* tokens,
+                                           const float* pos, const float* states, const float* grad_out,
+                                           const glom_b200_grads* gr, int batch, const int32_t* steps, int max_steps,
+                                           int grad_all, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!steps) return fail(GLOM_B200_ERR_INVALID, "backward_steps: steps is NULL");
+  if (reinterpret_cast<uintptr_t>(steps) % 4) return fail(GLOM_B200_ERR_INVALID, "backward_steps: steps must be 4-byte aligned");
+  if (max_steps < 0) return fail(GLOM_B200_ERR_INVALID, "backward_steps: max_steps must be >= 0 (got %d)", max_steps);
+  return backward_impl(cfg, w, tokens, pos, states, grad_out, gr, batch, max_steps, steps, grad_all, workspace,
+                       workspace_bytes, stream);
 }
 
 GLOM_B200_API int glom_b200_islands(const float* states, int slabs, int side_h, int side_w, int levels, int dim, float threshold,

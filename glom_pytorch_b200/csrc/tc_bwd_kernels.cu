@@ -63,7 +63,22 @@ struct BwdParams {
   // operand pair (maps a1 / b1) with its own layout flags; 0 = single product
   int k_split;
   int a_mn2, b_mn2, a_state2, b_state2;
+  // per-image step counts (NULL: none): at reverse step t the rows of images with steps[b] <= t have dY = 0, so BW_PRE /
+  // BW_DH / BW_DX skip a CTA's 128-row block and BW_DW a 64-row k-block when all its rows are such rows
+  const int32_t* steps;
+  int t;
 };
+
+// rows [r0, r0 + nr) below p.rows all belong to images frozen at this step (an empty range counts as frozen).  Every warp
+// role evaluates it for the same block, so producer and consumers skip the same tiles / k-blocks.  Warp-collective: the
+// lanes test one image each.
+__device__ __forceinline__ bool rows_frozen(const BwdParams& p, int r0, int nr, int lane) {
+  const int r1 = min(r0 + nr, p.rows);
+  bool live = false;
+  if (r0 < r1)
+    for (int b = r0 / p.n + lane; b <= (r1 - 1) / p.n; b += 32) live |= __ldg(p.steps + b) > p.t;
+  return !__any_sync(0xffffffffu, live);
+}
 
 struct Tile {
   int g, m_blk, n_blk, num_kb;
@@ -159,7 +174,11 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
       for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters) {
         const Tile t = decode<MODE>(p, tile);
         const int l = t.g >> 1;
+        if ((MODE == BW_PRE || MODE == BW_DH || MODE == BW_DX) && p.steps &&
+            rows_frozen(p, t.m_blk * 256 + cta_rank * BM, BM, lane))
+          continue;
         for (int kb = 0; kb < t.num_kb; ++kb) {
+          if (MODE == BW_DW && p.steps && rows_frozen(p, kb * BK, BK, lane)) continue;
           mbar_wait(&empty_bar[stage], phase ^ 1);
           if (elected) {
           const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES);
@@ -234,6 +253,9 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
     float frag[BN / 2];
     for (int tile = cluster_id; tile < p.num_tiles; tile += num_clusters) {
       const Tile t = decode<MODE>(p, tile);
+      if ((MODE == BW_PRE || MODE == BW_DH || MODE == BW_DX) && p.steps &&
+          rows_frozen(p, t.m_blk * 256 + cta_rank * BM, BM, lane))
+        continue;
       if (MODE == BW_PRE) {
         named_bar_sync(5, CONSUMER_WARPS * 32);
         for (int i = threadIdx.x; i < BN; i += CONSUMER_WARPS * 32) bias_s[i] = __ldg(p.b1p + (size_t)t.g * 4 * p.d + t.n_blk * BN + i);
@@ -243,6 +265,7 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
       for (int i = 0; i < BN / 2; ++i) frag[i] = 0.f;
       int prev = -1;                    // slot of the k-block whose MMAs may still be running
       for (int kb = 0; kb < t.num_kb; ++kb) {
+        if (MODE == BW_DW && p.steps && rows_frozen(p, kb * BK, BK, lane)) continue;
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + (size_t)stage * STAGE_BYTES) + (uint32_t)wg * 8192u;   // this warpgroup's 64 rows
         const uint32_t sb = smem_u32(smem + (size_t)stage * STAGE_BYTES) + A_BYTES;
@@ -261,6 +284,7 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      if (MODE == BW_DW && prev < 0) continue;     // every k-block was skipped: the tile adds nothing
       wgmma_wait<0>();
       wgmma_fence_regs(frag);
       __syncwarp();
@@ -494,6 +518,7 @@ int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int
   p.b1p = a.b1p; p.pre = a.pre; p.h = a.h; p.dpre = a.dpre; p.ds = a.ds; p.d_tokens = a.d_tokens; p.d_pos = a.d_pos;
   p.d_bu_w1 = a.d_bu_w1; p.d_bu_w2 = a.d_bu_w2; p.d_td_w1 = a.d_td_w1; p.d_td_w2 = a.d_td_w2;
   p.d_bu_b1 = a.d_bu_b1; p.d_td_b1 = a.d_td_b1;
+  p.steps = a.steps; p.t = a.t;
   const int nm = (rows + 255) / 256;
   cudaError_t e;
   p.num_tiles = G * nm * (4 * d / BN);

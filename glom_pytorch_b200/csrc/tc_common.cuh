@@ -125,11 +125,11 @@ struct K2Chunk {
 };
 // SETTLE (Glom.settle): row r of the band loads and stores nothing unless bit r of `live` is set (rows of images that
 // have stopped keep their state), and rowdsq[i] accumulates the squared change |S_{t+1} - S_t|^2 of row i * 4 + rsub
-// in the same order as rowsq.
+// in the same order as rowsq (only when want_dsq: the per-image step counts of forward_steps need no change partials).
 template <bool FULL, bool SETTLE = false>
 __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b4, uint8_t* patch, const K2Chunk& k,
                                          int col, int lane, int rows_left, float (&rowsq)[8], uint32_t live = ~0u,
-                                         float* rowdsq = nullptr) {
+                                         float* rowdsq = nullptr, bool want_dsq = false) {
 #pragma unroll
   for (int c = 0; c < 8; ++c)
     *reinterpret_cast<uint4*>(patch + lane * 128 + ((c ^ (lane & 7)) << 4)) =
@@ -175,7 +175,7 @@ __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b
       if (top) { o0 = o0 / 3.0f; o1 = o1 / 3.0f; o2 = o2 / 3.0f; o3 = o3 / 3.0f; }          // (:142) IEEE division
       else { o0 *= 0.25f; o1 *= 0.25f; o2 *= 0.25f; o3 *= 0.25f; }                          // x/4 == x*0.25 exactly
       const bool store = (FULL || r < rows_left) && (!SETTLE || ((live >> r) & 1u));
-      if constexpr (SETTLE) {
+      if constexpr (SETTLE) if (want_dsq) {
         // rows that store nothing contribute no change (and, below, no norm)
         const float e0 = store ? o0 - sv[j].x : 0.f, e1 = store ? o1 - sv[j].y : 0.f;
         const float e2 = store ? o2 - sv[j].z : 0.f, e3 = store ? o3 - sv[j].w : 0.f;

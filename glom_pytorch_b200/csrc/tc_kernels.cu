@@ -429,8 +429,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
             float rowsq[8], rowdsq[8];
 #pragma unroll
             for (int i = 0; i < 8; ++i) rowsq[i] = rowdsq[i] = 0.f;
-            if (rows_left >= 32) k2_chunk<true, SETTLE>(v, b4, patch, kc, col, lane, 32, rowsq, live, rowdsq);
-            else k2_chunk<false, SETTLE>(v, b4, patch, kc, col, lane, rows_left, rowsq, live, rowdsq);
+            const bool want_dsq = SETTLE && p.dsq_out != nullptr;         // settle: yes; forward_steps: no
+            if (rows_left >= 32) k2_chunk<true, SETTLE>(v, b4, patch, kc, col, lane, 32, rowsq, live, rowdsq, want_dsq);
+            else k2_chunk<false, SETTLE>(v, b4, patch, kc, col, lane, rows_left, rowsq, live, rowdsq, want_dsq);
             // one squared-norm partial per PART_COLS columns: with 64-column parts the two warps of the pair hold the two
             // 32-column halves, summed in chunk order (0 + first) + second as in prep_state_kernel.  SETTLE: the
             // squared changes take the same exchange through the second warp's transpose patch, which k2_chunk no
@@ -442,7 +443,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
               if (x == 1 && (lane & 7) == 0) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i) xch_p[i * 4 + (lane >> 3)] = rowsq[i];
-                if constexpr (SETTLE) {
+                if (want_dsq) {
 #pragma unroll
                   for (int i = 0; i < 8; ++i) dxch[i * 4 + (lane >> 3)] = rowdsq[i];
                 }
@@ -451,7 +452,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
               if (x == 0) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i) rowsq[i] += xch_p[i * 4 + (lane >> 3)];
-                if constexpr (SETTLE) {
+                if (want_dsq) {
 #pragma unroll
                   for (int i = 0; i < 8; ++i) rowdsq[i] += dxch[i * 4 + (lane >> 3)];
                 }
@@ -467,7 +468,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
                 const int r = i * 4 + (lane >> 3);
                 if (r < rows_left && (!SETTLE || ((live >> r) & 1u))) {
                   nsq[(unsigned)(r * ldn)] = rowsq[i];
-                  if constexpr (SETTLE) p.dsq_out[po + (unsigned)(r * ldn)] = rowdsq[i];
+                  if (want_dsq) p.dsq_out[po + (unsigned)(r * ldn)] = rowdsq[i];
                 }
               }
             }

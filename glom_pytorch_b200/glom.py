@@ -30,6 +30,7 @@ forward to ~1e-5).
 """
 from math import sqrt
 
+import operator
 import weakref
 
 import torch
@@ -134,13 +135,17 @@ class ConsensusAttention(nn.Module):
 
 class _ColumnUpdate(torch.autograd.Function):
     """The loop glom_pytorch.py:131-145 as one differentiable op: forward = glom_b200_forward (all states kept),
-    backward = glom_b200_backward (recompute per step; tensor-core GEMMs for the bf16 engine)."""
+    backward = glom_b200_backward (recompute per step; tensor-core GEMMs for the bf16 engine).  With `steps` (the
+    engine's (B,) int32 copy of a per-image step vector, iters = its maximum): forward_steps / backward_steps."""
 
     @staticmethod
-    def forward(ctx, module, iters, return_all, tokens, pos, state0, init_levels, *weights):
+    def forward(ctx, module, iters, steps, return_all, tokens, pos, state0, init_levels, *weights):
         tokens, pos = tokens.contiguous(), pos.contiguous()
-        states = module._run_engine(tokens, pos, state0, init_levels, iters, True)      # (T+1, B, n, L, d)
-        ctx.module, ctx.iters, ctx.return_all = module, iters, return_all
+        if steps is None:
+            states = module._run_engine(tokens, pos, state0, init_levels, iters, True)      # (T+1, B, n, L, d)
+        else:
+            states = module._run_engine_steps(tokens, pos, state0, init_levels, steps, iters, True)
+        ctx.module, ctx.iters, ctx.return_all, ctx.steps = module, iters, return_all, steps
         ctx.had_state0 = state0 is not None
         ctx.want_state0 = state0 is not None and state0.requires_grad
         ctx.save_for_backward(tokens, pos, states, *weights)
@@ -166,11 +171,16 @@ class _ColumnUpdate(torch.autograd.Function):
             cfg = module.engine_cfg(n)           # bf16 engine: MLP GEMMs of the backward on tensor cores
             ws_bytes = _native.backward_workspace_bytes(cfg, b)
             ws = module._get_workspace(ws_bytes, device, "_bwd_workspace")      # cached across steps
-            _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
-                             grad_out.data_ptr(), {k: (None if v is None else v.data_ptr()) for k, v in g.items()},
-                             b, iters, ctx.return_all, ws.data_ptr(), ws.numel(),
-                             torch.cuda.current_stream(device).cuda_stream)
-        return (None, None, None, g["d_tokens"], g["d_pos"], g["d_state0"] if ctx.want_state0 else None, g["d_init"],
+            ptrs = {k: (None if v is None else v.data_ptr()) for k, v in g.items()}
+            stream = torch.cuda.current_stream(device).cuda_stream
+            if ctx.steps is None:
+                _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
+                                 grad_out.data_ptr(), ptrs, b, iters, ctx.return_all, ws.data_ptr(), ws.numel(), stream)
+            else:
+                _native.backward_steps(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(),
+                                       states.data_ptr(), grad_out.data_ptr(), ptrs, b, ctx.steps.data_ptr(), iters,
+                                       ctx.return_all, ws.data_ptr(), ws.numel(), stream)
+        return (None, None, None, None, g["d_tokens"], g["d_pos"], g["d_state0"] if ctx.want_state0 else None, g["d_init"],
                 *[g[k] for k in names])
 
 
@@ -432,13 +442,74 @@ class Glom(nn.Module):
                                 "parity": parity}
         return out
 
+    def _run_engine_steps(self, tokens, pos, state_in, init, steps, max_steps, return_all):
+        """glom_b200_forward_steps: image b runs steps[b] steps (steps: the engine's (B,) int32 CUDA tensor, max_steps its
+        maximum).  The shadows of stopped images are stale afterwards: the next forward takes the ordinary prologue."""
+        device = tokens.device
+        b, n = tokens.shape[0], tokens.shape[1]
+        self._resume = None
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            tokens = tokens.detach().to(torch.float32).contiguous()
+            pos = pos.detach().to(torch.float32).contiguous()
+            init = init.detach().to(torch.float32).contiguous()
+            if state_in is not None:
+                state_in = state_in.detach().to(device=device, dtype=torch.float32).contiguous()
+            cfg = self.engine_cfg(n)
+            packed = self._packed_weights(cfg, device, stream)
+            shape = (b, n, self.levels, self.dim)
+            out = torch.empty(((max_steps + 1,) + shape) if return_all else shape, dtype=torch.float32, device=device)
+            ws = self._get_workspace(_native.forward_steps_workspace_bytes(cfg, b, max_steps, return_all), device)
+            _native.forward_steps(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(),
+                                  None if state_in is None else state_in.data_ptr(), init.data_ptr(), out.data_ptr(), b,
+                                  steps.data_ptr(), max_steps, return_all, ws.data_ptr(), ws.numel(), stream)
+            self.last_launches = _native.last_launch_count() + getattr(self, "_tok_launches", 0)
+        return out
+
+    def _parse_iters(self, iters, b):
+        """-> (iters, steps): a scalar step count and None, or, for a per-image vector whose entries differ, its maximum
+        and the vector itself (the caller's tensor, or an int64 CPU tensor made from a list).  Reads min / max of a
+        vector once on the host."""
+        if iters is None:
+            return self.levels * 2, None                                     # (:112)
+        if isinstance(iters, (list, tuple)):
+            try:
+                iters = torch.tensor([operator.index(v) for v in iters], dtype=torch.int64)
+            except TypeError:
+                raise ValueError("a per-image iters list must hold integers") from None
+        if not isinstance(iters, torch.Tensor) or iters.dim() == 0:
+            return int(iters), None
+        if iters.dim() != 1:
+            raise ValueError(f"per-image iters must be a 1-D tensor, got {iters.dim()} dimensions")
+        if iters.dtype.is_floating_point or iters.dtype.is_complex or iters.dtype == torch.bool:
+            raise ValueError(f"per-image iters must have an integer dtype, got {iters.dtype}")
+        if iters.shape[0] != b:
+            raise ValueError(f"per-image iters must have one entry per image ({b}), got {iters.shape[0]}")
+        lo, hi = torch.stack(torch.aminmax(iters)).tolist()                 # one device-to-host read for a CUDA tensor
+        if lo < 0:
+            raise ValueError(f"per-image iters must be >= 0, got {lo}")
+        if lo == hi:
+            return int(hi), None
+        return int(hi), iters
+
     # ------------------------------------------------------------------ the reference's forward (:110)
     def forward(self, img, iters=None, levels=None, return_all=False):
+        """The reference's forward.  ``iters`` is an int (None = 2L), or a per-image step count: a 1-D integer tensor
+        (CPU or CUDA) or a list of length B with entries >= 0.  With T = max(iters), image b then gets S_{iters[b]}
+        (``return_all``: (T+1, B, n, L, d), slab t of image b = S_{min(t, iters[b])}), bit-identical to
+        ``forward(img, iters=iters[b], levels=same)[b]``; under autograd a stopped image is the identity at the later
+        steps.  min / max of the vector are read once on the host (one device-to-host read for a CUDA tensor); a
+        vector whose entries are all equal takes the scalar path.  Per-image counts need precision='bf16' and clear
+        the resume state."""
+        b = img.shape[0]
+        iters, steps = self._parse_iters(iters, b)
+        if steps is not None and self.precision != "bf16":
+            raise RuntimeError("per-image iters need precision='bf16' (the fp32 engine has no per-image freezing)")
         if not img.is_cuda:
             raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
                                "move the module and inputs to an H100")
-        b = img.shape[0]
-        iters = self.levels * 2 if iters is None else int(iters)             # (:112)
+        if steps is not None:    # the engine's own int32 copy: later in-place edits of the caller's tensor change nothing
+            steps = steps.to(device=img.device, dtype=torch.int32, copy=True)
         needs_grad = torch.is_grad_enabled() and (
             img.requires_grad or (levels is not None and levels.requires_grad)
             or any(p.requires_grad for p in self.parameters()))
@@ -454,6 +525,9 @@ class Glom(nn.Module):
             tokens = self._take_staged(img)
             if tokens is None:
                 tokens = self.tokens(img)                                    # (:114) engine tokeniser
+            if steps is not None:
+                return self._run_engine_steps(tokens, self.pos_emb.weight[:n], levels, self.init_levels, steps, iters,
+                                              return_all)
             return self._run_engine(tokens, self.pos_emb.weight[:n], levels, self.init_levels, iters, return_all,
                                     allow_resume=not self.training)
         # training: the tokeniser and the loop are the engine's differentiable ops (the same kernels as without autograd);
@@ -466,7 +540,7 @@ class Glom(nn.Module):
             tokens = lin(self.image_to_tokens[0](img.float()))
         pos = self.pos_emb.weight[:n]                                                            # (:117)
         state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
-        return _ColumnUpdate.apply(self, iters, return_all, tokens, pos, state0, self.init_levels, *self._mlp_params())
+        return _ColumnUpdate.apply(self, iters, steps, return_all, tokens, pos, state0, self.init_levels, *self._mlp_params())
 
     # ------------------------------------------------------------------ inference until the columns settle
     def settle(self, img, tol, max_iters=None, levels=None):

@@ -137,6 +137,23 @@ GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_
                                    int max_iters, float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes,
                                    void* stream);
 
+/* Per-image step counts.  bf16 engine only.  The forward of glom_b200_forward run for max_steps (>= 0) steps from the same
+ * start (state_in, or init_levels broadcast), in which image b stops after steps[b] steps: its later steps skip its work
+ * and store nothing.  steps (B) int32 is device memory, read on the device only; each entry is clamped on the device to
+ * [0, max_steps].  With s_b = the clamped steps[b]:
+ *   return_all = 0: state_out (B, n, L, d), state_out[b] = S_{s_b} of image b (S_0 when s_b == 0);
+ *   return_all = 1: state_out (max_steps+1, B, n, L, d), slab t of image b = S_{min(t, s_b)}.
+ * Image b's result is bit-identical to glom_b200_forward(iters = s_b, same return_all) on the same batch; each step is
+ * the three-launch step.  The workspace (1024-byte aligned) is the forward workspace for (batch, max_steps, return_all)
+ * plus the per-image and per-256-row-block flags; a following glom_b200_forward_resume on it is not valid.  Argument
+ * errors (precision fp32, max_steps < 0, NULL steps) are reported before any device query. */
+GLOM_B200_API int glom_b200_forward_steps_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_steps, int return_all,
+                                                          size_t* out_bytes);
+GLOM_B200_API int glom_b200_forward_steps(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
+                                          const float* pos, const float* state_in, const float* init_levels, float* state_out,
+                                          int batch, const int32_t* steps, int max_steps, int return_all, void* workspace,
+                                          size_t workspace_bytes, void* stream);
+
 /* Tokeniser, the step before the loop: replaces image_to_tokens
  * (glom_pytorch.py:94-97, call :114): patchify 'b c (h p1) (w p2) -> b (h w) (p1 p2 c)'
  * fused with the Linear(3*p*p -> d).
@@ -184,6 +201,15 @@ GLOM_B200_API int glom_b200_backward(const glom_b200_cfg* cfg, const glom_b200_w
                        const float* tokens, const float* pos, const float* states, const float* grad_out,
                        const glom_b200_grads* grads, int batch, int iters, int grad_all,
                        void* workspace, size_t workspace_bytes, void* stream);
+/* Backward of glom_b200_forward_steps(return_all = 1): the same as glom_b200_backward with iters = max_steps, for the
+ * per-image program in which image b is the identity at every step t >= steps[b] (steps: the forward's (B) int32 device
+ * array).  At such a step the image's upstream gradient passes through unchanged and it adds nothing to any parameter,
+ * pos or token gradient; the MLP GEMMs of the tensor-core backward skip row blocks made only of such rows.  `states` is
+ * the forward_steps return_all output.  Same workspace as glom_b200_backward. */
+GLOM_B200_API int glom_b200_backward_steps(const glom_b200_cfg* cfg, const glom_b200_weights_ref* weights,
+                                           const float* tokens, const float* pos, const float* states, const float* grad_out,
+                                           const glom_b200_grads* grads, int batch, const int32_t* steps, int max_steps,
+                                           int grad_all, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Backward of glom_b200_tokenize (image_to_tokens, glom_pytorch.py:94-97; SURVEY 8 rows f1 + f2), fp32 on CUDA cores:
  *   d_weight (dim, 3 patch^2) += d_tokens^T . patches,   d_bias (dim) += column sums of d_tokens,
