@@ -20,6 +20,7 @@ EXPORTS = (
     "glom_b200_clock_probe", "glom_b200_mlp_schedule", "glom_b200_islands", "glom_b200_kernel_clocks",
     "glom_b200_settle", "glom_b200_settle_workspace_bytes",
     "glom_b200_forward_steps", "glom_b200_forward_steps_workspace_bytes", "glom_b200_backward_steps",
+    "glom_b200_settle_all", "glom_b200_settle_all_workspace_bytes",
 )
 PROFILE_KINDS = ("attention", "gemm1_gelu", "gemm2_combine", "prologue", "tokenize", "mlp_fused")
 
@@ -98,6 +99,11 @@ def load():
     lib.glom_b200_settle_workspace_bytes.restype = i32
     lib.glom_b200_settle.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, vp, sz, vp]
     lib.glom_b200_settle.restype = i32
+    lib.glom_b200_settle_all_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, i32, ctypes.POINTER(sz)]
+    lib.glom_b200_settle_all_workspace_bytes.restype = i32
+    lib.glom_b200_settle_all.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, vp, sz,
+                                         vp]
+    lib.glom_b200_settle_all.restype = i32
     lib.glom_b200_forward_steps_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, i32, i32, ctypes.POINTER(sz)]
     lib.glom_b200_forward_steps_workspace_bytes.restype = i32
     lib.glom_b200_forward_steps.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, vp, i32, i32, vp, sz, vp]
@@ -203,6 +209,20 @@ def settle(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr
     """glom_b200_settle: up to max_iters steps, each image stopped on the GPU; steps_ptr -> (batch,) int32 device words."""
     check(load().glom_b200_settle(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch,
                                   max_iters, float(tol), steps_ptr, ws_ptr, ws_bytes, stream))
+
+
+def settle_all_workspace_bytes(cfg, batch, max_iters):
+    out = ctypes.c_size_t()
+    check(load().glom_b200_settle_all_workspace_bytes(ctypes.byref(cfg), batch, max_iters, ctypes.byref(out)))
+    return out.value
+
+
+def settle_all(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, max_iters, tol, steps_ptr,
+               ws_ptr, ws_bytes, stream):
+    """glom_b200_settle_all: settle() with every state kept; out_ptr -> (max_iters+1, batch, n, L, d) fp32, slab t of
+    image b = S_min(t, steps[b])."""
+    check(load().glom_b200_settle_all(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr,
+                                      batch, max_iters, float(tol), steps_ptr, ws_ptr, ws_bytes, stream))
 
 
 def forward_steps_workspace_bytes(cfg, batch, max_steps, return_all):

@@ -101,10 +101,11 @@ static cudaError_t gemm_f32(const GemmF32& q, int batches, cudaStream_t st, int*
 // g (R, L, d)  <-  (gin + extra) (R, L, d) / c_l   (:142);   ds (R, L, d) <- g (residual term of the sum, :141)
 // `extra` (nullable) is the upstream gradient of this time step's own output when every step is returned (:147-148)
 // steps (nullable): per-image step counts; an image with steps[b] <= t is the identity at step t, so its rows get
-// g = 0 (every later contribution of theirs is an exact zero) and ds = gin + extra unscaled
+// g = 0 (every later contribution of theirs is an exact zero) and ds = gin + extra unscaled.  g_kept: g already holds
+// those zeros (written at reverse step t + 1, where the image was frozen too), so they are not stored again
 __global__ void scale_by_contrib_kernel(size_t total, int L, int d, const float* __restrict__ gin,
                                         const float* __restrict__ extra, float* __restrict__ g, float* __restrict__ ds,
-                                        const int32_t* __restrict__ steps, int t, size_t img4) {
+                                        const int32_t* __restrict__ steps, int t, size_t img4, int g_kept) {
   const size_t total4 = total / 4;
   const unsigned d4 = (unsigned)d / 4;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (size_t)gridDim.x * blockDim.x) {
@@ -112,7 +113,7 @@ __global__ void scale_by_contrib_kernel(size_t total, int L, int d, const float*
     float4 v = reinterpret_cast<const float4*>(gin)[i];
     if (extra) { const float4 e = reinterpret_cast<const float4*>(extra)[i]; v.x += e.x; v.y += e.y; v.z += e.z; v.w += e.w; }
     if (steps && __ldg(steps + i / img4) <= t) {
-      reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (!g_kept) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
       reinterpret_cast<float4*>(ds)[i] = v;
       continue;
     }
@@ -146,15 +147,21 @@ __global__ void gelu_bwd_kernel(size_t total, const float* __restrict__ pre, flo
 // out[c] += sum_r src[r * row_stride + c]          (bias gradients); grid (cols / 32, row chunks)
 // out2 (nullable) receives the same sums for its first cols2 columns (the top-down second-layer biases see the
 // same upstream gradient as the bottom-up ones on levels 0 .. L-2)
+// steps (nullable): rows r of images frozen at reverse step t (steps[r / n] <= t) hold zeros and are not read; the sums
+// are the same bits
 __global__ void colsum_acc_kernel(int rows, int cols, long long row_stride, const float* __restrict__ src,
-                                  float* __restrict__ out, float* __restrict__ out2 = nullptr, int cols2 = 0) {
+                                  float* __restrict__ out, float* __restrict__ out2 = nullptr, int cols2 = 0,
+                                  const int32_t* __restrict__ steps = nullptr, int t = 0, int n = 1) {
   const int c = blockIdx.x * 32 + (threadIdx.x & 31);
   const int part = threadIdx.x >> 5;                 // 8 row slices per block
   const int r_begin = (int)(((long long)rows * blockIdx.y) / gridDim.y), r_end = (int)(((long long)rows * (blockIdx.y + 1)) / gridDim.y);
   __shared__ float red[8][33];
   float acc = 0.f;
-  if (c < cols)
+  if (c < cols && !steps)
     for (int r = r_begin + part; r < r_end; r += 8) acc += src[(long long)r * row_stride + c];
+  else if (c < cols)
+    for (int r = r_begin + part; r < r_end; r += 8)
+      if (__ldg(steps + r / n) > t) acc += src[(long long)r * row_stride + c];
   red[part][threadIdx.x & 31] = acc;
   __syncthreads();
   if (part == 0 && c < cols) {
@@ -185,11 +192,24 @@ __global__ void add_kernel(size_t total, const float* __restrict__ src, float* _
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x)
     dst[i] += src[i];
 }
+// The four warp-per-row kernels of the attention backward take `FrozenRows`: at reverse step t of the tensor-core
+// backward with per-image step counts, the rows of images with steps[b] <= t are skipped.  Their rows are image-major in
+// both row spaces, (row, level) and (image * L + level, query), so image = row / (n L).  A skipped row's outputs (khat,
+// rnorm, khat_b, A, a_b, dA, dsim_b; ds is not touched) keep whatever they held, possibly never written: every reader of
+// them skips the same rows.
+struct FrozenRows {
+  const int32_t* steps;      // NULL: no row is skipped
+  int t, rows_per_image;
+  __device__ __forceinline__ bool operator()(int row) const {
+    return steps && __ldg(steps + row / rows_per_image) <= t;
+  }
+};
+
 // khat = S / max(|S|, 1e-12) per (row, level) ; rnorm = 1 / max(|S|, 1e-12)      (F.normalize, :58)
 __global__ void normalize_rows_kernel(int nrows, int d, const float* __restrict__ s, float* __restrict__ khat,
-                                      float* __restrict__ rnorm, __nv_bfloat16* __restrict__ khat_b) {
+                                      float* __restrict__ rnorm, __nv_bfloat16* __restrict__ khat_b, FrozenRows frozen) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= nrows) return;
+  if (row >= nrows || frozen(row)) return;
   const float* p = s + (size_t)row * d;
   float ss = 0.f;
   for (int c = lane; c < d; c += 32) ss = fmaf(p[c], p[c], ss);
@@ -205,9 +225,9 @@ __global__ void normalize_rows_kernel(int nrows, int d, const float* __restrict_
 }
 // in-place masked softmax over the last dim of sim (Z, n, n)     (:62-71); one warp per row
 __global__ void attn_softmax_kernel(int Z, int n, int attend_self, int mask_side, int mask_d2_max, float scale,
-                                    float* __restrict__ sim, __nv_bfloat16* __restrict__ a_b) {
+                                    float* __restrict__ sim, __nv_bfloat16* __restrict__ a_b, FrozenRows frozen) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= Z * n) return;
+  if (row >= Z * n || frozen(row)) return;
   const int i = row % n;
   float* p = sim + (size_t)row * n;
   float m = -3.402823466e+38f;
@@ -237,9 +257,9 @@ __global__ void attn_softmax_kernel(int Z, int n, int attend_self, int mask_side
 // dsim = A * (dA - sum_j A dA), zero where the logit was a constant (diagonal fill, radius mask); in place on dA
 __global__ void attn_softmax_bwd_kernel(int Z, int n, int attend_self, int mask_side, int mask_d2_max,
                                         const float* __restrict__ A, float* __restrict__ dA, float scale,
-                                        __nv_bfloat16* __restrict__ dsim_b) {
+                                        __nv_bfloat16* __restrict__ dsim_b, FrozenRows frozen) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= Z * n) return;
+  if (row >= Z * n || frozen(row)) return;
   const int i = row % n;
   const float* a = A + (size_t)row * n;
   float* g = dA + (size_t)row * n;
@@ -260,9 +280,9 @@ __global__ void attn_softmax_bwd_kernel(int Z, int n, int attend_self, int mask_
 }
 // ds[row] += (dkhat - khat (khat . dkhat)) * rnorm        (backward of F.normalize); one warp per (row, level)
 __global__ void normalize_bwd_kernel(int nrows, int d, const float* __restrict__ khat, const float* __restrict__ dkhat,
-                                     const float* __restrict__ rnorm, float* __restrict__ ds) {
+                                     const float* __restrict__ rnorm, float* __restrict__ ds, FrozenRows frozen) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (row >= nrows) return;
+  if (row >= nrows || frozen(row)) return;
   const float* k = khat + (size_t)row * d;
   const float* g = dkhat + (size_t)row * d;
   float dot = 0.f;
@@ -411,7 +431,7 @@ BackwardLayout backward_layout(const Geometry& g, int precision) {
 // accumulate parameter / token / pos gradients.
 static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const float* s_t, const float* gin,
                                  const float* gextra, float* ds, char* ws, const BackwardLayout& wl, bool mlp_on_tc,
-                                 bool attn_on_tc, const int32_t* steps, int t, cudaStream_t st, int* launches) {
+                                 bool attn_on_tc, const int32_t* steps, int t, bool gs_kept, cudaStream_t st, int* launches) {
   const int R = g.rows, L = g.L, d = g.d, n = g.n, h4 = 4 * g.d;
   const long long ld = (long long)L * d;
   float* gs = reinterpret_cast<float*>(ws + wl.gs_off);       // (gin + gextra) / c
@@ -421,7 +441,8 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
   float* xp = reinterpret_cast<float*>(ws + wl.xp_off);
   float* dx = reinterpret_cast<float*>(ws + wl.dx_off);
   const size_t state = (size_t)R * L * d;
-  scale_by_contrib_kernel<<<nblk(state), 256, 0, st>>>(state, L, d, gin, gextra, gs, ds, steps, t, (size_t)n * ld / 4);
+  scale_by_contrib_kernel<<<nblk(state), 256, 0, st>>>(state, L, d, gin, gextra, gs, ds, steps, t, (size_t)n * ld / 4,
+                                                       gs_kept ? 1 : 0);
   CKL();
 
   // ---- the two grouped MLPs (:23-36), one group at a time (fp32 path; the bf16 engine runs them on tensor cores)
@@ -495,13 +516,14 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
     const long long sb = (long long)n * ld, sl = d, nn = (long long)n * n;
     const float scale = 1.0f / sqrtf((float)d);
     const int wblocks = (R * L * 32 + 255) / 256;
-    normalize_rows_kernel<<<wblocks, 256, 0, st>>>(R * L, d, s_t, khat, rnorm, nullptr);
+    const FrozenRows all_rows{nullptr, 0, 1};           // masked by gs = 0 instead
+    normalize_rows_kernel<<<wblocks, 256, 0, st>>>(R * L, d, s_t, khat, rnorm, nullptr, all_rows);
     CKL();
     GemmF32 q{};
     // sim = scale * Q Khat^T                              (n x n per (b, l))
     q = GemmF32{n, n, d, L, Mat{s_t, ld, 1, sb, sl}, Mat{khat, 1, ld, sb, sl}, MatOut{A, n, 1, nn * L, nn}, 1.f, 0.f, nullptr};
     CK(gemm_f32(q, Z, st, launches));
-    attn_softmax_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, nullptr);
+    attn_softmax_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, nullptr, all_rows);
     CKL();
     // dA = dC V^T
     q = GemmF32{n, n, d, L, Mat{gs, ld, 1, sb, sl}, Mat{s_t, 1, ld, sb, sl}, MatOut{dA, n, 1, nn * L, nn}, 1.f, 0.f, nullptr};
@@ -509,7 +531,7 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
     // dV: ds += A^T dC
     q = GemmF32{n, d, n, L, Mat{A, 1, n, nn * L, nn}, Mat{gs, ld, 1, sb, sl}, MatOut{ds, ld, 1, sb, sl}, 1.f, 1.f, nullptr};
     CK(gemm_f32(q, Z, st, launches));
-    attn_softmax_bwd_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, 1.f, nullptr);
+    attn_softmax_bwd_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, 1.f, nullptr, all_rows);
     CKL();
     // dQ: ds += scale * dsim Khat
     q = GemmF32{n, d, n, L, Mat{dA, n, 1, nn * L, nn}, Mat{khat, ld, 1, sb, sl}, MatOut{ds, ld, 1, sb, sl}, scale, 1.f, nullptr};
@@ -517,7 +539,7 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
     // dKhat = scale * dsim^T Q
     q = GemmF32{n, d, n, L, Mat{dA, 1, n, nn * L, nn}, Mat{s_t, ld, 1, sb, sl}, MatOut{dkhat, ld, 1, sb, sl}, scale, 0.f, nullptr};
     CK(gemm_f32(q, Z, st, launches));
-    normalize_bwd_kernel<<<wblocks, 256, 0, st>>>(R * L, d, khat, dkhat, rnorm, ds);
+    normalize_bwd_kernel<<<wblocks, 256, 0, st>>>(R * L, d, khat, dkhat, rnorm, ds, all_rows);
     CKL();
   }
   return cudaSuccess;
@@ -554,14 +576,19 @@ __global__ void pack_bwd_weights_kernel(int d, int L, const float* __restrict__ 
   }
 }
 // bf16 shadows of a step: sb = bf16(S_t), sp = bf16(S_t[:, 1:] + pos), gsb = bf16(gs)
+// kept (nullable): the rows of images with kept[b] <= t are not rewritten.  Such an image was frozen at step t + 1 too,
+// so its gsb rows already hold the exact zeros the MLP GEMMs of partially frozen blocks need, and its sb / sp rows hold
+// finite values those GEMMs only multiply by zero (with return_all states they are the same bits: S_t == S_{t+1})
 __global__ void bwd_shadows_kernel(int rows, int n, int L, int d, const float* __restrict__ s, const float* __restrict__ gs,
                                    const float* __restrict__ pos, __nv_bfloat16* __restrict__ sb,
-                                   __nv_bfloat16* __restrict__ sp, __nv_bfloat16* __restrict__ gsb) {
+                                   __nv_bfloat16* __restrict__ sp, __nv_bfloat16* __restrict__ gsb,
+                                   const int32_t* __restrict__ kept, int t) {
   const size_t total4 = (size_t)rows * L * d / 4;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (size_t)gridDim.x * blockDim.x) {
     const size_t e = i * 4;
     const int c = (int)(e % d), l = (int)((e / d) % L);
     const size_t r = e / ((size_t)L * d);
+    if (kept && __ldg(kept + r / n) <= t) continue;
     const float4 v = *reinterpret_cast<const float4*>(s + e);
     const float4 gv = *reinterpret_cast<const float4*>(gs + e);
     *reinterpret_cast<uint2*>(sb + e) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
@@ -621,13 +648,21 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
   for (int t = iters - 1, k = 0; t >= 0; --t, ++k) {
     const float* s_t = a.states + (size_t)t * state;
     float* ds = slab[k & 1];
-    CKI(backward_step(g, a, s_t, gin, gextra, ds, ws, wl, tc, attn_tc, steps, t, st, launches));   // scale (+ the fp32 MLP / attention backward)
+    // an image frozen at step t (steps[b] <= t) below the first reverse step was frozen at step t + 1 as well: its rows
+    // of gs and of the bf16 shadows still hold what step t + 1 wrote (zeros in gs / gsb), so they are not rewritten.  A
+    // reverse step at which every image is frozen (t >= max(steps), the tail of a settle_all backward) then only passes
+    // ds = gin + gextra through; its other launches find no work.
+    const int32_t* kept = (steps && t < iters - 1) ? steps : nullptr;
+    CKI(backward_step(g, a, s_t, gin, gextra, ds, ws, wl, tc, attn_tc, steps, t, kept != nullptr, st,
+                      launches));   // scale (+ the fp32 MLP / attention backward)
     if (tc) {
       bwd_shadows_kernel<<<nblk(state / 4), 256, 0, st>>>(g.rows, g.n, g.L, g.d, s_t, gs, a.pos,
                                                           const_cast<__nv_bfloat16*>(m.sb), const_cast<__nv_bfloat16*>(m.sp),
-                                                          const_cast<__nv_bfloat16*>(m.gsb));
+                                                          const_cast<__nv_bfloat16*>(m.gsb), kept, t);
       CKLI();
-      // ---- consensus attention backward: the five (n x n x d) GEMM families on tensor cores, softmax in fp32
+      // ---- consensus attention backward: the five (n x n x d) GEMM families on tensor cores, softmax in fp32.  With
+      // per-image step counts, the problems / rows of images frozen at step t are skipped in every launch (their
+      // contribution to ds is an exact zero); the buffers they would have written are left stale and read by no one.
       if (attn_tc) {
         float* khat = reinterpret_cast<float*>(ws + wl.khat_off);
         float* dkhat = reinterpret_cast<float*>(ws + wl.dkhat_off);
@@ -640,27 +675,32 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
         const int Z = g.B * g.L, n = g.n, d = g.d;
         const float scale = 1.0f / sqrtf((float)d);
         const int wblocks = (g.rows * g.L * 32 + 255) / 256, rblocks = (Z * n * 32 + 255) / 256;
-        normalize_rows_kernel<<<wblocks, 256, 0, st>>>(g.rows * g.L, d, s_t, khat, rnorm, khat_b);
+        const FrozenRows frozen{steps, t, n * g.L};
+        normalize_rows_kernel<<<wblocks, 256, 0, st>>>(g.rows * g.L, d, s_t, khat, rnorm, khat_b, frozen);
         CKLI();
         // logits = Q Khat^T (scaled inside the softmax), dA = dC V^T
-        if (int r = attn_bwd_gemm_tc(g, m.sb, 1, 0, khat_b, 1, 0, n, d, 0, A, enc, num_sms, st, launches, err, errlen)) return r;
-        attn_softmax_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, a_b);
+        if (int r = attn_bwd_gemm_tc(g, m.sb, 1, 0, khat_b, 1, 0, n, d, 0, A, steps, t, enc, num_sms, st, launches, err,
+                                     errlen)) return r;
+        attn_softmax_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, a_b, frozen);
         CKLI();
-        if (int r = attn_bwd_gemm_tc(g, m.gsb, 1, 0, m.sb, 1, 0, n, d, 0, dA, enc, num_sms, st, launches, err, errlen)) return r;
-        attn_softmax_bwd_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, scale, dsim_b);
+        if (int r = attn_bwd_gemm_tc(g, m.gsb, 1, 0, m.sb, 1, 0, n, d, 0, dA, steps, t, enc, num_sms, st, launches, err,
+                                     errlen)) return r;
+        attn_softmax_bwd_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, scale, dsim_b,
+                                                         frozen);
         CKLI();
         // dV and dQ in one K-concatenated product: ds += [A^T | scale dsim] [dC ; Khat] ;  dKhat = (scale dsim)^T Q
-        if (int r = attn_bwd_gemm_tc(g, a_b, 0, 1, m.gsb, 1, 1, d, n, 1, ds, enc, num_sms, st, launches, err, errlen,
+        if (int r = attn_bwd_gemm_tc(g, a_b, 0, 1, m.gsb, 1, 1, d, n, 1, ds, steps, t, enc, num_sms, st, launches, err, errlen,
                                      dsim_b, 0, 0, khat_b, 1, 1)) return r;
-        if (int r = attn_bwd_gemm_tc(g, dsim_b, 0, 1, m.sb, 1, 1, d, n, 2, dkhat, enc, num_sms, st, launches, err, errlen)) return r;
-        normalize_bwd_kernel<<<wblocks, 256, 0, st>>>(g.rows * g.L, d, khat, dkhat, rnorm, ds);
+        if (int r = attn_bwd_gemm_tc(g, dsim_b, 0, 1, m.sb, 1, 1, d, n, 2, dkhat, steps, t, enc, num_sms, st, launches, err,
+                                     errlen)) return r;
+        normalize_bwd_kernel<<<wblocks, 256, 0, st>>>(g.rows * g.L, d, khat, dkhat, rnorm, ds, frozen);
         CKLI();
       }
       m.ds = ds;
       m.steps = steps; m.t = t;
       if (int r = mlp_backward_tc(g, m, enc, num_sms, st, launches, err, errlen)) return r;
       colsum_acc_kernel<<<dim3((g.L * g.d + 31) / 32, 16), 256, 0, st>>>(g.rows, g.L * g.d, (long long)g.L * g.d, gs, a.d_bu_b2,
-                                                                         a.d_td_b2, (g.L - 1) * g.d);
+                                                                         a.d_td_b2, (g.L - 1) * g.d, steps, t, g.n);
       CKLI();
     }
     gin = ds;

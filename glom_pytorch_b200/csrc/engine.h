@@ -218,8 +218,10 @@ int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int
                     char* err, size_t errlen);
 
 // (optional trailing arguments: a second product accumulated into the same output tile, see tc_bwd_kernels.cu)
+// steps (nullable): the problems of images with steps[b] <= t are skipped and their output is left as it was
 int attn_bwd_gemm_tc(const Geometry& g, const void* a_src, int a_state, int a_mn, const void* b_src, int b_state, int b_mn,
-                     int N, int K, int out_kind, float* out, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches,
+                     int N, int K, int out_kind, float* out, const int32_t* steps, int t, EncodeTiledFn enc, int num_sms,
+                     cudaStream_t st, int* launches,
                      char* err, size_t errlen, const void* a2_src = nullptr, int a2_state = 0, int a2_mn = 0,
                      const void* b2_src = nullptr, int b2_state = 0, int b2_mn = 0);
 

@@ -210,8 +210,8 @@ GLOM_B200_API int glom_b200_workspace_offset(const glom_b200_cfg* cfg, int batch
   }
 }
 
-// glom_b200_settle: a forward of max_iters steps (return_all = 0) that stops each image at the first step whose change
-// criterion is <= tol
+// glom_b200_settle / glom_b200_settle_all: a forward of max_iters steps (return_all = 0 / 1) that stops each image at the
+// first step whose change criterion is <= tol
 struct SettleRun { float tol; int32_t* steps; };
 
 static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
@@ -234,15 +234,39 @@ GLOM_B200_API int glom_b200_settle_workspace_bytes(const glom_b200_cfg* cfg, int
   return 0;
 }
 
+static int check_settle_run(float tol, const int32_t* steps_out) {
+  if (tol != tol) return fail(GLOM_B200_ERR_INVALID, "settle: tol is NaN");
+  if (!steps_out) return fail(GLOM_B200_ERR_INVALID, "settle: steps_out is NULL");
+  if (reinterpret_cast<uintptr_t>(steps_out) % 4) return fail(GLOM_B200_ERR_INVALID, "settle: steps_out must be 4-byte aligned");
+  return 0;
+}
+
 GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                                    const float* state_in, const float* init_levels, float* state_out, int batch, int max_iters,
                                    float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes, void* stream) {
   if (int r = check_settle(cfg, batch, max_iters)) return r;
-  if (tol != tol) return fail(GLOM_B200_ERR_INVALID, "settle: tol is NaN");
-  if (!steps_out) return fail(GLOM_B200_ERR_INVALID, "settle: steps_out is NULL");
-  if (reinterpret_cast<uintptr_t>(steps_out) % 4) return fail(GLOM_B200_ERR_INVALID, "settle: steps_out must be 4-byte aligned");
+  if (int r = check_settle_run(tol, steps_out)) return r;
   const SettleRun run{tol, steps_out};
   return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_iters, 0, workspace,
+                      workspace_bytes, stream, -1, &run);
+}
+
+// glom_b200_settle_all: glom_b200_settle with every state kept (the return_all form of forward_steps)
+GLOM_B200_API int glom_b200_settle_all_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_iters, size_t* out_bytes) {
+  if (int r = check_settle(cfg, batch, max_iters)) return r;
+  if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
+  *out_bytes = settle_layout(make_geometry(cfg, batch), max_iters, 1).total;
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_settle_all(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
+                                       const float* pos, const float* state_in, const float* init_levels, float* states_out,
+                                       int batch, int max_iters, float tol, int32_t* steps_out, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  if (int r = check_settle(cfg, batch, max_iters)) return r;
+  if (int r = check_settle_run(tol, steps_out)) return r;
+  const SettleRun run{tol, steps_out};
+  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, states_out, batch, max_iters, 1, workspace,
                       workspace_bytes, stream, -1, &run);
 }
 
@@ -410,14 +434,14 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
       }
     }
     // settle: image b's result S_steps[b] is in loc(steps[b]); the ones in the workspace slab move to state_out
-    if (settle) {
+    if (settle && !return_all) {
       e = launch_settle_gather(g, iters, settle->steps, wslab, state_out, nullptr, 0, st, &g_launches);
       if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle gather launch: %s", cudaGetErrorString(e));
     }
-    // forward_steps: return_all slab t of image b must be S_min(t, steps[b]); without return_all the result of an image
-    // with steps[b] == 0 is S_0, which step 0 read straight from state_in / init_levels when it ran
-    if (steps && return_all) {
-      e = launch_steps_fill(g, iters, steps, state_out, st, &g_launches);
+    // forward_steps and settle_all: return_all slab t of image b must be S_min(t, steps[b]); without return_all the result
+    // of an image with steps[b] == 0 (forward_steps only) is S_0, which step 0 read straight from state_in / init_levels
+    if ((steps || settle) && return_all) {
+      e = launch_steps_fill(g, iters, steps ? steps : settle->steps, state_out, st, &g_launches);
       if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "return_all fill launch: %s", cudaGetErrorString(e));
     } else if (steps && iters > 0) {
       e = launch_settle_gather(g, iters, steps, wslab, state_out, s0_direct ? (state_in ? state_in : init_levels) : nullptr,

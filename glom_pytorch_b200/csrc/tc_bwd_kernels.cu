@@ -64,7 +64,8 @@ struct BwdParams {
   int k_split;
   int a_mn2, b_mn2, a_state2, b_state2;
   // per-image step counts (NULL: none): at reverse step t the rows of images with steps[b] <= t have dY = 0, so BW_PRE /
-  // BW_DH / BW_DX skip a CTA's 128-row block and BW_DW a 64-row k-block when all its rows are such rows
+  // BW_DH / BW_DX skip a CTA's 128-row block and BW_DW a 64-row k-block when all its rows are such rows; BW_BATCH skips
+  // the problems of such images
   const int32_t* steps;
   int t;
 };
@@ -79,6 +80,10 @@ __device__ __forceinline__ bool rows_frozen(const BwdParams& p, int r0, int nr, 
     for (int b = r0 / p.n + lane; b <= (r1 - 1) / p.n; b += 32) live |= __ldg(p.steps + b) > p.t;
   return !__any_sync(0xffffffffu, live);
 }
+
+// BW_BATCH: problem z = image * L + level belongs to an image frozen at this step.  It depends on z alone, so the two
+// CTAs of a pair (which split one problem's rows) and every warp role skip the same tiles.
+__device__ __forceinline__ bool problem_frozen(const BwdParams& p, int z) { return __ldg(p.steps + z / p.L) <= p.t; }
 
 struct Tile {
   int g, m_blk, n_blk, num_kb;
@@ -177,6 +182,8 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
         if ((MODE == BW_PRE || MODE == BW_DH || MODE == BW_DX) && p.steps &&
             rows_frozen(p, t.m_blk * 256 + cta_rank * BM, BM, lane))
           continue;
+        if (MODE == BW_BATCH && p.steps && problem_frozen(p, t.g)) continue;
+        if (MODE == BW_DW && p.steps && rows_frozen(p, 0, p.rows, lane)) continue;     // every image frozen: no k-block runs
         for (int kb = 0; kb < t.num_kb; ++kb) {
           if (MODE == BW_DW && p.steps && rows_frozen(p, kb * BK, BK, lane)) continue;
           mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -256,6 +263,8 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
       if ((MODE == BW_PRE || MODE == BW_DH || MODE == BW_DX) && p.steps &&
           rows_frozen(p, t.m_blk * 256 + cta_rank * BM, BM, lane))
         continue;
+      if (MODE == BW_BATCH && p.steps && problem_frozen(p, t.g)) continue;
+      if (MODE == BW_DW && p.steps && rows_frozen(p, 0, p.rows, lane)) continue;
       if (MODE == BW_PRE) {
         named_bar_sync(5, CONSUMER_WARPS * 32);
         for (int i = threadIdx.x; i < BN; i += CONSUMER_WARPS * 32) bias_s[i] = __ldg(p.b1p + (size_t)t.g * 4 * p.d + t.n_blk * BN + i);
@@ -463,8 +472,8 @@ bool map3d_box(EncodeTiledFn enc, CUtensorMap* m, const void* base, uint64_t inn
 //   a2_src != nullptr: a second product A2[z] B2[z] of the same shape is accumulated into the same tile (its k blocks
 //   follow the first product's), so both land in `out` with one read-modify-write.
 int attn_bwd_gemm_tc(const Geometry& g, const void* a_src, int a_state, int a_mn, const void* b_src, int b_state, int b_mn,
-                     int N, int K, int out_kind, float* out, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches,
-                     char* err, size_t errlen, const void* a2_src, int a2_state, int a2_mn, const void* b2_src,
+                     int N, int K, int out_kind, float* out, const int32_t* steps, int t, EncodeTiledFn enc, int num_sms,
+                     cudaStream_t st, int* launches, char* err, size_t errlen, const void* a2_src, int a2_state, int a2_mn, const void* b2_src,
                      int b2_state, int b2_mn) {
   const int n = g.n, L = g.L, d = g.d, Z = g.B * L;
   CUtensorMap ma, mb, ma2, mb2;
@@ -479,6 +488,7 @@ int attn_bwd_gemm_tc(const Geometry& g, const void* a_src, int a_state, int a_mn
   BwdParams p{};
   p.rows = g.rows; p.d = d; p.L = L; p.n = n; p.G = g.G;
   p.bN = N; p.bK = K; p.a_mn = a_mn; p.b_mn = b_mn; p.a_state = a_state; p.b_state = b_state; p.out_kind = out_kind; p.out = out;
+  p.steps = steps; p.t = t;
   if (a2_src) { p.k_split = (K + BK - 1) / BK; p.a_mn2 = a2_mn; p.b_mn2 = b2_mn; p.a_state2 = a2_state; p.b_state2 = b2_state; }
   p.num_tiles = Z * ((n + 255) / 256) * ((N + BN - 1) / BN);
   cudaError_t e = launch<BW_BATCH>(ma, ma2, ma, mb, mb2, mb, p, num_sms, st);

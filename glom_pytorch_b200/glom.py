@@ -154,34 +154,63 @@ class _ColumnUpdate(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
-        module, iters = ctx.module, ctx.iters
-        tokens, pos, states, *weights = ctx.saved_tensors
-        device = states.device
-        b, n = tokens.shape[0], tokens.shape[1]
-        grad_out = grad_out.to(torch.float32).contiguous()
-        wts = [w.detach().to(torch.float32).contiguous() for w in weights]
-        zeros = torch.zeros
-        g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos),
-             "d_state0": zeros(states.shape[1:], dtype=torch.float32, device=device) if ctx.had_state0 else None,
-             "d_init": None if ctx.had_state0 else zeros(module.levels, module.dim, dtype=torch.float32, device=device)}
-        names = ("d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")
-        for k, w in zip(names, wts):
-            g[k] = zeros_like32(w)
-        with torch.cuda.device(device):
-            cfg = module.engine_cfg(n)           # bf16 engine: MLP GEMMs of the backward on tensor cores
-            ws_bytes = _native.backward_workspace_bytes(cfg, b)
-            ws = module._get_workspace(ws_bytes, device, "_bwd_workspace")      # cached across steps
-            ptrs = {k: (None if v is None else v.data_ptr()) for k, v in g.items()}
-            stream = torch.cuda.current_stream(device).cuda_stream
-            if ctx.steps is None:
-                _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
-                                 grad_out.data_ptr(), ptrs, b, iters, ctx.return_all, ws.data_ptr(), ws.numel(), stream)
-            else:
-                _native.backward_steps(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(),
-                                       states.data_ptr(), grad_out.data_ptr(), ptrs, b, ctx.steps.data_ptr(), iters,
-                                       ctx.return_all, ws.data_ptr(), ws.numel(), stream)
-        return (None, None, None, None, g["d_tokens"], g["d_pos"], g["d_state0"] if ctx.want_state0 else None, g["d_init"],
-                *[g[k] for k in names])
+        return (None, None, None, None, *_loop_backward(ctx, grad_out))
+
+
+def _loop_backward(ctx, grad_out):
+    """Backward of the loop for _ColumnUpdate and _Settle: ctx holds module, iters, return_all, steps (None or the
+    engine's private int32 copy), had_state0 / want_state0 and the saved (tokens, pos, states, *weights).  Returns the
+    gradients of (tokens, pos, state0, init_levels, *weights)."""
+    module, iters = ctx.module, ctx.iters
+    tokens, pos, states, *weights = ctx.saved_tensors
+    device = states.device
+    b, n = tokens.shape[0], tokens.shape[1]
+    grad_out = grad_out.to(torch.float32).contiguous()
+    wts = [w.detach().to(torch.float32).contiguous() for w in weights]
+    zeros = torch.zeros
+    g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos),
+         "d_state0": zeros(states.shape[1:], dtype=torch.float32, device=device) if ctx.had_state0 else None,
+         "d_init": None if ctx.had_state0 else zeros(module.levels, module.dim, dtype=torch.float32, device=device)}
+    names = ("d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")
+    for k, w in zip(names, wts):
+        g[k] = zeros_like32(w)
+    with torch.cuda.device(device):
+        cfg = module.engine_cfg(n)           # bf16 engine: MLP GEMMs of the backward on tensor cores
+        ws_bytes = _native.backward_workspace_bytes(cfg, b)
+        ws = module._get_workspace(ws_bytes, device, "_bwd_workspace")      # cached across steps
+        ptrs = {k: (None if v is None else v.data_ptr()) for k, v in g.items()}
+        stream = torch.cuda.current_stream(device).cuda_stream
+        if ctx.steps is None:
+            _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
+                             grad_out.data_ptr(), ptrs, b, iters, ctx.return_all, ws.data_ptr(), ws.numel(), stream)
+        else:
+            _native.backward_steps(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(),
+                                   states.data_ptr(), grad_out.data_ptr(), ptrs, b, ctx.steps.data_ptr(), iters,
+                                   ctx.return_all, ws.data_ptr(), ws.numel(), stream)
+    return (g["d_tokens"], g["d_pos"], g["d_state0"] if ctx.want_state0 else None, g["d_init"], *[g[k] for k in names])
+
+
+class _Settle(torch.autograd.Function):
+    """Glom.settle(differentiable=True): forward = glom_b200_settle_all (every state kept, each image stopped on the
+    GPU), backward = glom_b200_backward_steps with max_steps = max_iters and the settle's own step counts, which are
+    constants of the backward exactly as in forward(iters=steps).  Outputs (levels, steps); steps is not differentiable."""
+
+    @staticmethod
+    def forward(ctx, module, max_iters, tol, return_all, tokens, pos, state0, init_levels, *weights):
+        tokens, pos = tokens.contiguous(), pos.contiguous()
+        states, steps = module._run_settle(tokens, pos, state0, init_levels, max_iters, tol, True)
+        # the backward reads its own copy: an in-place edit of the returned steps changes no gradient
+        ctx.module, ctx.iters, ctx.return_all, ctx.steps = module, max_iters, return_all, steps.clone()
+        ctx.had_state0 = state0 is not None
+        ctx.want_state0 = state0 is not None and state0.requires_grad
+        ctx.save_for_backward(tokens, pos, states, *weights)
+        ctx.mark_non_differentiable(steps)
+        return (states if return_all else states[max_iters]), steps
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out, _grad_steps):
+        return (None, None, None, None, *_loop_backward(ctx, grad_out))
 
 
 def zeros_like32(t):
@@ -510,9 +539,7 @@ class Glom(nn.Module):
                                "move the module and inputs to an H100")
         if steps is not None:    # the engine's own int32 copy: later in-place edits of the caller's tensor change nothing
             steps = steps.to(device=img.device, dtype=torch.int32, copy=True)
-        needs_grad = torch.is_grad_enabled() and (
-            img.requires_grad or (levels is not None and levels.requires_grad)
-            or any(p.requires_grad for p in self.parameters()))
+        needs_grad = self._needs_grad(img, levels)
         p = self.patch_size
         if img.dim() != 4 or img.shape[1] != 3 or img.shape[2] % p or img.shape[3] % p:
             raise RuntimeError(f"image {tuple(img.shape)} is not (B, 3, H, W) with H, W multiples of {p}")
@@ -532,18 +559,24 @@ class Glom(nn.Module):
                                     allow_resume=not self.training)
         # training: the tokeniser and the loop are the engine's differentiable ops (the same kernels as without autograd);
         # only the parameter views (pos_emb slice) are plain torch ops
-        lin = self.image_to_tokens[1]
-        if self.use_native_tokenizer:
-            tokens = _Tokenize.apply(self, img, lin.weight, lin.bias)                            # (:114)
-        else:
-            self._tok_launches = 0
-            tokens = lin(self.image_to_tokens[0](img.float()))
+        tokens = self._differentiable_tokens(img)                                               # (:114)
         pos = self.pos_emb.weight[:n]                                                            # (:117)
         state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
         return _ColumnUpdate.apply(self, iters, steps, return_all, tokens, pos, state0, self.init_levels, *self._mlp_params())
 
+    def _differentiable_tokens(self, img):
+        lin = self.image_to_tokens[1]
+        if self.use_native_tokenizer:
+            return _Tokenize.apply(self, img, lin.weight, lin.bias)
+        self._tok_launches = 0
+        return lin(self.image_to_tokens[0](img.float()))
+
+    def _needs_grad(self, img, levels):
+        return torch.is_grad_enabled() and (img.requires_grad or (levels is not None and levels.requires_grad)
+                                            or any(p.requires_grad for p in self.parameters()))
+
     # ------------------------------------------------------------------ inference until the columns settle
-    def settle(self, img, tol, max_iters=None, levels=None):
+    def settle(self, img, tol, max_iters=None, levels=None, *, return_all=False, differentiable=False):
         """Run each image's column update until its levels stop changing -> ``(levels, steps)``.
 
         After step k the change of image b is ``max_l sqrt(sum_i |S_k[b,i,l] - S_{k-1}[b,i,l]|^2 / sum_i |S_k[b,i,l]|^2)``
@@ -551,16 +584,27 @@ class Glom(nn.Module):
         S_k, bit-identical to ``forward(img, iters=k, levels=same_start)[b]`` on the same batch, and ``steps[b] = k``.
         Images that never meet the rule run ``max_iters`` steps (``None`` = 2L as in ``forward``).  The stopping decisions
         are taken on the GPU inside the call: ``steps`` is a (B,) int32 CUDA tensor the host never reads, so the call does
-        not synchronise.  Inference only (raises if autograd would be needed), bf16 engine only."""
+        not synchronise.  bf16 engine only.
+
+        ``return_all=True`` returns every state, ``(max_iters+1, B, n, L, d)``: slab t of image b is S_min(t, steps[b]),
+        as in ``forward(iters=steps, return_all=True)``, with the same ``steps``.
+
+        By default settle is inference only and raises if autograd would be needed.  With ``differentiable=True`` it
+        settles and trains in one forward: under autograd the result is differentiable exactly like
+        ``forward(img, iters=steps, levels=levels, return_all=return_all)`` with the steps as constants, but without
+        running the steps a second time and without a host read of ``steps``.  The returned ``steps`` is not
+        differentiable; the backward keeps its own copy.  That path holds all max_iters+1 states in fp32 until the
+        backward, with or without ``return_all``: about 1.3 GB at dim 512, 6 levels, 256 patches, batch 32 and
+        max_iters 12.  Without autograd ``differentiable`` changes nothing."""
         if self.precision != "bf16":
             raise RuntimeError("Glom.settle needs precision='bf16' (the fp32 engine has no early stopping)")
         if not img.is_cuda:
             raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
                                "move the module and inputs to an H100")
-        if torch.is_grad_enabled() and (img.requires_grad or (levels is not None and levels.requires_grad)
-                                        or any(p.requires_grad for p in self.parameters())):
+        needs_grad = self._needs_grad(img, levels)
+        if needs_grad and not differentiable:
             raise RuntimeError("Glom.settle is inference only: call it under torch.no_grad() / torch.inference_mode() "
-                               "or with parameters and inputs that do not require grad")
+                               "or with parameters and inputs that do not require grad, or pass differentiable=True")
         max_iters = self.levels * 2 if max_iters is None else int(max_iters)
         if max_iters < 1:
             raise ValueError(f"max_iters must be >= 1, got {max_iters}")
@@ -575,25 +619,39 @@ class Glom(nn.Module):
             raise IndexError(f"{n} patches exceed pos_emb size {self.pos_emb.num_embeddings}")
         if levels is not None and tuple(levels.shape) != (b, n, self.levels, self.dim):
             raise RuntimeError(f"levels must have shape {(b, n, self.levels, self.dim)}, got {tuple(levels.shape)}")
+        if needs_grad:
+            tokens = self._differentiable_tokens(img)
+            pos = self.pos_emb.weight[:n]
+            state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
+            return _Settle.apply(self, max_iters, tol, return_all, tokens, pos, state0, self.init_levels,
+                                 *self._mlp_params())
         tokens = self._take_staged(img)
         if tokens is None:
             tokens = self.tokens(img)
+        return self._run_settle(tokens, self.pos_emb.weight[:n], levels, self.init_levels, max_iters, tol, return_all)
+
+    def _run_settle(self, tokens, pos, state_in, init, max_iters, tol, return_all):
+        """glom_b200_settle (return_all: glom_b200_settle_all) -> (levels or all states, steps).  The workspace shadows
+        of stopped images are stale afterwards: the next forward takes the ordinary state prologue."""
         device = tokens.device
-        # the workspace shadows of stopped images are stale: the next forward must take the ordinary state prologue
+        b, n = tokens.shape[0], tokens.shape[1]
         self._resume = None
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
             tokens = tokens.detach().to(torch.float32).contiguous()
-            pos = self.pos_emb.weight[:n].detach().to(torch.float32).contiguous()
-            init = self.init_levels.detach().to(torch.float32).contiguous()
-            state_in = None if levels is None else levels.detach().to(device=device, dtype=torch.float32).contiguous()
+            pos = pos.detach().to(torch.float32).contiguous()
+            init = init.detach().to(torch.float32).contiguous()
+            if state_in is not None:
+                state_in = state_in.detach().to(device=device, dtype=torch.float32).contiguous()
             cfg = self.engine_cfg(n)
             packed = self._packed_weights(cfg, device, stream)
-            out = torch.empty((b, n, self.levels, self.dim), dtype=torch.float32, device=device)
+            shape = (b, n, self.levels, self.dim)
+            out = torch.empty(((max_iters + 1,) + shape) if return_all else shape, dtype=torch.float32, device=device)
             steps = torch.empty(b, dtype=torch.int32, device=device)
-            ws = self._get_workspace(_native.settle_workspace_bytes(cfg, b, max_iters), device)
-            _native.settle(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(),
-                           None if state_in is None else state_in.data_ptr(), init.data_ptr(), out.data_ptr(), b,
-                           max_iters, tol, steps.data_ptr(), ws.data_ptr(), ws.numel(), stream)
+            run = _native.settle_all if return_all else _native.settle
+            ws_bytes = (_native.settle_all_workspace_bytes if return_all else _native.settle_workspace_bytes)(cfg, b, max_iters)
+            ws = self._get_workspace(ws_bytes, device)
+            run(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), None if state_in is None else state_in.data_ptr(),
+                init.data_ptr(), out.data_ptr(), b, max_iters, tol, steps.data_ptr(), ws.data_ptr(), ws.numel(), stream)
             self.last_launches = _native.last_launch_count() + getattr(self, "_tok_launches", 0)
         return out, steps

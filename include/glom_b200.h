@@ -136,6 +136,17 @@ GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_
                                    const float* state_in, const float* init_levels, float* state_out, int batch,
                                    int max_iters, float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes,
                                    void* stream);
+/* glom_b200_settle that keeps every state, for training through settle (its backward is glom_b200_backward_steps with
+ * max_steps = max_iters and this call's steps_out) and for analysis of a settled run.  The stopping rule, steps_out and
+ * the argument errors (reported before any device query) are those of glom_b200_settle.
+ *   states_out (max_iters+1, B, n, L, d) fp32: slab t of image b is S_min(t, steps_out[b]), slab 0 is S_0 -- the
+ *   return_all form of glom_b200_forward_steps.
+ * The workspace (1024-byte aligned) is that of glom_b200_forward_steps(max_steps = max_iters, return_all = 1). */
+GLOM_B200_API int glom_b200_settle_all_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_iters, size_t* out_bytes);
+GLOM_B200_API int glom_b200_settle_all(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
+                                       const float* pos, const float* state_in, const float* init_levels, float* states_out,
+                                       int batch, int max_iters, float tol, int32_t* steps_out, void* workspace,
+                                       size_t workspace_bytes, void* stream);
 
 /* Per-image step counts.  bf16 engine only.  The forward of glom_b200_forward run for max_steps (>= 0) steps from the same
  * start (state_in, or init_levels broadcast), in which image b stops after steps[b] steps: its later steps skip its work
@@ -204,8 +215,9 @@ GLOM_B200_API int glom_b200_backward(const glom_b200_cfg* cfg, const glom_b200_w
 /* Backward of glom_b200_forward_steps(return_all = 1): the same as glom_b200_backward with iters = max_steps, for the
  * per-image program in which image b is the identity at every step t >= steps[b] (steps: the forward's (B) int32 device
  * array).  At such a step the image's upstream gradient passes through unchanged and it adds nothing to any parameter,
- * pos or token gradient; the MLP GEMMs of the tensor-core backward skip row blocks made only of such rows.  `states` is
- * the forward_steps return_all output.  Same workspace as glom_b200_backward. */
+ * pos or token gradient; the MLP GEMMs of the tensor-core backward skip row blocks made only of such rows, and its
+ * consensus-attention backward skips such images entirely.  `states` is the return_all output of forward_steps or
+ * settle_all.  Same workspace as glom_b200_backward. */
 GLOM_B200_API int glom_b200_backward_steps(const glom_b200_cfg* cfg, const glom_b200_weights_ref* weights,
                                            const float* tokens, const float* pos, const float* states, const float* grad_out,
                                            const glom_b200_grads* grads, int batch, const int32_t* steps, int max_steps,
