@@ -9,19 +9,6 @@ LIB_PATH = os.environ.get("GLOM_B200_LIB") or os.path.join(_PKG, "libglom_b200.s
 
 ABI_VERSION = 1
 PRECISION = {"fp32": 0, "bf16": 1}
-
-EXPORTS = (
-    "glom_b200_abi_version", "glom_b200_last_error", "glom_b200_packed_weight_bytes",
-    "glom_b200_pack_weights", "glom_b200_workspace_bytes", "glom_b200_forward", "glom_b200_forward_resume",
-    "glom_b200_tokenize", "glom_b200_tokenize_workspace_bytes", "glom_b200_last_launch_count", "glom_b200_workspace_offset",
-    "glom_b200_profile_begin", "glom_b200_profile_end",
-    "glom_b200_backward", "glom_b200_backward_workspace_bytes",
-    "glom_b200_tokenize_backward", "glom_b200_tokenize_backward_workspace_bytes",
-    "glom_b200_clock_probe", "glom_b200_mlp_schedule", "glom_b200_islands", "glom_b200_kernel_clocks",
-    "glom_b200_settle", "glom_b200_settle_workspace_bytes",
-    "glom_b200_forward_steps", "glom_b200_forward_steps_workspace_bytes", "glom_b200_backward_steps",
-    "glom_b200_settle_all", "glom_b200_settle_all_workspace_bytes",
-)
 PROFILE_KINDS = ("attention", "gemm1_gelu", "gemm2_combine", "prologue", "tokenize", "mlp_fused")
 
 
@@ -42,6 +29,45 @@ class Grads(ctypes.Structure):
                                        "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")]
 
 
+_vp, _sz, _i32, _f32 = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_float
+_CFG, _W, _G = ctypes.POINTER(Cfg), ctypes.POINTER(WeightsRef), ctypes.POINTER(Grads)
+_SZP, _I32P = ctypes.POINTER(_sz), ctypes.POINTER(_i32)
+_SETTLE = [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _vp, _vp, _sz, _vp]
+
+# every symbol of include/glom_b200.h: name -> (restype, argtypes)
+SIGNATURES = {
+    "glom_b200_abi_version": (_i32, []),
+    "glom_b200_last_error": (ctypes.c_char_p, []),
+    "glom_b200_packed_weight_bytes": (_i32, [_CFG, _SZP]),
+    "glom_b200_pack_weights": (_i32, [_CFG, _W, _vp, _sz, _vp]),
+    "glom_b200_workspace_bytes": (_i32, [_CFG, _i32, _i32, _i32, _SZP]),
+    "glom_b200_forward": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_forward_resume": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _sz, _vp, _i32, _I32P]),
+    "glom_b200_settle_workspace_bytes": (_i32, [_CFG, _i32, _i32, _SZP]),
+    "glom_b200_settle": (_i32, _SETTLE),
+    "glom_b200_settle_all_workspace_bytes": (_i32, [_CFG, _i32, _i32, _SZP]),
+    "glom_b200_settle_all": (_i32, _SETTLE),
+    "glom_b200_forward_steps_workspace_bytes": (_i32, [_CFG, _i32, _i32, _i32, _SZP]),
+    "glom_b200_forward_steps": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_tokenize_workspace_bytes": (_i32, [_i32, _i32, _i32, _i32, _i32, _i32, _SZP]),
+    "glom_b200_tokenize": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_last_launch_count": (_i32, []),
+    "glom_b200_workspace_offset": (_i32, [_CFG, _i32, _i32, _i32, _i32, _SZP, _SZP]),
+    "glom_b200_backward_workspace_bytes": (_i32, [_CFG, _i32, _SZP]),
+    "glom_b200_backward": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_backward_steps": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _vp, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_tokenize_backward_workspace_bytes": (_i32, [_i32, _i32, _i32, _i32, _i32, _SZP]),
+    "glom_b200_tokenize_backward": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_profile_begin": (_i32, []),
+    "glom_b200_profile_end": (_i32, [ctypes.POINTER(ctypes.c_double), _I32P, _i32]),
+    "glom_b200_islands": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "glom_b200_mlp_schedule": (_i32, [_CFG, _i32, _i32, _vp, _i32, _I32P, _I32P]),
+    "glom_b200_clock_probe": (_i32, [_vp, _i32, _vp]),
+    "glom_b200_kernel_clocks": (_i32, [_vp, _vp, _vp, _i32, _i32]),
+}
+EXPORTS = tuple(SIGNATURES)
+
+
 class GlomB200Error(RuntimeError):
     pass
 
@@ -59,61 +85,9 @@ def load():
             f"{LIB_PATH} not found: build it with `python -m glom_pytorch_b200.build` "
             "(nvcc, sm_90a). There is no CPU or PyTorch fallback for the GLOM column update.")
     lib = ctypes.CDLL(LIB_PATH)
-    vp, sz, i32 = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
-    lib.glom_b200_abi_version.restype = i32
-    lib.glom_b200_last_error.restype = ctypes.c_char_p
-    lib.glom_b200_last_launch_count.restype = i32
-    lib.glom_b200_packed_weight_bytes.argtypes = [ctypes.POINTER(Cfg), ctypes.POINTER(sz)]
-    lib.glom_b200_pack_weights.argtypes = [ctypes.POINTER(Cfg), ctypes.POINTER(WeightsRef), vp, sz, vp]
-    lib.glom_b200_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, i32, i32, ctypes.POINTER(sz)]
-    lib.glom_b200_workspace_offset.argtypes = [ctypes.POINTER(Cfg), i32, i32, i32, i32,
-                                               ctypes.POINTER(sz), ctypes.POINTER(sz)]
-    lib.glom_b200_forward.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, sz, vp]
-    lib.glom_b200_tokenize.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, sz, vp]
-    lib.glom_b200_tokenize_workspace_bytes.argtypes = [i32, i32, i32, i32, i32, i32, ctypes.POINTER(sz)]
-    lib.glom_b200_tokenize_workspace_bytes.restype = i32
-    lib.glom_b200_profile_begin.restype = i32
-    lib.glom_b200_profile_end.argtypes = [ctypes.POINTER(ctypes.c_double), ctypes.POINTER(i32), i32]
-    lib.glom_b200_profile_end.restype = i32
-    lib.glom_b200_backward_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, ctypes.POINTER(sz)]
-    lib.glom_b200_backward_workspace_bytes.restype = i32
-    lib.glom_b200_backward.argtypes = [ctypes.POINTER(Cfg), ctypes.POINTER(WeightsRef), vp, vp, vp, vp,
-                                       ctypes.POINTER(Grads), i32, i32, i32, vp, sz, vp]
-    lib.glom_b200_backward.restype = i32
-    lib.glom_b200_mlp_schedule.argtypes = [ctypes.POINTER(Cfg), i32, i32, vp, i32, ctypes.POINTER(i32), ctypes.POINTER(i32)]
-    lib.glom_b200_mlp_schedule.restype = i32
-    lib.glom_b200_islands.argtypes = [vp, i32, i32, i32, i32, i32, ctypes.c_float, vp, vp, vp, vp, vp, vp]
-    lib.glom_b200_islands.restype = i32
-    lib.glom_b200_tokenize_backward_workspace_bytes.argtypes = [i32, i32, i32, i32, i32, ctypes.POINTER(sz)]
-    lib.glom_b200_tokenize_backward_workspace_bytes.restype = i32
-    lib.glom_b200_tokenize_backward.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, sz, vp]
-    lib.glom_b200_tokenize_backward.restype = i32
-    lib.glom_b200_forward_resume.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, i32, i32, i32, vp, sz, vp, i32,
-                                             ctypes.POINTER(i32)]
-    lib.glom_b200_forward_resume.restype = i32
-    lib.glom_b200_clock_probe.argtypes = [vp, i32, vp]
-    lib.glom_b200_clock_probe.restype = i32
-    lib.glom_b200_kernel_clocks.argtypes = [vp, vp, vp, i32, i32]
-    lib.glom_b200_kernel_clocks.restype = i32
-    lib.glom_b200_settle_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, i32, ctypes.POINTER(sz)]
-    lib.glom_b200_settle_workspace_bytes.restype = i32
-    lib.glom_b200_settle.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, vp, sz, vp]
-    lib.glom_b200_settle.restype = i32
-    lib.glom_b200_settle_all_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, i32, ctypes.POINTER(sz)]
-    lib.glom_b200_settle_all_workspace_bytes.restype = i32
-    lib.glom_b200_settle_all.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, i32, ctypes.c_float, vp, vp, sz,
-                                         vp]
-    lib.glom_b200_settle_all.restype = i32
-    lib.glom_b200_forward_steps_workspace_bytes.argtypes = [ctypes.POINTER(Cfg), i32, i32, i32, ctypes.POINTER(sz)]
-    lib.glom_b200_forward_steps_workspace_bytes.restype = i32
-    lib.glom_b200_forward_steps.argtypes = [ctypes.POINTER(Cfg), vp, vp, vp, vp, vp, vp, i32, vp, i32, i32, vp, sz, vp]
-    lib.glom_b200_forward_steps.restype = i32
-    lib.glom_b200_backward_steps.argtypes = [ctypes.POINTER(Cfg), ctypes.POINTER(WeightsRef), vp, vp, vp, vp,
-                                             ctypes.POINTER(Grads), i32, vp, i32, i32, vp, sz, vp]
-    lib.glom_b200_backward_steps.restype = i32
-    for f in ("glom_b200_packed_weight_bytes", "glom_b200_pack_weights", "glom_b200_workspace_bytes",
-              "glom_b200_workspace_offset", "glom_b200_forward", "glom_b200_tokenize"):
-        getattr(lib, f).restype = i32
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if lib.glom_b200_abi_version() != ABI_VERSION:
         raise GlomB200Error(f"libglom_b200 ABI {lib.glom_b200_abi_version()} != expected {ABI_VERSION}")
     _lib = lib
@@ -130,16 +104,19 @@ def make_cfg(dim, levels, n, attend_self, mask_side, mask_d2_max, precision):
                PRECISION[precision])
 
 
-def packed_weight_bytes(cfg):
+def _bytes(symbol, *args):
+    """The size_t that a *_bytes entry point writes through its last argument."""
     out = ctypes.c_size_t()
-    check(load().glom_b200_packed_weight_bytes(ctypes.byref(cfg), ctypes.byref(out)))
+    check(getattr(load(), symbol)(*args, ctypes.byref(out)))
     return out.value
+
+
+def packed_weight_bytes(cfg):
+    return _bytes("glom_b200_packed_weight_bytes", ctypes.byref(cfg))
 
 
 def workspace_bytes(cfg, batch, iters, return_all):
-    out = ctypes.c_size_t()
-    check(load().glom_b200_workspace_bytes(ctypes.byref(cfg), batch, iters, int(return_all), ctypes.byref(out)))
-    return out.value
+    return _bytes("glom_b200_workspace_bytes", ctypes.byref(cfg), batch, iters, int(return_all))
 
 
 def workspace_offset(cfg, batch, iters, return_all, which):
@@ -161,10 +138,7 @@ def forward(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_pt
 
 
 def tokenize_workspace_bytes(batch, height, width, patch, dim, precision):
-    out = ctypes.c_size_t()
-    check(load().glom_b200_tokenize_workspace_bytes(batch, height, width, patch, dim, PRECISION[precision],
-                                                    ctypes.byref(out)))
-    return out.value
+    return _bytes("glom_b200_tokenize_workspace_bytes", batch, height, width, patch, dim, PRECISION[precision])
 
 
 def tokenize(img_ptr, w_ptr, b_ptr, out_ptr, batch, height, width, patch, dim, precision, ws_ptr, ws_bytes, stream):
@@ -199,37 +173,26 @@ def forward_resume(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, out_ptr, 
 
 
 def settle_workspace_bytes(cfg, batch, max_iters):
-    out = ctypes.c_size_t()
-    check(load().glom_b200_settle_workspace_bytes(ctypes.byref(cfg), batch, max_iters, ctypes.byref(out)))
-    return out.value
-
-
-def settle(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, max_iters, tol, steps_ptr,
-           ws_ptr, ws_bytes, stream):
-    """glom_b200_settle: up to max_iters steps, each image stopped on the GPU; steps_ptr -> (batch,) int32 device words."""
-    check(load().glom_b200_settle(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch,
-                                  max_iters, float(tol), steps_ptr, ws_ptr, ws_bytes, stream))
+    return _bytes("glom_b200_settle_workspace_bytes", ctypes.byref(cfg), batch, max_iters)
 
 
 def settle_all_workspace_bytes(cfg, batch, max_iters):
-    out = ctypes.c_size_t()
-    check(load().glom_b200_settle_all_workspace_bytes(ctypes.byref(cfg), batch, max_iters, ctypes.byref(out)))
-    return out.value
-
-
-def settle_all(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, max_iters, tol, steps_ptr,
-               ws_ptr, ws_bytes, stream):
-    """glom_b200_settle_all: settle() with every state kept; out_ptr -> (max_iters+1, batch, n, L, d) fp32, slab t of
-    image b = S_min(t, steps[b])."""
-    check(load().glom_b200_settle_all(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr,
-                                      batch, max_iters, float(tol), steps_ptr, ws_ptr, ws_bytes, stream))
+    return _bytes("glom_b200_settle_all_workspace_bytes", ctypes.byref(cfg), batch, max_iters)
 
 
 def forward_steps_workspace_bytes(cfg, batch, max_steps, return_all):
-    out = ctypes.c_size_t()
-    check(load().glom_b200_forward_steps_workspace_bytes(ctypes.byref(cfg), batch, max_steps, int(bool(return_all)),
-                                                         ctypes.byref(out)))
-    return out.value
+    return _bytes("glom_b200_forward_steps_workspace_bytes", ctypes.byref(cfg), batch, max_steps, int(bool(return_all)))
+
+
+def settle(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, max_iters, return_all, tol,
+           steps_ptr, ws_ptr, ws_bytes, stream):
+    """glom_b200_settle: up to max_iters steps, each image stopped on the GPU; steps_ptr -> (batch,) int32 device words.
+    return_all: glom_b200_settle_all, every state kept; out_ptr -> (max_iters+1, batch, n, L, d) fp32, slab t of image b
+    = S_min(t, steps[b])."""
+    lib = load()
+    fn = lib.glom_b200_settle_all if return_all else lib.glom_b200_settle
+    check(fn(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, max_iters,
+             float(tol), steps_ptr, ws_ptr, ws_bytes, stream))
 
 
 def forward_steps(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, steps_ptr, max_steps,
@@ -240,37 +203,30 @@ def forward_steps(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, 
                                          batch, steps_ptr, max_steps, int(bool(return_all)), ws_ptr, ws_bytes, stream))
 
 
-def backward_steps(cfg, weight_ptrs, tokens_ptr, pos_ptr, states_ptr, grad_out_ptr, grad_ptrs, batch, steps_ptr, max_steps,
-                   grad_all, ws_ptr, ws_bytes, stream):
-    """glom_b200_backward_steps: the backward of forward_steps(return_all=1); arguments as for backward()."""
-    w = WeightsRef(ctypes.sizeof(WeightsRef), *weight_ptrs)
-    g = Grads(ctypes.sizeof(Grads), *[grad_ptrs.get(k) for k, _ in Grads._fields_[1:]])
-    check(load().glom_b200_backward_steps(ctypes.byref(cfg), ctypes.byref(w), tokens_ptr, pos_ptr, states_ptr,
-                                          grad_out_ptr, ctypes.byref(g), batch, steps_ptr, max_steps, int(grad_all),
-                                          ws_ptr, ws_bytes, stream))
-
-
 def backward_workspace_bytes(cfg, batch):
-    out = ctypes.c_size_t()
-    check(load().glom_b200_backward_workspace_bytes(ctypes.byref(cfg), batch, ctypes.byref(out)))
-    return out.value
+    return _bytes("glom_b200_backward_workspace_bytes", ctypes.byref(cfg), batch)
 
 
 def backward(cfg, weight_ptrs, tokens_ptr, pos_ptr, states_ptr, grad_out_ptr, grad_ptrs, batch, iters, grad_all,
-             ws_ptr, ws_bytes, stream):
+             ws_ptr, ws_bytes, stream, steps_ptr=None):
     """weight_ptrs: the 8 reference-layout tensors; grad_ptrs: dict of the Grads fields (None allowed for
-    d_state0 / d_init)."""
+    d_state0 / d_init).  With steps_ptr (the forward's (batch,) int32 step vector, iters = max_steps):
+    glom_b200_backward_steps, the backward of forward_steps / settle_all."""
     w = WeightsRef(ctypes.sizeof(WeightsRef), *weight_ptrs)
     g = Grads(ctypes.sizeof(Grads), *[grad_ptrs.get(k) for k, _ in Grads._fields_[1:]])
-    check(load().glom_b200_backward(ctypes.byref(cfg), ctypes.byref(w), tokens_ptr, pos_ptr, states_ptr,
-                                    grad_out_ptr, ctypes.byref(g), batch, iters, int(grad_all), ws_ptr, ws_bytes,
-                                    stream))
+    lib = load()
+    if steps_ptr is None:
+        rc = lib.glom_b200_backward(ctypes.byref(cfg), ctypes.byref(w), tokens_ptr, pos_ptr, states_ptr, grad_out_ptr,
+                                    ctypes.byref(g), batch, iters, int(grad_all), ws_ptr, ws_bytes, stream)
+    else:
+        rc = lib.glom_b200_backward_steps(ctypes.byref(cfg), ctypes.byref(w), tokens_ptr, pos_ptr, states_ptr,
+                                          grad_out_ptr, ctypes.byref(g), batch, steps_ptr, iters, int(grad_all), ws_ptr,
+                                          ws_bytes, stream)
+    check(rc)
 
 
 def tokenize_backward_workspace_bytes(batch, h, w, patch, need_d_img):
-    n = ctypes.c_size_t(0)
-    check(load().glom_b200_tokenize_backward_workspace_bytes(batch, h, w, patch, int(bool(need_d_img)), ctypes.byref(n)))
-    return n.value
+    return _bytes("glom_b200_tokenize_backward_workspace_bytes", batch, h, w, patch, int(bool(need_d_img)))
 
 
 def tokenize_backward(img_ptr, weight_ptr, d_tokens_ptr, d_weight_ptr, d_bias_ptr, d_img_ptr, batch, h, w, patch, dim,

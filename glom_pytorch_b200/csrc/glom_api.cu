@@ -219,81 +219,80 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
                         int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity,
                         const SettleRun* settle = nullptr, const int32_t* steps = nullptr);
 
-static int check_settle(const glom_b200_cfg* cfg, int batch, int max_iters) {
+// The freeze modes: settle / settle_all (bound max_iters >= 1) and forward_steps (bound max_steps >= 0) run the bf16
+// engine's SETTLE step kernels.  Their workspace is the forward's plus the freeze flags (settle_layout).
+struct FreezeMode { const char* name; const char* bound; int min_bound; };
+static const FreezeMode kSettle{"settle", "max_iters", 1}, kForwardSteps{"forward_steps", "max_steps", 0};
+
+static int check_freeze(const FreezeMode& m, const glom_b200_cfg* cfg, int batch, int bound) {
   if (int r = check_cfg(cfg)) return r;
-  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "settle: bf16 engine only (precision fp32 given)");
-  if (batch < 1) return fail(GLOM_B200_ERR_INVALID, "settle: batch must be >= 1 (got %d)", batch);
-  if (max_iters < 1) return fail(GLOM_B200_ERR_INVALID, "settle: max_iters must be >= 1 (got %d)", max_iters);
+  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "%s: bf16 engine only (precision fp32 given)", m.name);
+  if (batch < 1) return fail(GLOM_B200_ERR_INVALID, "%s: batch must be >= 1 (got %d)", m.name, batch);
+  if (bound < m.min_bound) return fail(GLOM_B200_ERR_INVALID, "%s: %s must be >= %d (got %d)", m.name, m.bound, m.min_bound, bound);
   return 0;
+}
+
+static int freeze_workspace_bytes(const FreezeMode& m, const glom_b200_cfg* cfg, int batch, int bound, int return_all,
+                                  size_t* out_bytes) {
+  if (int r = check_freeze(m, cfg, batch, bound)) return r;
+  if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
+  *out_bytes = settle_layout(make_geometry(cfg, batch), bound, return_all ? 1 : 0).total;
+  return 0;
+}
+
+static int check_steps_ptr(const char* fn, const char* arg, const int32_t* steps) {
+  if (!steps) return fail(GLOM_B200_ERR_INVALID, "%s: %s is NULL", fn, arg);
+  if (reinterpret_cast<uintptr_t>(steps) % 4) return fail(GLOM_B200_ERR_INVALID, "%s: %s must be 4-byte aligned", fn, arg);
+  return 0;
+}
+
+static int settle_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
+                       const float* state_in, const float* init_levels, float* state_out, int batch, int max_iters,
+                       int return_all, float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int r = check_freeze(kSettle, cfg, batch, max_iters)) return r;
+  if (tol != tol) return fail(GLOM_B200_ERR_INVALID, "settle: tol is NaN");
+  if (int r = check_steps_ptr("settle", "steps_out", steps_out)) return r;
+  const SettleRun run{tol, steps_out};
+  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_iters, return_all,
+                      workspace, workspace_bytes, stream, -1, &run);
 }
 
 GLOM_B200_API int glom_b200_settle_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_iters, size_t* out_bytes) {
-  if (int r = check_settle(cfg, batch, max_iters)) return r;
-  if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
-  *out_bytes = settle_layout(make_geometry(cfg, batch), max_iters).total;
-  return 0;
-}
-
-static int check_settle_run(float tol, const int32_t* steps_out) {
-  if (tol != tol) return fail(GLOM_B200_ERR_INVALID, "settle: tol is NaN");
-  if (!steps_out) return fail(GLOM_B200_ERR_INVALID, "settle: steps_out is NULL");
-  if (reinterpret_cast<uintptr_t>(steps_out) % 4) return fail(GLOM_B200_ERR_INVALID, "settle: steps_out must be 4-byte aligned");
-  return 0;
+  return freeze_workspace_bytes(kSettle, cfg, batch, max_iters, 0, out_bytes);
 }
 
 GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                                    const float* state_in, const float* init_levels, float* state_out, int batch, int max_iters,
                                    float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes, void* stream) {
-  if (int r = check_settle(cfg, batch, max_iters)) return r;
-  if (int r = check_settle_run(tol, steps_out)) return r;
-  const SettleRun run{tol, steps_out};
-  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_iters, 0, workspace,
-                      workspace_bytes, stream, -1, &run);
+  return settle_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_iters, 0, tol, steps_out,
+                     workspace, workspace_bytes, stream);
 }
 
 // glom_b200_settle_all: glom_b200_settle with every state kept (the return_all form of forward_steps)
 GLOM_B200_API int glom_b200_settle_all_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_iters, size_t* out_bytes) {
-  if (int r = check_settle(cfg, batch, max_iters)) return r;
-  if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
-  *out_bytes = settle_layout(make_geometry(cfg, batch), max_iters, 1).total;
-  return 0;
+  return freeze_workspace_bytes(kSettle, cfg, batch, max_iters, 1, out_bytes);
 }
 
 GLOM_B200_API int glom_b200_settle_all(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
                                        const float* pos, const float* state_in, const float* init_levels, float* states_out,
                                        int batch, int max_iters, float tol, int32_t* steps_out, void* workspace,
                                        size_t workspace_bytes, void* stream) {
-  if (int r = check_settle(cfg, batch, max_iters)) return r;
-  if (int r = check_settle_run(tol, steps_out)) return r;
-  const SettleRun run{tol, steps_out};
-  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, states_out, batch, max_iters, 1, workspace,
-                      workspace_bytes, stream, -1, &run);
+  return settle_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, states_out, batch, max_iters, 1, tol, steps_out,
+                     workspace, workspace_bytes, stream);
 }
 
 // glom_b200_forward_steps: a forward of max_steps steps in which image b stops after steps[b] (read on the device only)
-static int check_forward_steps(const glom_b200_cfg* cfg, int batch, int max_steps) {
-  if (int r = check_cfg(cfg)) return r;
-  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "forward_steps: bf16 engine only (precision fp32 given)");
-  if (batch < 1) return fail(GLOM_B200_ERR_INVALID, "forward_steps: batch must be >= 1 (got %d)", batch);
-  if (max_steps < 0) return fail(GLOM_B200_ERR_INVALID, "forward_steps: max_steps must be >= 0 (got %d)", max_steps);
-  return 0;
-}
-
 GLOM_B200_API int glom_b200_forward_steps_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_steps, int return_all,
                                                           size_t* out_bytes) {
-  if (int r = check_forward_steps(cfg, batch, max_steps)) return r;
-  if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
-  *out_bytes = settle_layout(make_geometry(cfg, batch), max_steps, return_all ? 1 : 0).total;
-  return 0;
+  return freeze_workspace_bytes(kForwardSteps, cfg, batch, max_steps, return_all, out_bytes);
 }
 
 GLOM_B200_API int glom_b200_forward_steps(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
                                           const float* pos, const float* state_in, const float* init_levels, float* state_out,
                                           int batch, const int32_t* steps, int max_steps, int return_all, void* workspace,
                                           size_t workspace_bytes, void* stream) {
-  if (int r = check_forward_steps(cfg, batch, max_steps)) return r;
-  if (!steps) return fail(GLOM_B200_ERR_INVALID, "forward_steps: steps is NULL");
-  if (reinterpret_cast<uintptr_t>(steps) % 4) return fail(GLOM_B200_ERR_INVALID, "forward_steps: steps must be 4-byte aligned");
+  if (int r = check_freeze(kForwardSteps, cfg, batch, max_steps)) return r;
+  if (int r = check_steps_ptr("forward_steps", "steps", steps)) return r;
   return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_steps, return_all ? 1 : 0,
                       workspace, workspace_bytes, stream, -1, nullptr, steps);
 }
@@ -433,20 +432,18 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
         if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle convergence launch after step %d: %s", t, cudaGetErrorString(e));
       }
     }
-    // settle: image b's result S_steps[b] is in loc(steps[b]); the ones in the workspace slab move to state_out
-    if (settle && !return_all) {
-      e = launch_settle_gather(g, iters, settle->steps, wslab, state_out, nullptr, 0, st, &g_launches);
-      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle gather launch: %s", cudaGetErrorString(e));
-    }
-    // forward_steps and settle_all: return_all slab t of image b must be S_min(t, steps[b]); without return_all the result
-    // of an image with steps[b] == 0 (forward_steps only) is S_0, which step 0 read straight from state_in / init_levels
-    if ((steps || settle) && return_all) {
-      e = launch_steps_fill(g, iters, steps ? steps : settle->steps, state_out, st, &g_launches);
+    // settle and forward_steps: return_all slab t of image b must be S_min(t, steps[b]).  Otherwise S_steps[b] is in
+    // loc(steps[b]) and the ones in the workspace slab move to state_out; steps[b] == 0 (forward_steps only) takes S_0,
+    // which step 0 read straight from state_in / init_levels
+    const int32_t* image_steps = settle ? settle->steps : steps;
+    if (image_steps && return_all) {
+      e = launch_steps_fill(g, iters, image_steps, state_out, st, &g_launches);
       if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "return_all fill launch: %s", cudaGetErrorString(e));
-    } else if (steps && iters > 0) {
-      e = launch_settle_gather(g, iters, steps, wslab, state_out, s0_direct ? (state_in ? state_in : init_levels) : nullptr,
-                               state_in ? 0 : 1, st, &g_launches);
-      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "step gather launch: %s", cudaGetErrorString(e));
+    } else if (image_steps && iters > 0) {
+      e = launch_settle_gather(g, iters, image_steps, wslab, state_out, state_in ? state_in : init_levels, state_in ? 0 : 1,
+                               st, &g_launches);
+      if (e != cudaSuccess)
+        return fail(GLOM_B200_ERR_CUDA, "%s gather launch: %s", settle ? "settle" : "step", cudaGetErrorString(e));
     }
   } else {
     cudaError_t e = launch_broadcast_init(g, state_in, init_levels, loc(0), st, &g_launches, &g_prof);
@@ -597,8 +594,7 @@ GLOM_B200_API int glom_b200_backward_steps(const glom_b200_cfg* cfg, const glom_
                                            const float* pos, const float* states, const float* grad_out,
                                            const glom_b200_grads* gr, int batch, const int32_t* steps, int max_steps,
                                            int grad_all, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!steps) return fail(GLOM_B200_ERR_INVALID, "backward_steps: steps is NULL");
-  if (reinterpret_cast<uintptr_t>(steps) % 4) return fail(GLOM_B200_ERR_INVALID, "backward_steps: steps must be 4-byte aligned");
+  if (int r = check_steps_ptr("backward_steps", "steps", steps)) return r;
   if (max_steps < 0) return fail(GLOM_B200_ERR_INVALID, "backward_steps: max_steps must be >= 0 (got %d)", max_steps);
   return backward_impl(cfg, w, tokens, pos, states, grad_out, gr, batch, max_steps, steps, grad_all, workspace,
                        workspace_bytes, stream);

@@ -46,6 +46,12 @@ def _aligned_bytes(nbytes, device, align=1024):
     return raw[off:off + nbytes]
 
 
+def _require_cuda(img):
+    if not img.is_cuda:
+        raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
+                           "move the module and inputs to an H100")
+
+
 class _Patchify(nn.Module):
     """Parameter-free placeholder at index 0 so the Linear keeps the key ``image_to_tokens.1.*``
     (the reference has an einops Rearrange there, glom_pytorch.py:95)."""
@@ -134,83 +140,56 @@ class ConsensusAttention(nn.Module):
 
 
 class _ColumnUpdate(torch.autograd.Function):
-    """The loop glom_pytorch.py:131-145 as one differentiable op: forward = glom_b200_forward (all states kept),
+    """The loop glom_pytorch.py:131-145 as one differentiable op: forward = the engine call with all states kept,
     backward = glom_b200_backward (recompute per step; tensor-core GEMMs for the bf16 engine).  With `steps` (the
-    engine's (B,) int32 copy of a per-image step vector, iters = its maximum): forward_steps / backward_steps."""
+    engine's (B,) int32 copy of a per-image step vector, iters = its maximum): forward_steps / backward_steps.  With
+    `tol` (Glom.settle(differentiable=True), iters = max_iters): settle_all / backward_steps with the settle's own step
+    counts, which are constants of the backward exactly as in forward(iters=steps); the outputs are then
+    (levels, steps), and steps is not differentiable."""
 
     @staticmethod
-    def forward(ctx, module, iters, steps, return_all, tokens, pos, state0, init_levels, *weights):
+    def forward(ctx, module, iters, steps, tol, return_all, tokens, pos, state0, init_levels, *weights):
         tokens, pos = tokens.contiguous(), pos.contiguous()
-        if steps is None:
-            states = module._run_engine(tokens, pos, state0, init_levels, iters, True)      # (T+1, B, n, L, d)
-        else:
-            states = module._run_engine_steps(tokens, pos, state0, init_levels, steps, iters, True)
-        ctx.module, ctx.iters, ctx.return_all, ctx.steps = module, iters, return_all, steps
+        states = module._run(tokens, pos, state0, init_levels, iters, True, steps=steps, tol=tol)   # (T+1, B, n, L, d)
+        if tol is not None:
+            states, steps = states
+            ctx.mark_non_differentiable(steps)
+        ctx.module, ctx.iters, ctx.return_all = module, iters, return_all
+        # settle: the backward reads its own copy, so an in-place edit of the returned steps changes no gradient
+        ctx.steps = steps if tol is None else steps.clone()
         ctx.had_state0 = state0 is not None
         ctx.want_state0 = state0 is not None and state0.requires_grad
         ctx.save_for_backward(tokens, pos, states, *weights)
-        return states if return_all else states[iters]
+        out = states if return_all else states[iters]
+        return out if tol is None else (out, steps)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, grad_out):
-        return (None, None, None, None, *_loop_backward(ctx, grad_out))
-
-
-def _loop_backward(ctx, grad_out):
-    """Backward of the loop for _ColumnUpdate and _Settle: ctx holds module, iters, return_all, steps (None or the
-    engine's private int32 copy), had_state0 / want_state0 and the saved (tokens, pos, states, *weights).  Returns the
-    gradients of (tokens, pos, state0, init_levels, *weights)."""
-    module, iters = ctx.module, ctx.iters
-    tokens, pos, states, *weights = ctx.saved_tensors
-    device = states.device
-    b, n = tokens.shape[0], tokens.shape[1]
-    grad_out = grad_out.to(torch.float32).contiguous()
-    wts = [w.detach().to(torch.float32).contiguous() for w in weights]
-    zeros = torch.zeros
-    g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos),
-         "d_state0": zeros(states.shape[1:], dtype=torch.float32, device=device) if ctx.had_state0 else None,
-         "d_init": None if ctx.had_state0 else zeros(module.levels, module.dim, dtype=torch.float32, device=device)}
-    names = ("d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")
-    for k, w in zip(names, wts):
-        g[k] = zeros_like32(w)
-    with torch.cuda.device(device):
-        cfg = module.engine_cfg(n)           # bf16 engine: MLP GEMMs of the backward on tensor cores
-        ws_bytes = _native.backward_workspace_bytes(cfg, b)
-        ws = module._get_workspace(ws_bytes, device, "_bwd_workspace")      # cached across steps
-        ptrs = {k: (None if v is None else v.data_ptr()) for k, v in g.items()}
-        stream = torch.cuda.current_stream(device).cuda_stream
-        if ctx.steps is None:
+    def backward(ctx, grad_out, *_grad_steps):
+        module, iters = ctx.module, ctx.iters
+        tokens, pos, states, *weights = ctx.saved_tensors
+        device = states.device
+        b, n = tokens.shape[0], tokens.shape[1]
+        grad_out = grad_out.to(torch.float32).contiguous()
+        wts = [w.detach().to(torch.float32).contiguous() for w in weights]
+        zeros = torch.zeros
+        g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos),
+             "d_state0": zeros(states.shape[1:], dtype=torch.float32, device=device) if ctx.had_state0 else None,
+             "d_init": None if ctx.had_state0 else zeros(module.levels, module.dim, dtype=torch.float32, device=device)}
+        names = ("d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")
+        for k, w in zip(names, wts):
+            g[k] = zeros_like32(w)
+        with torch.cuda.device(device):
+            cfg = module.engine_cfg(n)           # bf16 engine: MLP GEMMs of the backward on tensor cores
+            ws_bytes = _native.backward_workspace_bytes(cfg, b)
+            ws = module._get_workspace(ws_bytes, device, "_bwd_workspace")      # cached across steps
+            ptrs = {k: (None if v is None else v.data_ptr()) for k, v in g.items()}
             _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
-                             grad_out.data_ptr(), ptrs, b, iters, ctx.return_all, ws.data_ptr(), ws.numel(), stream)
-        else:
-            _native.backward_steps(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(),
-                                   states.data_ptr(), grad_out.data_ptr(), ptrs, b, ctx.steps.data_ptr(), iters,
-                                   ctx.return_all, ws.data_ptr(), ws.numel(), stream)
-    return (g["d_tokens"], g["d_pos"], g["d_state0"] if ctx.want_state0 else None, g["d_init"], *[g[k] for k in names])
-
-
-class _Settle(torch.autograd.Function):
-    """Glom.settle(differentiable=True): forward = glom_b200_settle_all (every state kept, each image stopped on the
-    GPU), backward = glom_b200_backward_steps with max_steps = max_iters and the settle's own step counts, which are
-    constants of the backward exactly as in forward(iters=steps).  Outputs (levels, steps); steps is not differentiable."""
-
-    @staticmethod
-    def forward(ctx, module, max_iters, tol, return_all, tokens, pos, state0, init_levels, *weights):
-        tokens, pos = tokens.contiguous(), pos.contiguous()
-        states, steps = module._run_settle(tokens, pos, state0, init_levels, max_iters, tol, True)
-        # the backward reads its own copy: an in-place edit of the returned steps changes no gradient
-        ctx.module, ctx.iters, ctx.return_all, ctx.steps = module, max_iters, return_all, steps.clone()
-        ctx.had_state0 = state0 is not None
-        ctx.want_state0 = state0 is not None and state0.requires_grad
-        ctx.save_for_backward(tokens, pos, states, *weights)
-        ctx.mark_non_differentiable(steps)
-        return (states if return_all else states[max_iters]), steps
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, grad_out, _grad_steps):
-        return (None, None, None, None, *_loop_backward(ctx, grad_out))
+                             grad_out.data_ptr(), ptrs, b, iters, ctx.return_all, ws.data_ptr(), ws.numel(),
+                             torch.cuda.current_stream(device).cuda_stream,
+                             None if ctx.steps is None else ctx.steps.data_ptr())
+        return (None, None, None, None, None, g["d_tokens"], g["d_pos"], g["d_state0"] if ctx.want_state0 else None,
+                g["d_init"], *[g[k] for k in names])
 
 
 def zeros_like32(t):
@@ -275,24 +254,26 @@ class Glom(nn.Module):
         self.top_down = GroupedFeedForward(dim=dim, groups=levels - 1)
         self.attention = ConsensusAttention(num_patches_side, attend_self=consensus_self,
                                             local_consensus_radius=local_consensus_radius)
-        self._packed = None          # (key, tensor)
-        self._scratch = {}           # (slot, device index, stream) -> buffer, grown on demand, reused across calls
-        self._resume = None          # cross-call persistence: what the workspace still holds about the last returned state
-        self._staged = None          # tokens of the next frame computed ahead on a side stream (stage_tokens)
+        self.__dict__.update(self._empty_scratch())
         self.use_native_tokenizer = True
         self.last_launches = 0
 
     # ------------------------------------------------------------------ cache hygiene
-    _SCRATCH_ATTRS = ("_packed", "_scratch", "_tok_launches", "_resume", "_staged")
+    @staticmethod
+    def _empty_scratch():
+        """The device-side caches, empty.  .to() / .cuda() / .float() (parameters are replaced), pickling and deepcopy
+        reset them to this."""
+        return {"_packed": None,    # (key, tensor)
+                "_scratch": {},     # (slot, device index, stream) -> buffer, grown on demand, reused across calls
+                "_resume": None,    # cross-call persistence: what the workspace still holds about the last returned state
+                "_staged": None}    # tokens of the next frame computed ahead on a side stream (stage_tokens)
 
     def invalidate_packed(self):
         """Drop the cached packed copy of the MLP weights (needed after in-place ``param.data`` edits in eval mode)."""
         self._packed = None
 
-    def _apply(self, fn, *args, **kwargs):                 # .to() / .cuda() / .float() ...: parameters are replaced
-        self._packed = None
-        self._scratch = {}
-        self._resume = self._staged = None
+    def _apply(self, fn, *args, **kwargs):
+        self.__dict__.update(self._empty_scratch())
         return super()._apply(fn, *args, **kwargs)
 
     def _load_from_state_dict(self, *args, **kwargs):      # load_state_dict copies in place: versions bump, but be explicit
@@ -301,8 +282,7 @@ class Glom(nn.Module):
 
     def __getstate__(self):                                # torch.save(model) / pickle: no scratch buffers
         st = dict(super().__getstate__() if hasattr(super(), "__getstate__") else self.__dict__)
-        st["_packed"], st["_scratch"] = None, {}
-        st["_resume"] = st["_staged"] = None
+        st.update(self._empty_scratch())
         return st
 
     def __deepcopy__(self, memo):
@@ -310,15 +290,9 @@ class Glom(nn.Module):
         cls = self.__class__
         new = cls.__new__(cls)
         memo[id(self)] = new
+        empty = self._empty_scratch()
         for k, v in self.__dict__.items():
-            if k == "_packed":
-                new.__dict__[k] = None
-            elif k == "_scratch":
-                new.__dict__[k] = {}
-            elif k in ("_resume", "_staged"):
-                new.__dict__[k] = None
-            else:
-                new.__dict__[k] = copy.deepcopy(v, memo)
+            new.__dict__[k] = empty[k] if k in empty else copy.deepcopy(v, memo)
         return new
 
     @property
@@ -376,15 +350,14 @@ class Glom(nn.Module):
     def tokens(self, img):
         """image_to_tokens (:114): fp32 CUDA-core kernel (precision fp32) or bf16 gather + wgmma GEMM (bf16)."""
         lin = self.image_to_tokens[1]
-        b, c, h, w = img.shape
+        _, _, h, w = img.shape
+        b, n = self._check_input(img, loop=False)
         p = self.patch_size
-        if c != 3 or h % p or w % p:
-            raise RuntimeError(f"image {tuple(img.shape)} is not (B, 3, H, W) with H, W multiples of {p}")
         if not self.use_native_tokenizer:
             return lin(self.image_to_tokens[0](img.float())).contiguous()
         img = img.float().contiguous()
         with torch.cuda.device(img.device):      # the library launches on the CURRENT device
-            out = torch.empty(b, (h // p) * (w // p), self.dim, dtype=torch.float32, device=img.device)
+            out = torch.empty(b, n, self.dim, dtype=torch.float32, device=img.device)
             wt, bs = lin.weight.detach().float().contiguous(), lin.bias.detach().float().contiguous()
             tws_bytes = _native.tokenize_workspace_bytes(b, h, w, p, self.dim, self.precision)
             tws = self._get_workspace(tws_bytes, img.device, "_tok_ws") if tws_bytes else None
@@ -429,20 +402,25 @@ class Glom(nn.Module):
         st["tokens"].record_stream(cur)
         return st["tokens"]
 
-    # ------------------------------------------------------------------ engine call (no autograd)
-    def _run_engine(self, tokens, pos, state_in, init, iters, return_all, allow_resume=False):
-        """tokens (B,n,d), pos (n,d), state_in (B,n,L,d) or None, init (L,d): fp32 contiguous CUDA tensors.
-        allow_resume (eval, no autograd): when `state_in` IS the tensor the previous call returned, unmodified, and the
-        workspace is the same, the engine still holds that state's bf16 shadows / norm partials: the state prologue is
-        skipped (glom_b200_forward_resume)."""
+    # ------------------------------------------------------------------ engine call
+    def _run(self, tokens, pos, state_in, init, iters, return_all, *, steps=None, tol=None, allow_resume=False):
+        """One engine call.  tokens (B,n,d), pos (n,d), state_in (B,n,L,d) or None, init (L,d): CUDA tensors.
+        * Plain (glom_b200_forward): `iters` steps.  allow_resume (eval, no autograd): when `state_in` IS the tensor the
+          previous call returned, unmodified, and the workspace is the same, the engine still holds that state's bf16
+          shadows / norm partials: the state prologue is skipped (glom_b200_forward_resume).
+        * `steps` (glom_b200_forward_steps): image b runs steps[b] steps (steps: the engine's (B,) int32 CUDA tensor,
+          iters its maximum).
+        * `tol` (glom_b200_settle / _settle_all): up to `iters` steps, each image stopped on the GPU -> (out, steps).
+        After a per-image run the shadows of stopped images are stale: the next forward takes the ordinary prologue."""
         device = tokens.device
         b, n = tokens.shape[0], tokens.shape[1]
         resume, self._resume = self._resume, None
+        plain = steps is None and tol is None
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
             pos_key = (self.pos_emb.weight.data_ptr(), self.pos_emb.weight._version)
             call_key = (device.index, stream, b, n, self.precision, pos_key)
-            use_resume = (allow_resume and resume is not None and state_in is not None and iters >= 1
+            use_resume = (plain and allow_resume and resume is not None and state_in is not None and iters >= 1
                           and self.precision == "bf16" and resume["ref"]() is state_in
                           and state_in._version == resume["version"] and resume["key"] == call_key)
             tokens = tokens.detach().to(torch.float32).contiguous()
@@ -450,50 +428,40 @@ class Glom(nn.Module):
             init = init.detach().to(torch.float32).contiguous()
             if state_in is not None:
                 state_in = state_in.detach().to(device=device, dtype=torch.float32).contiguous()
+            state_ptr = None if state_in is None else state_in.data_ptr()
             cfg = self.engine_cfg(n)
             packed = self._packed_weights(cfg, device, stream)
             shape = (b, n, self.levels, self.dim)
             out = torch.empty(((iters + 1,) + shape) if return_all else shape, dtype=torch.float32, device=device)
-            ws_bytes = _native.workspace_bytes(cfg, b, iters, return_all)
+            if tol is not None:
+                steps = torch.empty(b, dtype=torch.int32, device=device)
+            if plain:
+                ws_bytes = _native.workspace_bytes(cfg, b, iters, return_all)
+            elif tol is None:
+                ws_bytes = _native.forward_steps_workspace_bytes(cfg, b, iters, return_all)
+            else:
+                ws_bytes = (_native.settle_all_workspace_bytes if return_all else _native.settle_workspace_bytes)(cfg, b, iters)
             ws = self._get_workspace(ws_bytes, device)
-            parity = iters & 1
-            if use_resume and ws.data_ptr() == resume["ws"]:
-                parity = _native.forward_resume(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_in.data_ptr(),
+            if tol is not None:
+                _native.settle(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
+                               out.data_ptr(), b, iters, return_all, tol, steps.data_ptr(), ws.data_ptr(), ws.numel(), stream)
+            elif steps is not None:
+                _native.forward_steps(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
+                                      out.data_ptr(), b, steps.data_ptr(), iters, return_all, ws.data_ptr(), ws.numel(),
+                                      stream)
+            elif use_resume and ws.data_ptr() == resume["ws"]:
+                parity = _native.forward_resume(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr,
                                                 out.data_ptr(), b, iters, return_all, ws.data_ptr(), ws.numel(), stream,
                                                 resume["parity"])
             else:
-                _native.forward(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(),
-                                None if state_in is None else state_in.data_ptr(), init.data_ptr(),
+                parity = iters & 1
+                _native.forward(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
                                 out.data_ptr(), b, iters, return_all, ws.data_ptr(), ws.numel(), stream)
             self.last_launches = _native.last_launch_count() + getattr(self, "_tok_launches", 0)
-            if allow_resume and not return_all and iters >= 1 and self.precision == "bf16":
+            if plain and allow_resume and not return_all and iters >= 1 and self.precision == "bf16":
                 self._resume = {"ref": weakref.ref(out), "version": out._version, "key": call_key, "ws": ws.data_ptr(),
                                 "parity": parity}
-        return out
-
-    def _run_engine_steps(self, tokens, pos, state_in, init, steps, max_steps, return_all):
-        """glom_b200_forward_steps: image b runs steps[b] steps (steps: the engine's (B,) int32 CUDA tensor, max_steps its
-        maximum).  The shadows of stopped images are stale afterwards: the next forward takes the ordinary prologue."""
-        device = tokens.device
-        b, n = tokens.shape[0], tokens.shape[1]
-        self._resume = None
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            tokens = tokens.detach().to(torch.float32).contiguous()
-            pos = pos.detach().to(torch.float32).contiguous()
-            init = init.detach().to(torch.float32).contiguous()
-            if state_in is not None:
-                state_in = state_in.detach().to(device=device, dtype=torch.float32).contiguous()
-            cfg = self.engine_cfg(n)
-            packed = self._packed_weights(cfg, device, stream)
-            shape = (b, n, self.levels, self.dim)
-            out = torch.empty(((max_steps + 1,) + shape) if return_all else shape, dtype=torch.float32, device=device)
-            ws = self._get_workspace(_native.forward_steps_workspace_bytes(cfg, b, max_steps, return_all), device)
-            _native.forward_steps(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(),
-                                  None if state_in is None else state_in.data_ptr(), init.data_ptr(), out.data_ptr(), b,
-                                  steps.data_ptr(), max_steps, return_all, ws.data_ptr(), ws.numel(), stream)
-            self.last_launches = _native.last_launch_count() + getattr(self, "_tok_launches", 0)
-        return out
+        return out if tol is None else (out, steps)
 
     def _parse_iters(self, iters, b):
         """-> (iters, steps): a scalar step count and None, or, for a per-image vector whose entries differ, its maximum
@@ -530,50 +498,53 @@ class Glom(nn.Module):
         steps.  min / max of the vector are read once on the host (one device-to-host read for a CUDA tensor); a
         vector whose entries are all equal takes the scalar path.  Per-image counts need precision='bf16' and clear
         the resume state."""
-        b = img.shape[0]
-        iters, steps = self._parse_iters(iters, b)
+        iters, steps = self._parse_iters(iters, img.shape[0])
         if steps is not None and self.precision != "bf16":
             raise RuntimeError("per-image iters need precision='bf16' (the fp32 engine has no per-image freezing)")
-        if not img.is_cuda:
-            raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
-                               "move the module and inputs to an H100")
+        _require_cuda(img)
         if steps is not None:    # the engine's own int32 copy: later in-place edits of the caller's tensor change nothing
             steps = steps.to(device=img.device, dtype=torch.int32, copy=True)
-        needs_grad = self._needs_grad(img, levels)
-        p = self.patch_size
-        if img.dim() != 4 or img.shape[1] != 3 or img.shape[2] % p or img.shape[3] % p:
-            raise RuntimeError(f"image {tuple(img.shape)} is not (B, 3, H, W) with H, W multiples of {p}")
-        n = (img.shape[2] // p) * (img.shape[3] // p)
-        if n > self.pos_emb.num_embeddings:
-            raise IndexError(f"{n} patches exceed pos_emb size {self.pos_emb.num_embeddings}")   # (:117)
-        if levels is not None and tuple(levels.shape) != (b, n, self.levels, self.dim):          # (:123)
-            raise RuntimeError(f"levels must have shape {(b, n, self.levels, self.dim)}, got {tuple(levels.shape)}")
-        if not needs_grad:
-            tokens = self._take_staged(img)
-            if tokens is None:
-                tokens = self.tokens(img)                                    # (:114) engine tokeniser
-            if steps is not None:
-                return self._run_engine_steps(tokens, self.pos_emb.weight[:n], levels, self.init_levels, steps, iters,
-                                              return_all)
-            return self._run_engine(tokens, self.pos_emb.weight[:n], levels, self.init_levels, iters, return_all,
-                                    allow_resume=not self.training)
-        # training: the tokeniser and the loop are the engine's differentiable ops (the same kernels as without autograd);
-        # only the parameter views (pos_emb slice) are plain torch ops
-        tokens = self._differentiable_tokens(img)                                               # (:114)
-        pos = self.pos_emb.weight[:n]                                                            # (:117)
-        state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
-        return _ColumnUpdate.apply(self, iters, steps, return_all, tokens, pos, state0, self.init_levels, *self._mlp_params())
-
-    def _differentiable_tokens(self, img):
-        lin = self.image_to_tokens[1]
-        if self.use_native_tokenizer:
-            return _Tokenize.apply(self, img, lin.weight, lin.bias)
-        self._tok_launches = 0
-        return lin(self.image_to_tokens[0](img.float()))
+        return self._column_update(img, levels, self._needs_grad(img, levels), iters, return_all, steps=steps)
 
     def _needs_grad(self, img, levels):
         return torch.is_grad_enabled() and (img.requires_grad or (levels is not None and levels.requires_grad)
                                             or any(p.requires_grad for p in self.parameters()))
+
+    def _check_input(self, img, levels=None, loop=True):
+        """-> (b, n) of a (B, 3, H, W) image with H, W multiples of the patch size.  For the column update (`loop`) the
+        n patches must fit pos_emb, and `levels`, if given, must have shape (b, n, L, d)."""
+        p = self.patch_size
+        if img.dim() != 4 or img.shape[1] != 3 or img.shape[2] % p or img.shape[3] % p:
+            raise RuntimeError(f"image {tuple(img.shape)} is not (B, 3, H, W) with H, W multiples of {p}")
+        b, n = img.shape[0], (img.shape[2] // p) * (img.shape[3] // p)
+        if loop and n > self.pos_emb.num_embeddings:
+            raise IndexError(f"{n} patches exceed pos_emb size {self.pos_emb.num_embeddings}")   # (:117)
+        if levels is not None and tuple(levels.shape) != (b, n, self.levels, self.dim):          # (:123)
+            raise RuntimeError(f"levels must have shape {(b, n, self.levels, self.dim)}, got {tuple(levels.shape)}")
+        return b, n
+
+    def _column_update(self, img, levels, needs_grad, iters, return_all, *, steps=None, tol=None):
+        """forward and settle after their own argument checks: check the image and `levels`, take the tokens, and run the
+        engine (`_run`'s arguments), through the autograd Function _ColumnUpdate when gradients are needed."""
+        _, n = self._check_input(img, levels)
+        if not needs_grad:
+            tokens = self._take_staged(img)
+            if tokens is None:
+                tokens = self.tokens(img)                                    # (:114) engine tokeniser
+            return self._run(tokens, self.pos_emb.weight[:n], levels, self.init_levels, iters, return_all, steps=steps,
+                             tol=tol, allow_resume=not self.training)
+        # training: the tokeniser and the loop are the engine's differentiable ops (the same kernels as without autograd);
+        # only the parameter views (pos_emb slice) are plain torch ops
+        lin = self.image_to_tokens[1]
+        if self.use_native_tokenizer:
+            tokens = _Tokenize.apply(self, img, lin.weight, lin.bias)                           # (:114)
+        else:
+            self._tok_launches = 0
+            tokens = lin(self.image_to_tokens[0](img.float()))
+        pos = self.pos_emb.weight[:n]                                                            # (:117)
+        state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
+        return _ColumnUpdate.apply(self, iters, steps, tol, return_all, tokens, pos, state0, self.init_levels,
+                                   *self._mlp_params())
 
     # ------------------------------------------------------------------ inference until the columns settle
     def settle(self, img, tol, max_iters=None, levels=None, *, return_all=False, differentiable=False):
@@ -598,9 +569,7 @@ class Glom(nn.Module):
         max_iters 12.  Without autograd ``differentiable`` changes nothing."""
         if self.precision != "bf16":
             raise RuntimeError("Glom.settle needs precision='bf16' (the fp32 engine has no early stopping)")
-        if not img.is_cuda:
-            raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
-                               "move the module and inputs to an H100")
+        _require_cuda(img)
         needs_grad = self._needs_grad(img, levels)
         if needs_grad and not differentiable:
             raise RuntimeError("Glom.settle is inference only: call it under torch.no_grad() / torch.inference_mode() "
@@ -611,47 +580,4 @@ class Glom(nn.Module):
         tol = float(tol)
         if tol != tol:
             raise ValueError("tol is NaN")
-        b, p = img.shape[0], self.patch_size
-        if img.dim() != 4 or img.shape[1] != 3 or img.shape[2] % p or img.shape[3] % p:
-            raise RuntimeError(f"image {tuple(img.shape)} is not (B, 3, H, W) with H, W multiples of {p}")
-        n = (img.shape[2] // p) * (img.shape[3] // p)
-        if n > self.pos_emb.num_embeddings:
-            raise IndexError(f"{n} patches exceed pos_emb size {self.pos_emb.num_embeddings}")
-        if levels is not None and tuple(levels.shape) != (b, n, self.levels, self.dim):
-            raise RuntimeError(f"levels must have shape {(b, n, self.levels, self.dim)}, got {tuple(levels.shape)}")
-        if needs_grad:
-            tokens = self._differentiable_tokens(img)
-            pos = self.pos_emb.weight[:n]
-            state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
-            return _Settle.apply(self, max_iters, tol, return_all, tokens, pos, state0, self.init_levels,
-                                 *self._mlp_params())
-        tokens = self._take_staged(img)
-        if tokens is None:
-            tokens = self.tokens(img)
-        return self._run_settle(tokens, self.pos_emb.weight[:n], levels, self.init_levels, max_iters, tol, return_all)
-
-    def _run_settle(self, tokens, pos, state_in, init, max_iters, tol, return_all):
-        """glom_b200_settle (return_all: glom_b200_settle_all) -> (levels or all states, steps).  The workspace shadows
-        of stopped images are stale afterwards: the next forward takes the ordinary state prologue."""
-        device = tokens.device
-        b, n = tokens.shape[0], tokens.shape[1]
-        self._resume = None
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            tokens = tokens.detach().to(torch.float32).contiguous()
-            pos = pos.detach().to(torch.float32).contiguous()
-            init = init.detach().to(torch.float32).contiguous()
-            if state_in is not None:
-                state_in = state_in.detach().to(device=device, dtype=torch.float32).contiguous()
-            cfg = self.engine_cfg(n)
-            packed = self._packed_weights(cfg, device, stream)
-            shape = (b, n, self.levels, self.dim)
-            out = torch.empty(((max_iters + 1,) + shape) if return_all else shape, dtype=torch.float32, device=device)
-            steps = torch.empty(b, dtype=torch.int32, device=device)
-            run = _native.settle_all if return_all else _native.settle
-            ws_bytes = (_native.settle_all_workspace_bytes if return_all else _native.settle_workspace_bytes)(cfg, b, max_iters)
-            ws = self._get_workspace(ws_bytes, device)
-            run(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), None if state_in is None else state_in.data_ptr(),
-                init.data_ptr(), out.data_ptr(), b, max_iters, tol, steps.data_ptr(), ws.data_ptr(), ws.numel(), stream)
-            self.last_launches = _native.last_launch_count() + getattr(self, "_tok_launches", 0)
-        return out, steps
+        return self._column_update(img, levels, needs_grad, max_iters, return_all, tol=tol)

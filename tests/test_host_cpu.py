@@ -71,6 +71,29 @@ def test_state_dict_surface_matches_reference_layout():
     assert m.levels == 3
 
 
+@pytest.mark.parametrize("how", ["deepcopy", "pickle", "float"])
+def test_copies_and_conversions_drop_the_device_caches(how):
+    """deepcopy, a pickle round trip and .float() reset the packed weights, the scratch buffers, the resume state and the
+    staged tokens; the parameters and the other attributes survive."""
+    import copy
+    import pickle
+    torch.manual_seed(0)
+    m = G.Glom(dim=64, levels=3, image_size=28, patch_size=7)
+    want = {k: v.clone() for k, v in m.state_dict().items()}
+    m._packed = (("key",), torch.zeros(4))
+    m._scratch = {("_workspace", 0, 0): torch.zeros(8)}
+    m._resume = {"parity": 1}
+    m._staged = {"version": 0}
+    m._tok_launches = 2
+    new = {"deepcopy": lambda: copy.deepcopy(m), "pickle": lambda: pickle.loads(pickle.dumps(m)), "float": m.float}[how]()
+    assert new._packed is None and new._scratch == {} and new._resume is None and new._staged is None
+    assert new._tok_launches == 2
+    got = new.state_dict()
+    assert got.keys() == want.keys() and all(torch.equal(got[k], want[k]) for k in want)
+    if how != "float":
+        assert m._packed is not None and m._scratch and m._resume and m._staged     # the original keeps its caches
+
+
 def test_radius_mask_params_follow_the_buffer():
     from oracle.glom_oracle import radius_mask
     for side, r in [(4, 1.5), (4, 1), (8, 2), (8, 2.9), (6, 10)]:
