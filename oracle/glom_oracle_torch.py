@@ -5,7 +5,9 @@ outputs), written with batched torch CPU ops (``torch.bmm`` over the MLP groups,
 that it uses every host core the way the reference's own torch/oneDNN path does.  ``bench.py`` times it as the CPU
 arm (``kind: "port"``) ONLY when the unmodified reference package is not importable on the box
 (``$GLOM_REF_PATH`` -> ``baseline/_ref`` -> ``/root/reference``); ``tests/test_oracle_golden.py`` checks it against
-the same golden fixtures as the numpy oracle.  Only ``tests/`` and ``bench.py``'s CPU legs may import this module.
+the same golden fixtures as the numpy oracle.  ``column_step`` is the loop body as a differentiable float64-capable
+function; ``grads_at_states`` and ``step_backward_bf16`` are the backward references of ``tests/test_backward_oracle.py``.
+Only ``tests/`` and ``bench.py``'s CPU legs may import this module.
 
 Restates (``glom_pytorch/glom_pytorch.py``): GroupedFeedForward :23-36, ConsensusAttention.forward :56-73
 (F.normalize eps 1e-12 :58, d**-0.5 :60, diagonal -5e-4 :11/:62-65 before the radius mask :67-69), image_to_tokens
@@ -51,6 +53,195 @@ def radius_mask(side, radius):
     return torch.cdist(co, co) > radius
 
 
+def column_step(levels, tokens, pos, P, mask, attend_self):
+    """One step of the Jacobi loop (:132-144), differentiable.  levels (B, n, L, d), tokens (B, n, d), pos (n, d),
+    P: reference state_dict keys -> tensors, mask: (n, n) bool (True = masked) or None."""
+    L = levels.shape[2]
+    contrib = torch.full((L,), 4.0, dtype=levels.dtype)                                  # (:128)
+    contrib[-1] = 3.0                                                                     # (:129)
+    lwi = torch.cat((tokens[:, :, None, :], levels), dim=-2)                              # (:132)
+    bu = _grouped_ff(lwi[..., :-1, :], P["bottom_up.net.1.weight"], P["bottom_up.net.1.bias"],
+                     P["bottom_up.net.3.weight"], P["bottom_up.net.3.bias"])              # (:134)
+    td = _grouped_ff(lwi[..., 2:, :] + pos[None, :, None, :], P["top_down.net.1.weight"], P["top_down.net.1.bias"],
+                     P["top_down.net.3.weight"], P["top_down.net.3.bias"])                # (:136)
+    td = F.pad(td, (0, 0, 0, 1))                                                          # (:137)
+    cons = _consensus(levels, attend_self, mask)                                          # (:139)
+    return (levels + bu + td + cons) / contrib[None, None, :, None]                       # (:141-142)
+
+
+MLP_KEYS = ("bottom_up.net.1.weight", "bottom_up.net.1.bias", "bottom_up.net.3.weight", "bottom_up.net.3.bias",
+            "top_down.net.1.weight", "top_down.net.1.bias", "top_down.net.3.weight", "top_down.net.3.bias")
+
+
+def _f64(x):
+    return torch.as_tensor(x).detach().to(device="cpu", dtype=torch.float64)
+
+
+def grads_at_states(P, tokens, pos, states, cot, *, return_all, steps=None, attend_self=False, mask=None):
+    """The backward of T column steps as a chain of one-step VJPs in float64, each taken at the GIVEN states.
+
+    states: (>= T+1, B, n, L, d) with S_0..S_T (e.g. the engine's own return_all slabs; S_T is not read); T = the
+    number of steps = cot.shape[0] - 1 with `return_all` (cot: one cotangent per slab), else states.shape[0] - 1 (cot:
+    the cotangent of S_T).  steps (B,) ints or None: image b is the identity at step t when steps[b] <= t (its cotangent
+    passes through and it adds nothing to any other gradient).  This is what the engine's backward computes: its fp32
+    (or tensor-core) backward evaluated at its forward's states, so the forward's own rounding drops out.
+    Returns float64 CPU tensors: d_state0 (dL/dS_0), d_tokens, d_pos (n, d) and one entry per MLP_KEYS name."""
+    P = {k: _f64(P[k]).requires_grad_(True) for k in MLP_KEYS}
+    tokens = _f64(tokens).requires_grad_(True)
+    pos = _f64(pos).requires_grad_(True)
+    states = _f64(states)
+    cot = _f64(cot)
+    T = cot.shape[0] - 1 if return_all else states.shape[0] - 1
+    if mask is not None:
+        mask = torch.as_tensor(mask, dtype=torch.bool, device="cpu")
+    live_all = None if steps is None else torch.as_tensor(steps).to("cpu", torch.int64)
+    acc = {k: torch.zeros_like(v) for k, v in P.items()}
+    acc["d_tokens"] = torch.zeros_like(tokens)
+    acc["d_pos"] = torch.zeros_like(pos)
+    g = cot[T] if return_all else cot
+    for t in range(T - 1, -1, -1):
+        s = states[t].clone().requires_grad_(True)
+        gv = g
+        if live_all is not None:
+            live = (live_all > t).to(torch.float64)[:, None, None, None]
+            gv = g * live
+        out = column_step(s, tokens, pos, P, mask, attend_self)
+        leaves = [s, tokens, pos] + [P[k] for k in MLP_KEYS]
+        gr = torch.autograd.grad(out, leaves, gv, allow_unused=True)
+        for k, v in zip(["d_tokens", "d_pos"] + list(MLP_KEYS), gr[1:]):
+            if v is not None:
+                acc[k] += v
+        g = gr[0] + (g - gv)                                  # frozen images: the identity
+        if return_all:
+            g = g + cot[t]
+    acc["d_state0"] = g
+    return acc
+
+
+def patchify(img, p):
+    """'b c (h p1) (w p2) -> b (h w) (p1 p2 c)' (:95)."""
+    B, C, H, W = img.shape
+    return img.reshape(B, C, H // p, p, W // p, p).permute(0, 2, 4, 3, 5, 1).reshape(B, (H // p) * (W // p), p * p * C)
+
+
+def token_grads(img, weight, bias, patch_size, d_tokens):
+    """image_to_tokens (:94-97) backward in float64: d_tokens (B, n, d) -> d_img, d_weight, d_bias."""
+    img = _f64(img).requires_grad_(True)
+    w = _f64(weight).requires_grad_(True)
+    b = _f64(bias).requires_grad_(True)
+    tok = F.linear(patchify(img, patch_size), w, b)
+    gi, gw, gb = torch.autograd.grad(tok, (img, w, b), _f64(d_tokens))
+    return {"d_img": gi, "image_to_tokens.1.weight": gw, "image_to_tokens.1.bias": gb}
+
+
+def bf16(x):
+    """Round to the nearest bfloat16 (ties to even), back in the input's dtype."""
+    return x.to(torch.float32).to(torch.bfloat16).to(x.dtype)
+
+
+def _gelu_and_grad(x):
+    cdf = 0.5 * (1.0 + torch.erf(x * (0.5 ** 0.5)))
+    pdf = torch.exp(-0.5 * x * x) * (2.0 * math.pi) ** -0.5
+    return x * cdf, cdf + x * pdf
+
+
+def step_backward_bf16(P, tokens, pos, s, g, *, attend_self=False, mask=None, attn_tc=True):
+    """One reverse step of the bf16 engine's tensor-core backward, float64 except for bf16 rounding at exactly the
+    points where the engine rounds.  s = S_t (B, n, L, d), g = dL/dS_{t+1} (plus that slab's own cotangent).
+    Returns d_state (dL/dS_t), d_tokens, d_pos and the MLP_KEYS gradients of this step.
+
+    Roundings (bwd_kernels.cu / tc_bwd_kernels.cu):
+      bf16 shadows: xb = bf16(tokens), sb = bf16(S_t), sp = bf16(S_t[:, :, 1:] + pos), gsb = bf16(g / c)
+      (cast_bf16_rows, bwd_shadows_kernel); weights w1p = w1t = bf16(W1), w2t = bf16(W2); b1 stays fp32.
+      BW_PRE: pre = xb W1^T + b1 -> h = bf16(gelu(pre)), gp = bf16(gelu'(pre)).
+      BW_DH: dpre = (gsb W2) * gp -> bf16(dpre); the b1 gradient sums the UNROUNDED dpre, the b2 gradient sums g / c.
+      BW_DX: dx = bf16(dpre) W1.  BW_DW: dW2 += gsb^T h, dW1 += bf16(dpre)^T xb.
+    With attn_tc (n % 8 == 0) the consensus backward runs on tensor cores too:
+      khat_b = bf16(khat) (normalize_rows_kernel); logits = sb khat_b^T; a_b = bf16(A) (attn_softmax_kernel);
+      dA = gsb sb^T; dsim_b = bf16(scale * dsim) (attn_softmax_bwd_kernel); ds += a_b^T gsb + dsim_b khat_b;
+      dkhat = dsim_b^T sb; the normalisation backward is fp32 on khat, rnorm.
+    Without attn_tc (the mixed path) the consensus backward is fp32 on S_t and g / c: exact here."""
+    P = {k: _f64(P[k]) for k in MLP_KEYS}
+    tokens, pos, s, g = _f64(tokens), _f64(pos), _f64(s), _f64(g)
+    B, n, L, d = s.shape
+    contrib = torch.full((L,), 4.0, dtype=torch.float64)
+    contrib[-1] = 3.0
+    gs = g / contrib[None, None, :, None]
+    gsb = bf16(gs)
+    sb = bf16(s)
+    out = {k: torch.zeros_like(v) for k, v in P.items()}
+    out["d_tokens"] = torch.zeros_like(tokens)
+    out["d_pos"] = torch.zeros_like(pos)
+    ds = gs.clone()                                                           # residual term (:141)
+    for net, groups in (("bottom_up", L), ("top_down", L - 1)):
+        W1 = P[f"{net}.net.1.weight"].reshape(groups, 4 * d, d)
+        b1 = P[f"{net}.net.1.bias"].reshape(groups, 4 * d)
+        W2 = P[f"{net}.net.3.weight"].reshape(groups, d, 4 * d)
+        dW1, dW2 = torch.zeros_like(W1), torch.zeros_like(W2)
+        db1, db2 = torch.zeros_like(b1), torch.zeros(groups, d, dtype=torch.float64)
+        for l in range(groups):
+            if net == "bottom_up":
+                x = bf16(tokens if l == 0 else s[:, :, l - 1])
+            else:
+                x = bf16(s[:, :, l + 1] + pos[None])
+            x = x.reshape(B * n, d)
+            dy = gsb[:, :, l].reshape(B * n, d)
+            w1b, w2b = bf16(W1[l]), bf16(W2[l])
+            hv, gp = _gelu_and_grad(x @ w1b.T + b1[l])
+            h, gp = bf16(hv), bf16(gp)
+            dpre = (dy @ w2b) * gp
+            db1[l] = dpre.sum(0)
+            db2[l] = gs[:, :, l].reshape(B * n, d).sum(0)
+            dpre = bf16(dpre)
+            dW2[l] = dy.T @ h
+            dW1[l] = dpre.T @ x
+            dx = (dpre @ w1b).reshape(B, n, d)
+            if net == "bottom_up" and l == 0:
+                out["d_tokens"] += dx
+            elif net == "bottom_up":
+                ds[:, :, l - 1] += dx
+            else:
+                ds[:, :, l + 1] += dx
+                out["d_pos"] += dx.sum(0)
+        out[f"{net}.net.1.weight"] = dW1.reshape(groups * 4 * d, d, 1)
+        out[f"{net}.net.1.bias"] = db1.reshape(-1)
+        out[f"{net}.net.3.weight"] = dW2.reshape(groups * d, 4 * d, 1)
+        out[f"{net}.net.3.bias"] = db2.reshape(-1)
+    # consensus (:56-73), per (image, level): q = v = S_t, k = normalize(S_t)
+    q = s.permute(0, 2, 1, 3)                                                 # b l i d
+    dc = gs.permute(0, 2, 1, 3)
+    rn = 1.0 / q.norm(dim=-1, keepdim=True).clamp_min(1e-12)
+    khat = q * rn
+    scale = d ** -0.5
+    fixed = torch.zeros(n, n, dtype=torch.bool)
+    if not attend_self:
+        fixed |= torch.eye(n, dtype=torch.bool)
+    if mask is not None:
+        fixed |= torch.as_tensor(mask, dtype=torch.bool)
+    if attn_tc:
+        qs, kk, dcs = bf16(q), bf16(khat), bf16(dc)
+    else:
+        qs, kk, dcs = q, khat, dc
+    logits = (qs @ kk.transpose(-1, -2)) * scale
+    if not attend_self:
+        logits = logits.masked_fill(torch.eye(n, dtype=torch.bool)[None, None], TOKEN_ATTEND_SELF_VALUE)
+    if mask is not None:
+        logits = logits.masked_fill(torch.as_tensor(mask, dtype=torch.bool)[None, None], -math.inf)
+    A = logits.softmax(-1)
+    dA = dcs @ qs.transpose(-1, -2)
+    dsim = (A * (dA - (A * dA).sum(-1, keepdim=True))).masked_fill(fixed[None, None], 0.0)
+    if attn_tc:
+        ab, dsb = bf16(A), bf16(scale * dsim)
+    else:
+        ab, dsb = A, scale * dsim
+    dq = ab.transpose(-1, -2) @ dcs + dsb @ kk
+    dk = dsb.transpose(-1, -2) @ qs
+    dq = dq + (dk - khat * (khat * dk).sum(-1, keepdim=True)) * rn
+    ds += dq.permute(0, 2, 1, 3)
+    out["d_state"] = ds
+    return out
+
+
 @torch.no_grad()
 def glom_forward(params, img, *, patch_size, iters=None, levels=None, return_all=False, consensus_self=False,
                  local_consensus_radius=0, dtype=torch.float32):
@@ -64,8 +255,6 @@ def glom_forward(params, img, *, patch_size, iters=None, levels=None, return_all
     tokens = F.linear(x, P["image_to_tokens.1.weight"], P["image_to_tokens.1.bias"])      # (:114)
     n = tokens.shape[1]
     iters = 2 * L if iters is None else iters                                             # (:112)
-    pos = P["pos_emb.weight"][:n][None, :, None, :]                                       # (:117-118)
-    bottom = tokens[:, :, None, :]                                                        # (:121)
     if levels is None:
         levels = P["init_levels"][None, None].expand(B, n, L, d)                          # (:123-124)
     else:
@@ -73,18 +262,9 @@ def glom_forward(params, img, *, patch_size, iters=None, levels=None, return_all
     mask = None
     if local_consensus_radius > 0:
         mask = radius_mask(int(round(math.sqrt(P["pos_emb.weight"].shape[0]))), local_consensus_radius)
-    contrib = torch.full((L,), 4.0, dtype=dtype)                                          # (:128)
-    contrib[-1] = 3.0                                                                     # (:129)
     hiddens = [levels]
     for _ in range(iters):                                                                # (:131)
-        lwi = torch.cat((bottom, levels), dim=-2)                                         # (:132)
-        bu = _grouped_ff(lwi[..., :-1, :], P["bottom_up.net.1.weight"], P["bottom_up.net.1.bias"],
-                         P["bottom_up.net.3.weight"], P["bottom_up.net.3.bias"])          # (:134)
-        td = _grouped_ff(lwi[..., 2:, :] + pos, P["top_down.net.1.weight"], P["top_down.net.1.bias"],
-                         P["top_down.net.3.weight"], P["top_down.net.3.bias"])            # (:136)
-        td = F.pad(td, (0, 0, 0, 1))                                                      # (:137)
-        cons = _consensus(levels, consensus_self, mask)                                   # (:139)
-        levels = (levels + bu + td + cons) / contrib[None, None, :, None]                 # (:141-142)
+        levels = column_step(levels, tokens, P["pos_emb.weight"][:n], P, mask, consensus_self)
         hiddens.append(levels)                                                            # (:145)
     if return_all:
         return torch.stack(hiddens)                                                       # (:147-148)

@@ -56,14 +56,21 @@ GRAD_CASES = {
     # carried-in levels (gradient w.r.t. the input state), radius mask + consensus_self, loss on the last step only
     "grad_c1_masked": dict(dim=64, levels=3, image_size=28, patch_size=7, batch=2, iters=3, return_all=False,
                            param_seed=12, consensus_self=True, local_consensus_radius=1.5, with_levels=True),
+    # two levels (one top-down group), radius 1 (the four grid neighbours, no self), carried-in levels, every time step
+    "grad_l2_radius1": dict(dim=64, levels=2, image_size=16, patch_size=4, batch=2, iters=3, return_all=True,
+                            param_seed=13, local_consensus_radius=1, with_levels=True),
+    # non-square image, n < num_patches: 16x32 with patch 4 -> n = 32 of 64; pos_emb rows >= n get no gradient
+    "grad_nonsquare": dict(dim=64, levels=3, image_size=32, patch_size=4, batch=2, iters=2, return_all=True,
+                           param_seed=14, img_hw=(16, 32)),
 }
 
 
 def grad_inputs(case):
     rng = np.random.default_rng(2000 + case["param_seed"])
     B, L, d = case["batch"], case["levels"], case["dim"]
-    n = (case["image_size"] // case["patch_size"]) ** 2
-    img = rng.standard_normal((B, 3, case["image_size"], case["image_size"])).astype(np.float32)
+    H, W = case.get("img_hw", (case["image_size"],) * 2)
+    n = (H // case["patch_size"]) * (W // case["patch_size"])
+    img = rng.standard_normal((B, 3, H, W)).astype(np.float32)
     lv = rng.standard_normal((B, n, L, d)).astype(np.float32) if case.get("with_levels") else None
     shape = ((case["iters"] + 1,) if case["return_all"] else ()) + (B, n, L, d)
     cot = rng.standard_normal(shape).astype(np.float32)

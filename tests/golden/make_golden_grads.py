@@ -1,6 +1,6 @@
 """Golden GRADIENT fixtures from the live reference (autograd on CPU, fp32).  Run in the build container:
 
-    python tests/golden/make_golden_grads.py
+    python tests/golden/make_golden_grads.py [case ...]      (default: every case)
 
 loss = sum(out * cot) with a seeded cotangent; gradients of every parameter, of the image and (when given) of the
 carried-in `levels` are stored."""
@@ -23,7 +23,8 @@ from cases import GRAD_CASES, grad_inputs  # noqa: E402
 
 def main():
     torch.set_num_threads(8)
-    for name, case in GRAD_CASES.items():
+    for name in sys.argv[1:] or GRAD_CASES:
+        case = GRAD_CASES[name]
         kw = dict(dim=case["dim"], levels=case["levels"], image_size=case["image_size"], patch_size=case["patch_size"],
                   consensus_self=case.get("consensus_self", False),
                   local_consensus_radius=case.get("local_consensus_radius", 0))
