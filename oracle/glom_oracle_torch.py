@@ -6,7 +6,8 @@ that it uses every host core the way the reference's own torch/oneDNN path does.
 arm (``kind: "port"``) ONLY when the unmodified reference package is not importable on the box
 (``$GLOM_REF_PATH`` -> ``baseline/_ref`` -> ``/root/reference``); ``tests/test_oracle_golden.py`` checks it against
 the same golden fixtures as the numpy oracle.  ``column_step`` is the loop body as a differentiable float64-capable
-function; ``grads_at_states`` and ``step_backward_bf16`` are the backward references of ``tests/test_backward_oracle.py``.
+function; ``grads_at_states`` and ``step_backward_bf16`` are the backward references of ``tests/test_backward_oracle.py``,
+``step_forward_bf16`` the one-step forward reference of ``tests/test_forward_oracle.py``.
 Only ``tests/`` and ``bench.py``'s CPU legs may import this module.
 
 Restates (``glom_pytorch/glom_pytorch.py``): GroupedFeedForward :23-36, ConsensusAttention.forward :56-73
@@ -240,6 +241,156 @@ def step_backward_bf16(P, tokens, pos, s, g, *, attend_self=False, mask=None, at
     ds += dq.permute(0, 2, 1, 3)
     out["d_state"] = ds
     return out
+
+
+LOG2E = 1.4426950408889634
+ATTN_BOUND_MAX = 96.0          # attn_kernel: a 16-row warp with a logit bound beyond this takes the exact running maximum
+
+
+def forward_tiles(d):
+    """(bn, part_w) of the bf16 engine at dim d: K2's N tile and the columns of one squared-norm partial."""
+    bn = 256 if d % 256 == 0 else 128 if d % 128 == 0 else 64
+    return bn, 64 if bn == 256 else bn // 2
+
+
+def _fwd_k1_operands(xb, sb, sp):
+    """K1's A operand of each MLP group, (B, n, d): group 2l = bottom-up l (tokens, then S[l-1]), 2l+1 = top-down l."""
+    L = sb.shape[2]
+    ops = []
+    for l in range(L):
+        ops.append(xb if l == 0 else sb[:, :, l - 1])
+        if l < L - 1:
+            ops.append(sp[:, :, l])
+    return ops
+
+
+def _fwd_key_norm(nsq):
+    """attn_row_norm: |S_j| from its squared-norm partials (..., nparts)."""
+    return nsq.sum(-1).sqrt()
+
+
+def _fwd_attn_logits(q, rs, attend_self, mask):
+    """attn_kernel's logits in log2 units, (b, l, i, j): (sb_i . sb_j) rs_j, then the diagonal fill, then the mask."""
+    n = q.shape[-2]
+    x = (q @ q.transpose(-1, -2)) * rs[..., None, :]
+    if not attend_self:
+        x = x.masked_fill(torch.eye(n, dtype=torch.bool), TOKEN_ATTEND_SELF_VALUE * LOG2E)
+    if mask is not None:
+        x = x.masked_fill(mask, -math.inf)
+    return x
+
+
+def _fwd_attn_passes(n):
+    """Key ranges (key0, nk) of the launches of attn_kernel: one up to 576 keys, else passes of 512."""
+    if n <= 576:
+        return [(0, n)]
+    return [(k0, min(512, n - k0)) for k0 in range(0, n, 512)]
+
+
+def _fwd_consensus(sb, nrm, attend_self, mask):
+    """attn_kernel (K3) in float64 with its bf16 roundings.  sb (B, n, L, d) bf16 values, nrm (B, n, L) key norms."""
+    B, n, L, d = sb.shape
+    q = sb.permute(0, 2, 1, 3)                                                # b l i d
+    nrm = nrm.permute(0, 2, 1)
+    c = d ** -0.5 * LOG2E
+    rs, bound = c / nrm.clamp_min(1e-12), c * nrm
+    logits = _fwd_attn_logits(q, rs, attend_self, mask)
+    n16 = -(-n // 16) * 16
+    over = F.pad(~(bound <= ATTN_BOUND_MAX), (0, n16 - n)).reshape(B, L, n16 // 16, 16).any(-1)
+    exact = over.repeat_interleave(16, -1)[..., :n, None]                      # per 16-row warp
+    bnd = bound[..., None]
+    passes = _fwd_attn_passes(n)
+    keys = 256 if len(passes) == 1 and 128 < n16 <= 256 else 128
+    ninf = torch.tensor(-math.inf, dtype=torch.float64)
+    zero = torch.zeros((), dtype=torch.float64)
+    m_acc = torch.full_like(bnd, -math.inf)
+    l_acc = torch.zeros_like(bnd)
+    o_acc = torch.zeros(B, L, n, d, dtype=torch.float64)
+    for k0, nk in passes:
+        m_run = torch.where(exact, ninf, bnd)
+        l_run = torch.zeros_like(bnd)
+        blocks = []
+        for j0 in range(k0, k0 + nk, keys):
+            x = logits[..., j0:min(j0 + keys, k0 + nk)]
+            m_new = torch.maximum(m_run, x.amax(-1, keepdim=True))
+            m_ex = torch.where(m_new == -math.inf, zero, m_new)
+            l_run = torch.where(exact & (m_run > -math.inf), l_run * torch.exp2(m_run - m_ex), torch.where(exact, zero, l_run))
+            m_run = torch.where(exact, m_new, m_run)
+            m_safe = torch.where(exact, m_ex, bnd)
+            e = torch.exp2(x - m_safe)
+            l_run = l_run + e.sum(-1, keepdim=True)
+            blocks.append((bf16(e), m_safe))
+        # exact path: every block's P onto the final maximum, rounded to bf16 a second time
+        m_fin = torch.where(m_run == -math.inf, zero, m_run)
+        p = torch.cat([torch.where(exact & (mu != m_fin), bf16(pb * torch.exp2(mu - m_fin)), pb) for pb, mu in blocks], -1)
+        o = p @ q[..., k0:k0 + nk, :]
+        m_pass = torch.where(l_run == 0, ninf, m_run)                        # no unmasked key in this pass
+        m_new = torch.maximum(m_acc, m_pass)
+        f_old = torch.where(m_acc == -math.inf, zero, torch.exp2(m_acc - m_new))
+        f_new = torch.where(m_pass == -math.inf, zero, torch.exp2(m_pass - m_new))
+        l_acc = l_acc * f_old + l_run * f_new
+        o_acc = o_acc * f_old + o * f_new
+        m_acc = m_new
+    return bf16(o_acc / l_acc).permute(0, 2, 1, 3)
+
+
+def _fwd_k2(S, H, C, w2bu, w2td, b2, contrib):
+    """K2: S' = ((S + (acc + b2)) + C) / c_l with acc = H_bu,l W2bu_l^T + H_td,l W2td_l^T.  H (G, B*n, 4d)."""
+    B, n, L, d = S.shape
+    acc = []
+    for l in range(L):
+        a = H[2 * l] @ w2bu[l].T
+        if l < L - 1:
+            a = a + H[2 * l + 1] @ w2td[l].T
+        acc.append(a.reshape(B, n, d))
+    acc = torch.stack(acc, 2)
+    return ((S + (acc + b2)) + C) / contrib[None, None, :, None]
+
+
+def step_forward_bf16(P, tokens, pos, S, *, attend_self=False, mask=None):
+    """One step of the bf16 engine (K1 -> K3 -> K2), float64 except for bf16 rounding at exactly the points where the
+    kernels round.  S = S_t (B, n, L, d), tokens (B, n, d), pos (n, d), mask (n, n) bool (True = masked) or None.
+    Returns {"state": S_{t+1}, "H": (2L-1, B*n, 4d) hidden activations by group (bu_0, td_0, bu_1, ...), "C": (B, n, L, d)
+    consensus, "nsq": (B*n, L, nparts) squared-norm partials of S_{t+1}}.
+
+    Roundings (prep_state_kernel, pack_weights_kernel, gemm_kernel, attn_kernel):
+      shadows xb = bf16(tokens), sb = bf16(S), sp = bf16(fp32(S[:, :, 1:] + pos)); W1, W2 in bf16; b1, b2 stay fp32
+      (b2 = bu_b2 + td_b2, summed in fp32 by the packer: below this reference's resolution, kept in float64 here).
+      K1: H_g = bf16(gelu(A_g W1_g^T + b1_g)); the kernel's GELU fit is within 1.9e-6 of the erf form used here.
+      K3: key norm |S_j| from the partials of S, logits (sb_i . sb_j) d^-1/2 log2e / max(|S_j|, 1e-12) in log2 units,
+          diagonal -5e-4 log2e unless attend_self, masked keys -inf; stabiliser = the Cauchy-Schwarz bound
+          d^-1/2 log2e |S_i| unless a row of the 16-row warp has a bound > ATTN_BOUND_MAX, then the exact running maximum
+          per key block (256 keys for a single pass of 129..256 padded keys, else 128), each block's P rounded at its own
+          maximum and rescaled and rounded again onto the final one; P = bf16(2^(logit - m)), row sum of the unrounded
+          values, C = bf16(P sb / l); beyond 576 keys, passes of 512 with (m, l, O) carried between them.
+      K2: S_{t+1} = ((S + (acc + b2)) + C) / 3 on the top level, * 0.25 elsewhere; nsq = sum of squares of S_{t+1}
+          over each part_w-column part."""
+    P = {k: _f64(P[k]) for k in MLP_KEYS}
+    tokens, pos, S = _f64(tokens), _f64(pos), _f64(S)
+    B, n, L, d = S.shape
+    _, part_w = forward_tiles(d)
+    if mask is not None:
+        mask = torch.as_tensor(mask, dtype=torch.bool, device="cpu")
+    xb, sb = bf16(tokens), bf16(S)
+    sp = bf16(S[:, :, 1:] + pos[None, :, None, :])
+    w1 = [P["bottom_up.net.1.weight"].reshape(L, 4 * d, d), P["top_down.net.1.weight"].reshape(L - 1, 4 * d, d)]
+    b1 = [P["bottom_up.net.1.bias"].reshape(L, 4 * d), P["top_down.net.1.bias"].reshape(L - 1, 4 * d)]
+    H = []
+    for g, a in enumerate(_fwd_k1_operands(xb, sb, sp)):
+        net, l = g & 1, g >> 1
+        H.append(bf16(F.gelu(a.reshape(B * n, d) @ bf16(w1[net][l]).T + b1[net][l])))
+    H = torch.stack(H)
+    nsq_in = S.reshape(B, n, L, d // part_w, part_w).square().sum(-1)
+    C = _fwd_consensus(sb, _fwd_key_norm(nsq_in), attend_self, mask)
+    contrib = torch.full((L,), 4.0, dtype=torch.float64)
+    contrib[-1] = 3.0
+    b2 = P["bottom_up.net.3.bias"].reshape(L, d).clone()
+    b2[:-1] += P["top_down.net.3.bias"].reshape(L - 1, d)
+    w2bu = bf16(P["bottom_up.net.3.weight"].reshape(L, d, 4 * d))
+    w2td = bf16(P["top_down.net.3.weight"].reshape(L - 1, d, 4 * d))
+    state = _fwd_k2(S, H, C, w2bu, w2td, b2, contrib)
+    nsq = state.reshape(B * n, L, d // part_w, part_w).square().sum(-1)
+    return {"state": state, "H": H, "C": C, "nsq": nsq}
 
 
 @torch.no_grad()

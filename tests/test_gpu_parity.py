@@ -107,7 +107,8 @@ def test_zero_iters_returns_initial_state_and_fresh_tensor():
 
 def test_stage_buffers_hidden_and_consensus():
     """Single-stage checks through the workspace: after one bf16 step the hidden activations H and
-    the consensus C left in the workspace match the oracle's (localises GEMM1 / attention faults)."""
+    the consensus C left in the workspace match the oracle's (localises GEMM1 / attention faults), and match
+    step_forward_bf16 per kernel tile at the bounds of tests/test_forward_oracle.py."""
     case, params, _ = load("mid_return_all")
     m = make_model(case, params, "bf16")
     img, _ = inputs(case)
@@ -145,6 +146,15 @@ def test_stage_buffers_hidden_and_consensus():
         assert err <= 2e-2 * max(1.0, np.abs(want).max()), ("H td", l, err)
     wantC = O.consensus(S0, False, None)
     assert np.abs(C - wantC).max() <= 2e-2 * max(1.0, np.abs(wantC).max())
+    # per K1 tile / K3 item against the bf16-faithful one-step reference, fed the engine's own tokens
+    from test_forward_oracle import TOL, check, errors
+    from oracle import glom_oracle_torch as OT
+    with torch.no_grad():
+        tok = m.tokens(x).cpu()
+    Pt = {k: q.detach().cpu() for k, q in m.named_parameters()}
+    emu = OT.step_forward_bf16(Pt, tok, Pt["pos_emb.weight"][:n], torch.from_numpy(np.ascontiguousarray(S0)))
+    got = {"H": torch.from_numpy(H).permute(1, 0, 2), "C": torch.from_numpy(C)}
+    check(errors(got, {"H": emu["H"], "C": emu["C"]}, (B, n, L, d)), TOL["emu"], "stage buffers")
 
 
 def test_native_tokenizer_matches_oracle():
