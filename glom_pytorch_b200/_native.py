@@ -47,6 +47,7 @@ SIGNATURES = {
     "glom_b200_settle": (_i32, _SETTLE),
     "glom_b200_settle_all_workspace_bytes": (_i32, [_CFG, _i32, _i32, _SZP]),
     "glom_b200_settle_all": (_i32, _SETTLE),
+    "glom_b200_settle_workspace_offset": (_i32, [_CFG, _i32, _i32, _i32, _i32, _SZP, _SZP]),
     "glom_b200_forward_steps_workspace_bytes": (_i32, [_CFG, _i32, _i32, _i32, _SZP]),
     "glom_b200_forward_steps": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _sz, _vp]),
     "glom_b200_tokenize_workspace_bytes": (_i32, [_i32, _i32, _i32, _i32, _i32, _i32, _SZP]),
@@ -123,6 +124,14 @@ def workspace_offset(cfg, batch, iters, return_all, which):
     off, nb = ctypes.c_size_t(), ctypes.c_size_t()
     check(load().glom_b200_workspace_offset(ctypes.byref(cfg), batch, iters, int(return_all), which,
                                             ctypes.byref(off), ctypes.byref(nb)))
+    return off.value, nb.value
+
+
+def settle_workspace_offset(cfg, batch, max_iters, return_all, which):
+    """(offset, bytes) of settle buffer `which` (0 dsq, 1 level_q, 2 frozen, 3 block_frozen) in the settle workspace."""
+    off, nb = ctypes.c_size_t(), ctypes.c_size_t()
+    check(load().glom_b200_settle_workspace_offset(ctypes.byref(cfg), batch, max_iters, int(return_all), which,
+                                                   ctypes.byref(off), ctypes.byref(nb)))
     return off.value, nb.value
 
 

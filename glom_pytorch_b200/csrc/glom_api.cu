@@ -73,10 +73,10 @@ SettleLayout settle_layout(const Geometry& g, int max_iters, int return_all) {
   s.fwd = workspace_layout(g, GLOM_B200_BF16, max_iters, return_all);
   size_t off = s.fwd.total;
   s.dsq_off = off; off = align_up(off + s.fwd.nsq_bytes, 1024);
-  s.flags_off = off;
-  s.frozen_off = off; off += (size_t)g.B * 4;
-  s.block_frozen_off = off; off += (size_t)(g.rows + 255) / 256 * 4;
-  s.done_off = off; off += 4;
+  s.flags_off = off;                  // each flag buffer 16-byte aligned: glom_b200_settle_workspace_offset hands them out
+  s.frozen_off = off; off = align_up(off + (size_t)g.B * 4, 16);
+  s.block_frozen_off = off; off = align_up(off + (size_t)(g.rows + 255) / 256 * 4, 16);
+  s.done_off = off; off = align_up(off + 4, 16);
   s.level_q_off = off; off += (size_t)g.B * g.L * 4;
   s.flags_bytes = off - s.flags_off;
   s.total = align_up(off, 1024);
@@ -259,6 +259,21 @@ static int settle_impl(const glom_b200_cfg* cfg, const void* packed_weights, con
 
 GLOM_B200_API int glom_b200_settle_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_iters, size_t* out_bytes) {
   return freeze_workspace_bytes(kSettle, cfg, batch, max_iters, 0, out_bytes);
+}
+
+GLOM_B200_API int glom_b200_settle_workspace_offset(const glom_b200_cfg* cfg, int batch, int max_iters, int return_all,
+                                                    int which, size_t* out_offset, size_t* out_bytes) {
+  if (int r = check_freeze(kSettle, cfg, batch, max_iters)) return r;
+  if (!out_offset || !out_bytes) return fail(GLOM_B200_ERR_INVALID, "settle: out_offset / out_bytes is NULL");
+  const Geometry g = make_geometry(cfg, batch);
+  const SettleLayout s = settle_layout(g, max_iters, return_all ? 1 : 0);
+  switch (which) {
+    case 0: *out_offset = s.dsq_off; *out_bytes = s.fwd.nsq_bytes; return 0;
+    case 1: *out_offset = s.level_q_off; *out_bytes = (size_t)g.B * g.L * 4; return 0;
+    case 2: *out_offset = s.frozen_off; *out_bytes = (size_t)g.B * 4; return 0;
+    case 3: *out_offset = s.block_frozen_off; *out_bytes = (size_t)(g.rows + 255) / 256 * 4; return 0;
+    default: return fail(GLOM_B200_ERR_INVALID, "unknown settle buffer id %d", which);
+  }
 }
 
 GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,

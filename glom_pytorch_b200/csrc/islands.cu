@@ -124,6 +124,13 @@ cudaError_t launch_islands(const float* states, int slabs, int side_h, int side_
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   const size_t smem = (size_t)n * 4 + 2 * (size_t)n;
+  // 6n bytes plus the kernel's static shared memory exceed the default 48 KB per block from n = 8190 on (the API allows
+  // n <= 8192): opt in above 46 KB
+  static SmemOptIn optin;
+  if (smem > 46 * 1024) {
+    e = optin.ensure(island_label_kernel, smem);
+    if (e != cudaSuccess) return e;
+  }
   island_label_kernel<<<dim3(L, slabs), 256, smem, st>>>(cos_right, cos_down, side_h, side_w, threshold, agreement,
                                                           labels, num_islands);
   if (launches) ++*launches;

@@ -191,6 +191,17 @@ GLOM_B200_API int glom_b200_last_launch_count(void);
 GLOM_B200_API int glom_b200_workspace_offset(const glom_b200_cfg* cfg, int batch, int iters, int return_all,
                                int which, size_t* out_offset, size_t* out_bytes);
 
+/* Diagnostics: byte offsets of the settle buffers inside the workspace of glom_b200_settle (return_all = 0) or
+ * glom_b200_settle_all (return_all = 1) for the same (cfg, batch, max_iters).  Each is 16-byte aligned and lies after
+ * the forward layout, so H, C and the squared-norm partials are found with glom_b200_workspace_offset(iters = max_iters).
+ * which: 0 = squared-change partials of the last step (rows, L, nparts) f32,
+ *        1 = per-(image, level) ratios q (B, L) f32 of each image's last step,
+ *        2 = frozen (B) int32, 1: the image met the stopping rule,
+ *        3 = block_frozen (ceil(rows / 256)) int32, 1: every image with rows in the 256-row block is frozen.
+ * Argument errors (those of glom_b200_settle_workspace_bytes, unknown ids) are reported before any device query. */
+GLOM_B200_API int glom_b200_settle_workspace_offset(const glom_b200_cfg* cfg, int batch, int max_iters, int return_all,
+                                                    int which, size_t* out_offset, size_t* out_bytes);
+
 /* Backward of the column update: gradients of glom_b200_forward's loop
  * (glom_pytorch.py:123-148) with respect to tokens, pos, the initial state (or init_levels) and the
  * eight MLP tensors, given dL/d(output).  Per-step intermediates are recomputed from the saved states.  precision

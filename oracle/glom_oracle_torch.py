@@ -7,7 +7,8 @@ arm (``kind: "port"``) ONLY when the unmodified reference package is not importa
 (``$GLOM_REF_PATH`` -> ``baseline/_ref`` -> ``/root/reference``); ``tests/test_oracle_golden.py`` checks it against
 the same golden fixtures as the numpy oracle.  ``column_step`` is the loop body as a differentiable float64-capable
 function; ``grads_at_states`` and ``step_backward_bf16`` are the backward references of ``tests/test_backward_oracle.py``,
-``step_forward_bf16`` the one-step forward reference of ``tests/test_forward_oracle.py``.
+``step_forward_bf16`` the one-step forward reference of ``tests/test_forward_oracle.py``, ``settle_change``,
+``settle_ratio`` and ``settle_rule`` the settle references of ``tests/test_settle_oracle.py``.
 Only ``tests/`` and ``bench.py``'s CPU legs may import this module.
 
 Restates (``glom_pytorch/glom_pytorch.py``): GroupedFeedForward :23-36, ConsensusAttention.forward :56-73
@@ -391,6 +392,33 @@ def step_forward_bf16(P, tokens, pos, S, *, attend_self=False, mask=None):
     state = _fwd_k2(S, H, C, w2bu, w2td, b2, contrib)
     nsq = state.reshape(B * n, L, d // part_w, part_w).square().sum(-1)
     return {"state": state, "H": H, "C": C, "nsq": nsq}
+
+
+def settle_change(s_prev, s_next, part_w):
+    """K2's squared-change partials of a settle step in float64: (B, n, L, d) states S_{k-1}, S_k -> (B*n, L, nparts),
+    sum of |S_k - S_{k-1}|^2 over each part_w-column part (part_w as in forward_tiles)."""
+    s_prev, s_next = _f64(s_prev), _f64(s_next)
+    B, n, L, d = s_next.shape
+    return (s_next - s_prev).reshape(B * n, L, d // part_w, part_w).square().sum(-1)
+
+
+def settle_ratio(dsq, s_next):
+    """settle_converge_kernel's ratio in float64: q[b, l] = sqrt(sum_i dsq[b, i, l] / sum_i |S_k[b, i, l]|^2) from the
+    change partials (B*n, L, nparts) and S_k (B, n, L, d); 0/0 counts as 0, x/0 (x > 0) as inf."""
+    s_next = _f64(s_next)
+    B, n, L, d = s_next.shape
+    num = _f64(dsq).reshape(B, n, L, -1).sum(dim=(1, 3))
+    den = s_next.square().sum(dim=(1, 3))
+    return torch.where((num == 0) & (den == 0), torch.zeros_like(num), (num / den).sqrt())
+
+
+def settle_rule(q_per_step, tol):
+    """The stopping rule: q_per_step (K, B, L), the ratios of steps 1..K -> steps (B,) int32, the first k at which every
+    level has q <= tol (a NaN never stops an image), K for an image that never stops."""
+    hit = (torch.as_tensor(q_per_step) <= tol).all(dim=-1)              # (K, B)
+    K = hit.shape[0]
+    first = torch.where(hit, torch.arange(1, K + 1)[:, None], torch.full_like(hit, K + 1, dtype=torch.long))
+    return first.amin(dim=0).clamp_max(K).to(torch.int32)
 
 
 @torch.no_grad()
