@@ -9,7 +9,7 @@ LIB_PATH = os.environ.get("GLOM_B200_LIB") or os.path.join(_PKG, "libglom_b200.s
 
 ABI_VERSION = 1
 PRECISION = {"fp32": 0, "bf16": 1}
-PROFILE_KINDS = ("attention", "gemm1_gelu", "gemm2_combine", "prologue", "tokenize", "mlp_fused")
+PROFILE_KINDS = ("attention", "gemm1_gelu", "gemm2_combine", "prologue", "tokenize")
 
 
 class Cfg(ctypes.Structure):
@@ -62,7 +62,6 @@ SIGNATURES = {
     "glom_b200_profile_begin": (_i32, []),
     "glom_b200_profile_end": (_i32, [ctypes.POINTER(ctypes.c_double), _I32P, _i32]),
     "glom_b200_islands": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "glom_b200_mlp_schedule": (_i32, [_CFG, _i32, _i32, _vp, _i32, _I32P, _I32P]),
     "glom_b200_clock_probe": (_i32, [_vp, _i32, _vp]),
     "glom_b200_kernel_clocks": (_i32, [_vp, _vp, _vp, _i32, _i32]),
 }
@@ -257,15 +256,6 @@ def kernel_clocks(reset=True):
     mhz, ms, wf = (ctypes.c_double * k)(), (ctypes.c_double * k)(), (ctypes.c_double * (6 * k))()
     check(load().glom_b200_kernel_clocks(mhz, ms, wf, k, int(bool(reset))))
     return {PROFILE_KINDS[i]: (mhz[i], ms[i], [round(wf[6 * i + j], 4) for j in range(6)]) for i in range(k) if ms[i] > 0}
-
-
-def mlp_schedule(cfg, batch, num_sms=132):
-    """Work list of the merged MLP kernel: (list of (kind, z, m_blk, n_blk), delay).  Host only."""
-    n, dl = ctypes.c_int(), ctypes.c_int()
-    check(load().glom_b200_mlp_schedule(ctypes.byref(cfg), batch, num_sms, None, 0, ctypes.byref(n), ctypes.byref(dl)))
-    buf = (ctypes.c_int32 * (4 * n.value))()
-    check(load().glom_b200_mlp_schedule(ctypes.byref(cfg), batch, num_sms, buf, n.value, ctypes.byref(n), ctypes.byref(dl)))
-    return [tuple(buf[4 * i:4 * i + 4]) for i in range(n.value)], dl.value
 
 
 def islands(states_ptr, slabs, side_h, side_w, levels, dim, threshold, cos_right_ptr, cos_down_ptr, agreement_ptr,

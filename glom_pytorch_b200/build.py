@@ -9,7 +9,7 @@ import sys
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libglom_b200.so")
-SOURCES = ["glom_api.cu", "simt_kernels.cu", "tc_kernels.cu", "mlp_kernel.cu", "islands.cu", "bwd_kernels.cu", "tc_bwd_kernels.cu",
+SOURCES = ["glom_api.cu", "simt_kernels.cu", "tc_kernels.cu", "islands.cu", "bwd_kernels.cu", "tc_bwd_kernels.cu",
            "settle_kernels.cu"]
 HEADERS = ["engine.h", "ptx.cuh", "tc_common.cuh", os.path.join("..", "..", "include", "glom_b200.h")]
 NVCC_FLAGS = [

@@ -1,5 +1,5 @@
-// Pieces shared by the tensor-core kernels (tc_kernels.cu: K1 / K2 / K3, mlp_kernel.cu: the merged persistent MLP
-// kernel): tile constants, the accumulator hand-off, the K1 / K2 epilogue chunk bodies and the tensor-map helpers.
+// Pieces shared by the tensor-core kernels: tile constants, the accumulator hand-off, the K2 epilogue chunk body and the
+// tensor-map helpers.
 #pragma once
 #include "engine.h"
 #include "ptx.cuh"
@@ -72,45 +72,6 @@ __device__ __forceinline__ float row_chunk_sumsq(float a, float b, float c, floa
   q += __shfl_xor_sync(0xffffffffu, q, 2);
   q += __shfl_xor_sync(0xffffffffu, q, 4);
   return q;
-}
-
-// ---- K1 epilogue chunk: 32 rows x 32 columns.  Row-per-thread bias + exact-erf GELU + bf16 pack, transpose
-// through the warp's 2 KB patch (16-byte chunk c of row r stored at chunk c ^ ((r >> 1) & 3)), then 64-byte
-// row segments out (8 rows x 64 B per store instruction).
-// HPOL: 0 = streaming stores (two-kernel step: H is consumed by the NEXT launch, keep it out of L2's way),
-//       1 = L2 evict-last policy `pol` (merged MLP kernel: H is consumed a few row blocks later by GEMM2 tiles of the same launch
-//           and must survive the rest of the traffic until then; the consumer's evict-first loads demote it again)
-template <bool FULL, int HPOL = 0>
-__device__ __forceinline__ void k1_chunk(const uint32_t (&v)[32], const float* bias, uint8_t* patch,
-                                         __nv_bfloat16* hdst /* &H[row0][col] */, size_t pitch, int lane, int rows_left,
-                                         uint64_t pol = 0) {
-  uint32_t pk[16];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    // bias slice read per use (broadcast LDS.128): 32 fewer live registers, so the polynomial's constant pairs stay in
-    // registers instead of being re-materialised for every pair
-    const float4 b = *reinterpret_cast<const float4*>(bias + 4 * i);
-    pk[2 * i] = gelu_pair_bf16(__uint_as_float(v[4 * i + 0]), __uint_as_float(v[4 * i + 1]), b.x, b.y);
-    pk[2 * i + 1] = gelu_pair_bf16(__uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3]), b.z, b.w);
-  }
-#pragma unroll
-  for (int c = 0; c < 4; ++c)
-    *reinterpret_cast<uint4*>(patch + lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4)) =
-        make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
-  __syncwarp();
-  const int c = lane & 3;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = i * 8 + (lane >> 2);
-    const uint4 val = *reinterpret_cast<const uint4*>(patch + r * 64 + ((c ^ ((r >> 1) & 3)) << 4));
-    // streaming (evict-first) stores: H (369 MB per step) never fits L2, and letting it through the normal policy
-    // would evict the state shadows and weights the GEMMs and the consensus kernel re-read
-    if (FULL || r < rows_left) {
-      if (HPOL == 0) __stcs(reinterpret_cast<uint4*>(hdst + (size_t)r * pitch + c * 8), val);
-      else st_global_v4_hint(hdst + (size_t)r * pitch + c * 8, val, pol);
-    }
-  }
-  __syncwarp();
 }
 
 // ---- K2 epilogue chunk: the 4-way combine (glom_pytorch.py:141-142) on a 32 x 32 accumulator chunk.

@@ -65,11 +65,6 @@ struct GemmParams {
   // tokeniser (MODE 2)
   float* tok_out;
   int tok_kb;      // K blocks of 64 of the zero-padded patch dimension
-  int h_prefetch;  // K2: k-blocks of H prefetched into L2 ahead of the TMA loads (0 = off)
-  int z_rev;        // K1: groups walked from G - 1 down to z0 (see step_bf16)
-  int h_keep_z;     // K1: H blocks of groups <= h_keep_z are stored with the default L2 policy instead of evict-first
-  int h_load_policy; // K2: L2 hint of the H loads (GLOM_B200_K2_HPOL, default 0 = evict-first on every load)
-  int epi_prefetch; // K2: L2 prefetch of the epilogue's state / consensus lines at tile start (GLOM_B200_K2_EPI_PREFETCH, default on)
   // SETTLE instantiations (Glom.settle), flags written by the convergence kernel of the previous step
   const int* frozen;        // [B] 1: the image has stopped
   const int* block_frozen;  // [num_m] 1: every row of the 256-row block belongs to a stopped image
@@ -110,7 +105,7 @@ __device__ __forceinline__ TileInfo decode_tile(const GemmParams& p, int tile) {
   t.n_blk = tile % p.num_n;
   const int r = tile / p.num_n;
   t.m_blk = r % p.num_m;
-  t.z = (MODE == 0 && p.z_rev) ? p.G - 1 - r / p.num_m : p.z0 + r / p.num_m;
+  t.z = p.z0 + r / p.num_m;
   if (MODE == 0) t.num_kb = p.d / BK;
   else if (MODE == 1) t.num_kb = ((t.z == p.L - 1) ? 4 * p.d : 8 * p.d) / BK;   // top level: no top-down half (:137)
   else t.num_kb = p.tok_kb;
@@ -227,26 +222,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
       const uint64_t pol_first = l2_policy_evict_first();
       const int kbg_n = 4 * p.d / BK;
       const int blk_skip = (p.m128 - 1) * kbg_n;
-      // K2: H comes from HBM (written by the previous launch) and the ring is consumed in order.  A cursor running
-      // h_prefetch k-blocks ahead of the loads (across tile boundaries) can pull the 16 KB blocks into L2 first.
-      int pf_it = 0, pf_kb = 0, pf_nkb = 0, pf_blk0 = 0;
-      bool pf_valid = false;
-      auto pf_tile = [&](int it_) {
-        pf_it = it_; pf_kb = 0;
-        const int tl = sched_tile<MODE>(p, cluster_id, num_clusters, it_);
-        pf_valid = tl >= 0;
-        if (pf_valid) {
-          const TileInfo tt = decode_tile<MODE>(p, tl);
-          pf_nkb = tt.num_kb;
-          pf_blk0 = (2 * tt.z * p.m128 + ((tt.m_blk * 256 + cta_rank * BM) >> 7)) * kbg_n;
-        }
-      };
-      auto pf_step = [&]() {
-        if (!pf_valid) return;
-        const int blk = pf_blk0 + pf_kb + (pf_kb >= kbg_n ? blk_skip : 0);
-        if (elected) tma_prefetch_2d(&map_a0, 0, blk * BM);
-        if (++pf_kb == pf_nkb) pf_tile(pf_it + 1);
-      };
       for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
         const TileInfo t = decode_tile<MODE>(p, tile);
         if constexpr (SETTLE) { if (p.block_frozen[t.m_blk]) continue; }
@@ -269,12 +244,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
         // K2: block (group g, 128-row block, 64-wide k block); [H_bu,l | H_td,l] are groups 2l and 2l+1, so k block kb
         // of the concatenation is block blk0 + kb of group 2l and, from kb = kbg_n on, of the group behind it
         const int blk0 = (2 * t.z * p.m128 + (a_row >> 7)) * kbg_n;
-        if (MODE == 1 && it == 0 && p.h_prefetch > 0) {            // prime the prefetch cursor
-          pf_tile(0);
-          for (int i = 0; i < p.h_prefetch; ++i) pf_step();
-        }
         for (int kb = 0; kb < t.num_kb; ++kb) {
-          if (MODE == 1 && p.h_prefetch > 0) pf_step();
           GLOM_CNT_WAIT(w0, mbar_wait(&empty_bar[stage], phase ^ 1));
           if (elected) {
             const uint32_t sa = smem0 + (uint32_t)stage * Cfg::STAGE_BYTES;
@@ -283,9 +253,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
             if (MODE == 1) {
               const int blk = blk0 + kb + (kb >= kbg_n ? blk_skip : 0);
               // H streams through once per pair of column tiles: evict-first keeps it from displacing weights / state
-              // (h_load_policy, diagnostics: 1 = only the row block's last column tile marks it evict-first, 2 = no hint)
-              if (p.h_load_policy == 0 || (p.h_load_policy == 1 && t.n_blk == p.num_n - 1)) tma_load_2d_hint(sa, amap, bar, 0, blk * BM, pol_first);
-              else tma_load_2d(sa, amap, bar, 0, blk * BM);
+              tma_load_2d_hint(sa, amap, bar, 0, blk * BM, pol_first);
             } else {
               tma_load_2d(sa, amap, bar, a_col + kb * BK, a_row);
             }
@@ -309,7 +277,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
     uint8_t* patch = patches + (size_t)cw * Cfg::PATCH_BYTES;
     float* xch_p = xch + pair * 32;
     const uint32_t smem0 = smem_u32(smem);
-    const uint64_t pol_keep = l2_policy_evict_normal();
     const uint64_t pol_stream = l2_policy_evict_first();
     // K1: the thread that issues the warpgroup's TMA stores (bulk groups are tracked per thread) and the lane's part of the
     // stmatrix addresses: lanes 8i .. 8i + 7 address the rows of matrix i = (column group j & 1, row half h)
@@ -332,7 +299,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
       uint32_t live = ~0u;                                              // SETTLE, K2: bit r = row row0 + r is stored
       if constexpr (SETTLE && MODE == 1)
         live = __ballot_sync(0xffffffffu, row0 + lane < p.rows && !p.frozen[(row0 + lane) / p.n]);
-      if (MODE == 1 && p.epi_prefetch && lane < rows_left) {
+      if (MODE == 1 && lane < rows_left) {
         // The combine reads this band's fp32 state and C lines: pull them into L2 before the main loop, so the epilogue's
         // dependent global loads hit L2 instead of paying the HBM latency
         const size_t o = ((size_t)(row0 + lane) * p.L + t.z) * p.d + t.n_blk * BN + x * (BN / 2);
@@ -375,8 +342,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
         if (wrow0 < p.rows) {                                           // warpgroup-uniform
           const int hblk0 = (t.z * p.m128 + (t.m_blk * 2 + cta_rank)) * (4 * p.d / BK) + t.n_blk * (BN / BK);
           const float* bias = p.bias + (size_t)t.z * 4 * p.d + t.n_blk * BN + 2 * (lane & 3);
-          // groups read first by the GEMM2 launch that follows keep the default policy (stay in L2 if they fit)
-          const uint64_t pol = t.z <= p.h_keep_z ? pol_keep : pol_stream;
           // all of the tile's GELU work first, with no barrier in between: pk[16 s + 2 j + h] holds columns
           // 64 s + 8 j + 2 (lane & 3) + {0, 1} of row half h
           uint32_t pk[BN / 4];
@@ -403,7 +368,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
           if (st_issuer) {
 #pragma unroll
             for (int s = 0; s < BN / 64; ++s)
-              tma_store_2d_hint(&map_out, out_wg + (uint32_t)s * Cfg::OUT_BOX_BYTES, 0, (hblk0 + s) * BM + 64 * wg, pol);
+              tma_store_2d_hint(&map_out, out_wg + (uint32_t)s * Cfg::OUT_BOX_BYTES, 0, (hblk0 + s) * BM + 64 * wg, pol_stream);
             bulk_commit_group();
           }
         }
@@ -1157,14 +1122,9 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiled
   return 0;
 }
 
-int step_bf16(const Geometry& g, const Bf16Buffers& b, int* sched, int step_index, EncodeTiledFn enc, int num_sms, cudaStream_t st,
+int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTiledFn enc, int num_sms, cudaStream_t st,
               int* launches, char* err, size_t errlen, Profiler* prof) {
   const int d = g.d, L = g.L, n = g.n, rows = g.rows;
-  if (sched && mlp_fused_supported(g)) {
-    // consensus first (reads the state shadow of step t), then ONE persistent kernel for both grouped GEMMs
-    if (int rc = launch_attention(g, b, enc, num_sms, st, launches, err, errlen, prof)) return rc;
-    return step_bf16_mlp_fused(g, b, sched, enc, num_sms, st, launches, err, errlen, prof);
-  }
   // One launch each of K1 (all groups), K3, K2 (all levels).
   // H: (group, 128-row block, 64-column k block) blocks of 128 x 64, read by K2 a block at a time (mh) and written by
   // K1 a warpgroup's 64 rows at a time (mh_out)
@@ -1184,18 +1144,10 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int* sched, int step_inde
     GemmParams p{};
     p.rows = rows; p.d = d; p.L = L; p.n = n; p.G = g.G;
     // group 0 (bottom-up net of level 0) reads the tokens, which are the same in every step of a call (:132-134): its block
-    // of H is written by the call's first step and stays valid; the later steps run the other 2L - 2 groups only
-    static int reuse_g0 = -1;
-    if (reuse_g0 < 0) { const char* ev = getenv("GLOM_B200_REUSE_BU0"); reuse_g0 = ev ? atoi(ev) : 1; }
-    p.z0 = (step_index > 0 && reuse_g0 && g.G > 1) ? 1 : 0;
-    // Group order: GEMM2 of the previous step wrote the shadows level 0 first, the top level last, and this step's GEMM2
-    // reads H level 0 first.  Walking the groups from the top down reads the most recently written shadows first (L2
-    // hits) and leaves the groups GEMM2 starts with (levels 0, 1) as the last ones written; those are stored with the
-    // default L2 policy instead of evict-first.  (GLOM_B200_K1_ORDER: bit 0 = reverse walk, bits 1.. = keep groups)
-    static int k1_order = -1;
-    if (k1_order < 0) { const char* ev = getenv("GLOM_B200_K1_ORDER"); k1_order = ev ? atoi(ev) : 0; }
-    p.z_rev = k1_order & 1;
-    p.h_keep_z = (k1_order >> 1) - 1;
+    // of H is written by the call's first step and stays valid; the later steps run the other 2L - 2 groups only.
+    // The groups are walked upward from z0, and every H box is stored evict-first: H streams through L2 and must not
+    // displace the weights and state shadows that the GEMMs and the consensus kernel re-read
+    p.z0 = (step_index > 0 && g.G > 1) ? 1 : 0;
     p.num_m = (rows + 255) / 256; p.num_n = 4 * d / 256; p.num_tiles = (g.G - p.z0) * p.num_m * p.num_n;
     p.bias = b.b1; p.m128 = m128;
     p.frozen = b.frozen; p.block_frozen = b.block_frozen;
@@ -1216,15 +1168,6 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int* sched, int step_inde
     p.bias = b.b2; p.s32_in = b.s32_in; p.s_bcast = b.s32_in_bcast; p.c_in = b.c; p.pos = b.pos;
     p.s32_out = b.s32_out; p.sb_out = b.sb_out; p.sp_out = b.sp_out; p.nsq_out = b.nsq_out; p.nparts = g.nparts;
     p.frozen = b.frozen; p.block_frozen = b.block_frozen; p.dsq_out = b.dsq_out;
-    static int h_pf = -1;
-    if (h_pf < 0) { const char* ev = getenv("GLOM_B200_K2_PREFETCH"); h_pf = ev ? atoi(ev) : 0; }
-    p.h_prefetch = h_pf;
-    static int epi_pf = -1;
-    if (epi_pf < 0) { const char* ev = getenv("GLOM_B200_K2_EPI_PREFETCH"); epi_pf = ev ? atoi(ev) : 1; }
-    p.epi_prefetch = epi_pf;
-    static int k2_hpol = -1;
-    if (k2_hpol < 0) { const char* ev = getenv("GLOM_B200_K2_HPOL"); k2_hpol = ev ? atoi(ev) : 0; }
-    p.h_load_policy = k2_hpol;
     cudaError_t e;
     ProfScope scope(prof, PROF_GEMM2, st);
     if (g.bn2 == 256) e = launch_gemm<1, 256>(mh, mh, mh, mw2, mh, p, num_sms, st);
