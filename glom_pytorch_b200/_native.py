@@ -48,6 +48,10 @@ SIGNATURES = {
     "glom_b200_settle_all_workspace_bytes": (_i32, [_CFG, _i32, _i32, _SZP]),
     "glom_b200_settle_all": (_i32, _SETTLE),
     "glom_b200_settle_workspace_offset": (_i32, [_CFG, _i32, _i32, _i32, _i32, _SZP, _SZP]),
+    "glom_b200_settle_queue_workspace_bytes": (_i32, [_CFG, _i32, _i32, _SZP]),
+    "glom_b200_settle_queue_begin": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _sz, _vp]),
+    "glom_b200_settle_queue_run": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _sz, _vp,
+                                          _i32, _i32, _vp]),
     "glom_b200_forward_steps_workspace_bytes": (_i32, [_CFG, _i32, _i32, _i32, _SZP]),
     "glom_b200_forward_steps": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _sz, _vp]),
     "glom_b200_tokenize_workspace_bytes": (_i32, [_i32, _i32, _i32, _i32, _i32, _i32, _SZP]),
@@ -201,6 +205,26 @@ def settle(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr
     fn = lib.glom_b200_settle_all if return_all else lib.glom_b200_settle
     check(fn(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, max_iters,
              float(tol), steps_ptr, ws_ptr, ws_bytes, stream))
+
+
+def settle_queue_workspace_bytes(cfg, slots, max_iters):
+    return _bytes("glom_b200_settle_queue_workspace_bytes", ctypes.byref(cfg), slots, max_iters)
+
+
+def settle_queue_begin(cfg, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, steps_ptr, images, slots, max_iters, tol,
+                       ws_ptr, ws_bytes, stream):
+    """glom_b200_settle_queue_begin: every slot empty, all `images` queued (enqueued on `stream`)."""
+    check(load().glom_b200_settle_queue_begin(ctypes.byref(cfg), tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr,
+                                              steps_ptr, images, slots, max_iters, float(tol), ws_ptr, ws_bytes, stream))
+
+
+def settle_queue_run(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, steps_ptr, images, slots,
+                     max_iters, tol, ws_ptr, ws_bytes, stream, first_step, num_steps, remaining_ptr):
+    """glom_b200_settle_queue_run: global steps first_step .. first_step + num_steps - 1, then the unfinished count into
+    remaining_ptr (device int32); num_steps = 0 enqueues the final hand-over only."""
+    check(load().glom_b200_settle_queue_run(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr,
+                                            out_ptr, steps_ptr, images, slots, max_iters, float(tol), ws_ptr, ws_bytes,
+                                            stream, first_step, num_steps, remaining_ptr))
 
 
 def forward_steps(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, steps_ptr, max_steps,

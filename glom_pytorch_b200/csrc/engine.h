@@ -86,6 +86,31 @@ struct SettleLayout {
 };
 SettleLayout settle_layout(const Geometry& g, int max_iters, int return_all = 0);
 
+// Glom.settle_queue (bf16 engine): B = slots.  The settle workspace for (slots, max_iters), whose fp32 slab is slab 0 of
+// the two private slabs that hold S_t of the slots (slab t & 1), followed by slab 1 and the per-slot queue state
+struct QueueLayout {
+  SettleLayout settle;
+  size_t slab_off[2];      // (B, n, L, d) f32 each
+  size_t queue_off;        // initialised by glom_b200_settle_queue_begin:
+  size_t slot_img_off;     //   [B] int   image in the slot, -1: none
+  size_t age_off;          //   [B] int   steps the slot's image has run
+  size_t pending_off;      //   [B] int   1: the image stopped; its final state waits in the slab for the next fill
+  size_t gather_off;       //   [B] int   this step's fill hands the slot's final state to this image, -1: none
+  size_t fresh_off;        //   [B] int   1: the slot admitted an image at this step
+  size_t block_fresh_off;  //   [ceil(rows/256)] int   1: the block holds a slot admitted at this step
+  size_t head_off;         //   [1] int   next queued image
+  size_t unfinished_off;   //   [1] int   images queued or in flight
+  size_t queue_bytes;
+  size_t total;
+};
+QueueLayout queue_layout(const Geometry& g, int max_iters);
+
+// device pointers into the queue state (QueueLayout), images = N; all NULL for Glom.settle
+struct QueueSlots {
+  int *slot_img, *age, *pending, *gather_img, *fresh, *block_fresh, *head, *unfinished;
+  int images, max_iters;
+};
+
 // ---- launchers (return cudaError_t of the launch; all asynchronous on `st`) -----------------
 struct Bf16Buffers {
   const float* s32_in;  float* s32_out;              // fp32 master state of step t / t+1
@@ -102,6 +127,9 @@ struct Bf16Buffers {
   const int* frozen;                                  // [B] 1: the image has stopped
   const int* block_frozen;                            // [ceil(rows / 256)] 1: all rows of the block belong to stopped images
   float* dsq_out;                                     // (rows, L, nparts) squared-change partials |S_{t+1} - S_t|^2
+  // Glom.settle_queue only (NULL otherwise): [ceil(rows / 256)] 1 = the block holds a slot admitted at this step; K1 then
+  // runs MLP group 0 at every step, for these blocks only
+  const int* block_fresh;
 };
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -122,9 +150,24 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTil
 
 // Glom.settle (settle_kernels.cu): the stopping rule after step `step` (one launch), and the copy of the stopped images
 // whose final state is in the workspace slab into state_out (after the last step)
+// settle queue (q != NULL): the rule is applied per running slot, which stops when it holds or its image has run
+// q->max_iters steps; steps[image] = the image's step count
 cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
                                    int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, cudaStream_t st,
-                                   int* launches);
+                                   int* launches, const QueueSlots* q = nullptr);
+// Glom.settle_queue (settle_kernels.cu).  init: the queue state of a new call (every slot empty, N images queued).
+// schedule, before step t: each finished or empty slot, in slot order, hands its stopped image over to the fill and,
+// when `admit` and the queue is not empty, takes the next queued image; writes frozen / block_frozen / block_fresh.
+// fill, after the schedule: the handed-over images' final states from slab (S_t of the slots) into state_out, then S_0
+// of each admitted image into slab, its bf16 shadows sb / sp and norm partials nsq, and its bf16 token rows xb.
+cudaError_t launch_queue_init(const Geometry& g, const QueueSlots& q, int* frozen, int* block_frozen, unsigned int* done,
+                              cudaStream_t st, int* launches, Profiler* prof);
+cudaError_t launch_queue_schedule(const Geometry& g, const QueueSlots& q, int admit, int* frozen, int* block_frozen,
+                                  cudaStream_t st, int* launches, Profiler* prof);
+cudaError_t launch_queue_fill(const Geometry& g, const QueueSlots& q, const float* tokens, const float* pos,
+                              const float* state_in, const float* init_levels, float* state_out, float* slab,
+                              __nv_bfloat16* sb, __nv_bfloat16* sp, float* nsq, __nv_bfloat16* xb, cudaStream_t st,
+                              int* launches, Profiler* prof);
 // s0 (nullable): where S_0 is when no step materialised it (the carried state, or init_levels broadcast if s0_bcast);
 // images with steps[b] == 0 are copied from there
 cudaError_t launch_settle_gather(const Geometry& g, int max_iters, const int32_t* steps, const float* slab, float* state_out,

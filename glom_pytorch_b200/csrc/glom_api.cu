@@ -79,6 +79,27 @@ SettleLayout settle_layout(const Geometry& g, int max_iters, int return_all) {
   return s;
 }
 
+QueueLayout queue_layout(const Geometry& g, int max_iters) {
+  QueueLayout q{};
+  q.settle = settle_layout(g, max_iters, 0);
+  size_t off = q.settle.total;
+  q.slab_off[0] = q.settle.fwd.s32_off;
+  q.slab_off[1] = off; off = align_up(off + q.settle.fwd.s32_bytes, 1024);
+  const size_t slots = align_up((size_t)g.B * 4, 16), blocks = align_up((size_t)(g.rows + 255) / 256 * 4, 16);
+  q.queue_off = off;
+  q.slot_img_off = off; off += slots;
+  q.age_off = off; off += slots;
+  q.pending_off = off; off += slots;
+  q.gather_off = off; off += slots;
+  q.fresh_off = off; off += slots;
+  q.block_fresh_off = off; off += blocks;
+  q.head_off = off; off += 16;
+  q.unfinished_off = off; off += 16;
+  q.queue_bytes = off - q.queue_off;
+  q.total = align_up(off, 1024);
+  return q;
+}
+
 static int check_cfg(const glom_b200_cfg* cfg) {
   if (!cfg) return fail(GLOM_B200_ERR_INVALID, "cfg is NULL");
   if (cfg->struct_size != sizeof(glom_b200_cfg))
@@ -319,6 +340,139 @@ GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void*
   return r;
 }
 
+// glom_b200_settle_queue_*: the arguments shared by _begin and _run, checked in the same order as settle's
+struct QueueArgs {
+  const glom_b200_cfg* cfg; const float *tokens, *pos, *state_in, *init_levels; float* state_out; int32_t* steps_out;
+  int images, slots, max_iters; float tol; void* workspace; size_t workspace_bytes; void* stream;
+};
+
+static int check_queue_sizes(const glom_b200_cfg* cfg, int images, int slots, int max_iters) {
+  if (int r = check_cfg(cfg)) return r;
+  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "settle_queue: bf16 engine only (precision fp32 given)");
+  if (images < 1) return fail(GLOM_B200_ERR_INVALID, "settle_queue: images must be >= 1 (got %d)", images);
+  if (slots < 1) return fail(GLOM_B200_ERR_INVALID, "settle_queue: slots must be >= 1 (got %d)", slots);
+  if (max_iters < 1) return fail(GLOM_B200_ERR_INVALID, "settle_queue: max_iters must be >= 1 (got %d)", max_iters);
+  return 0;
+}
+
+// -> 0 and the geometry / layout of the slots, after every argument check and the device query
+static int check_queue(const QueueArgs& a, Geometry* g, QueueLayout* ql, DeviceInfo* di) {
+  if (int r = check_queue_sizes(a.cfg, a.images, a.slots, a.max_iters)) return r;
+  if (a.tol != a.tol) return fail(GLOM_B200_ERR_INVALID, "settle_queue: tol is NaN");
+  if (int r = check_steps_ptr("settle_queue", "steps_out", a.steps_out)) return r;
+  if (!a.tokens || !a.pos || !a.state_out) return fail(GLOM_B200_ERR_INVALID, "settle_queue: a required pointer is NULL");
+  if (!a.state_in && !a.init_levels) return fail(GLOM_B200_ERR_INVALID, "settle_queue: need state_in or init_levels");
+  if (a.state_in == a.state_out) return fail(GLOM_B200_ERR_INVALID, "settle_queue: state_out must not alias state_in");
+  if (reinterpret_cast<uintptr_t>(a.workspace) % 1024) return fail(GLOM_B200_ERR_INVALID, "settle_queue: workspace must be 1024-byte aligned");
+  if (reinterpret_cast<uintptr_t>(a.tokens) % 16 || reinterpret_cast<uintptr_t>(a.pos) % 16 ||
+      reinterpret_cast<uintptr_t>(a.state_out) % 16 || reinterpret_cast<uintptr_t>(a.state_in) % 16 ||
+      reinterpret_cast<uintptr_t>(a.init_levels) % 16)
+    return fail(GLOM_B200_ERR_INVALID, "settle_queue: tensor pointers must be 16-byte aligned");
+  *g = make_geometry(a.cfg, a.slots);
+  *ql = queue_layout(*g, a.max_iters);
+  if (!a.workspace || a.workspace_bytes < ql->total)
+    return fail(GLOM_B200_ERR_WORKSPACE, "settle_queue workspace: need %zu bytes, got %zu", ql->total, a.workspace_bytes);
+  return device_info(di);
+}
+
+static QueueSlots queue_slots(const QueueArgs& a, const QueueLayout& ql) {
+  char* ws = static_cast<char*>(a.workspace);
+  QueueSlots q{};
+  q.slot_img = reinterpret_cast<int*>(ws + ql.slot_img_off);
+  q.age = reinterpret_cast<int*>(ws + ql.age_off);
+  q.pending = reinterpret_cast<int*>(ws + ql.pending_off);
+  q.gather_img = reinterpret_cast<int*>(ws + ql.gather_off);
+  q.fresh = reinterpret_cast<int*>(ws + ql.fresh_off);
+  q.block_fresh = reinterpret_cast<int*>(ws + ql.block_fresh_off);
+  q.head = reinterpret_cast<int*>(ws + ql.head_off);
+  q.unfinished = reinterpret_cast<int*>(ws + ql.unfinished_off);
+  q.images = a.images;
+  q.max_iters = a.max_iters;
+  return q;
+}
+
+static int queue_begin(const QueueArgs& a) {
+  Geometry g{}; QueueLayout ql{}; DeviceInfo di{};
+  if (int r = check_queue(a, &g, &ql, &di)) return r;
+  char* ws = static_cast<char*>(a.workspace);
+  g_launches = 0;
+  const cudaError_t e = launch_queue_init(g, queue_slots(a, ql), reinterpret_cast<int*>(ws + ql.settle.frozen_off),
+                                          reinterpret_cast<int*>(ws + ql.settle.block_frozen_off),
+                                          reinterpret_cast<unsigned int*>(ws + ql.settle.done_off),
+                                          static_cast<cudaStream_t>(a.stream), &g_launches, &g_prof);
+  if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle_queue init launch: %s", cudaGetErrorString(e));
+  g_err[0] = 0;
+  return 0;
+}
+
+// Global steps first_step .. first_step + num_steps - 1: schedule, fill, K1, K3, K2, convergence each.  num_steps == 0:
+// the schedule and fill of step first_step without admissions, i.e. the hand-over of the images that stopped last.
+static int queue_run(const QueueArgs& a, const void* packed_weights, int first_step, int num_steps, int32_t* remaining_out) {
+  Geometry g{}; QueueLayout ql{}; DeviceInfo di{};
+  if (int r = check_queue_sizes(a.cfg, a.images, a.slots, a.max_iters)) return r;
+  if (!packed_weights || reinterpret_cast<uintptr_t>(packed_weights) % 1024)
+    return fail(GLOM_B200_ERR_INVALID, "settle_queue: packed weights NULL or not 1024-byte aligned");
+  if (first_step < 0 || num_steps < 0)
+    return fail(GLOM_B200_ERR_INVALID, "settle_queue: first_step and num_steps must be >= 0 (got %d, %d)", first_step, num_steps);
+  if (reinterpret_cast<uintptr_t>(remaining_out) % 4)
+    return fail(GLOM_B200_ERR_INVALID, "settle_queue: remaining_out must be 4-byte aligned");
+  if (int r = check_queue(a, &g, &ql, &di)) return r;
+  const WorkspaceLayout& wl = ql.settle.fwd;
+  const PackedLayout pl = packed_layout(g.d, g.L, GLOM_B200_BF16);
+  const char* pw = static_cast<const char*>(packed_weights);
+  char* ws = static_cast<char*>(a.workspace);
+  cudaStream_t st = static_cast<cudaStream_t>(a.stream);
+  const QueueSlots q = queue_slots(a, ql);
+  float* slab[2] = {reinterpret_cast<float*>(ws + ql.slab_off[0]), reinterpret_cast<float*>(ws + ql.slab_off[1])};
+  __nv_bfloat16* sb[2] = {reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off[0]), reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off[1])};
+  __nv_bfloat16* sp[2] = {reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off[0]), reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off[1])};
+  float* nsq[2] = {reinterpret_cast<float*>(ws + wl.nsq_off[0]), reinterpret_cast<float*>(ws + wl.nsq_off[1])};
+  __nv_bfloat16* xb = reinterpret_cast<__nv_bfloat16*>(ws + wl.xb_off);
+  int* frozen = reinterpret_cast<int*>(ws + ql.settle.frozen_off);
+  int* block_frozen = reinterpret_cast<int*>(ws + ql.settle.block_frozen_off);
+  float* dsq = reinterpret_cast<float*>(ws + ql.settle.dsq_off);
+  g_launches = 0;
+  const int last = first_step + (num_steps > 0 ? num_steps : 1);
+  for (int t = first_step; t < last; ++t) {
+    const int p = t & 1;
+    cudaError_t e = launch_queue_schedule(g, q, num_steps > 0, frozen, block_frozen, st, &g_launches, &g_prof);
+    if (e == cudaSuccess)
+      e = launch_queue_fill(g, q, a.tokens, a.pos, a.state_in, a.init_levels, a.state_out, slab[p], sb[p], sp[p], nsq[p], xb, st,
+                            &g_launches, &g_prof);
+    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle_queue slot launch before step %d: %s", t, cudaGetErrorString(e));
+    if (num_steps == 0) break;
+    Bf16Buffers b{};
+    b.s32_in = slab[p]; b.s32_out = slab[p ^ 1]; b.s32_in_bcast = 0;
+    b.sb_in = sb[p]; b.sb_out = sb[p ^ 1];
+    b.sp_in = sp[p]; b.sp_out = sp[p ^ 1];
+    b.xb = xb;
+    b.h = reinterpret_cast<__nv_bfloat16*>(ws + wl.h_off);
+    b.attn_acc = wl.attn_acc_bytes ? reinterpret_cast<float*>(ws + wl.attn_acc_off) : nullptr;
+    b.c = reinterpret_cast<__nv_bfloat16*>(ws + wl.c_off);
+    b.nsq_in = nsq[p]; b.nsq_out = nsq[p ^ 1];
+    b.pos = a.pos;
+    b.w1 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w1_off);
+    b.w2 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w2_off);
+    b.b1 = reinterpret_cast<const float*>(pw + pl.b1_off);
+    b.b2 = reinterpret_cast<const float*>(pw + pl.b2_off);
+    b.frozen = frozen; b.block_frozen = block_frozen; b.dsq_out = dsq; b.block_fresh = q.block_fresh;
+    char msg[400] = "";
+    const int r = step_bf16(g, b, t, g_encode, di.sms, st, &g_launches, msg, sizeof(msg), &g_prof);
+    if (r) return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "settle_queue step %d: %s", t, msg);
+    e = launch_settle_converge(g, t + 1, a.tol, dsq, b.nsq_out, frozen, block_frozen,
+                               reinterpret_cast<unsigned int*>(ws + ql.settle.done_off),
+                               reinterpret_cast<float*>(ws + ql.settle.level_q_off), a.steps_out, st, &g_launches, &q);
+    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle_queue convergence launch after step %d: %s", t, cudaGetErrorString(e));
+  }
+  if (remaining_out) {
+    const cudaError_t e = cudaMemcpyAsync(remaining_out, q.unfinished, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle_queue count copy: %s", cudaGetErrorString(e));
+    ++g_launches;
+  }
+  g_err[0] = 0;
+  return 0;
+}
+
 static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                         const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
                         int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity,
@@ -453,6 +607,31 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
   }
   g_err[0] = 0;
   return 0;
+}
+
+// Glom.settle_queue: N images through `slots` batch slots, see include/glom_b200.h
+GLOM_B200_API int glom_b200_settle_queue_workspace_bytes(const glom_b200_cfg* cfg, int slots, int max_iters, size_t* out_bytes) {
+  if (int r = check_queue_sizes(cfg, 1, slots, max_iters)) return r;
+  if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
+  *out_bytes = queue_layout(make_geometry(cfg, slots), max_iters).total;
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_settle_queue_begin(const glom_b200_cfg* cfg, const float* tokens, const float* pos,
+                                               const float* state_in, const float* init_levels, float* state_out,
+                                               int32_t* steps_out, int images, int slots, int max_iters, float tol,
+                                               void* workspace, size_t workspace_bytes, void* stream) {
+  return queue_begin({cfg, tokens, pos, state_in, init_levels, state_out, steps_out, images, slots, max_iters, tol, workspace,
+                      workspace_bytes, stream});
+}
+
+GLOM_B200_API int glom_b200_settle_queue_run(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
+                                             const float* pos, const float* state_in, const float* init_levels,
+                                             float* state_out, int32_t* steps_out, int images, int slots, int max_iters,
+                                             float tol, void* workspace, size_t workspace_bytes, void* stream, int first_step,
+                                             int num_steps, int32_t* remaining_out) {
+  return queue_run({cfg, tokens, pos, state_in, init_levels, state_out, steps_out, images, slots, max_iters, tol, workspace,
+                    workspace_bytes, stream}, packed_weights, first_step, num_steps, remaining_out);
 }
 
 static int tok_kp(int patch) { return (3 * patch * patch + 63) / 64 * 64; }

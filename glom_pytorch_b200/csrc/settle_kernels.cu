@@ -1,7 +1,9 @@
 // Glom.settle on CUDA cores: the per-image stopping rule applied after every step, and the final gather of the images
 // whose last state sits in the workspace's half of the ping-pong.  Also the per-image step counts of
 // glom_b200_forward_steps: the flags of each step from the given counts, and the return_all fill of stopped images' slabs.
+// And Glom.settle_queue's slot kernels: queue initialisation, the slot schedule and the slot fill of every step.
 #include "engine.h"
+#include "prep_state.cuh"
 #include "ptx.cuh"
 
 #include <math.h>
@@ -18,10 +20,13 @@ constexpr int SETTLE_THREADS = 256;
 // as 0, x/0 (x > 0) as inf.  The block that finishes last applies the rule, max_l q_bl <= tol, i.e. q_bl <= tol for
 // every level (a NaN never stops an image): steps[b] = step for every running image, frozen[b] = 1 for those that stop
 // (so an image that never stops ends with steps[b] = max_iters), and recomputes the per-256-row-block flags.
+// Settle queue (q.slot_img != NULL): b is a slot.  Each running slot's age goes up by one, the slot also stops when its
+// age reaches q.max_iters, steps[q.slot_img[b]] = age, and a stopping slot is marked pending (its final state is
+// handed over by the next fill) and leaves the unfinished count.
 __global__ void __launch_bounds__(SETTLE_THREADS)
 settle_converge_kernel(int n, int L, int nparts, int B, int rows, int step, float tol, const float* __restrict__ dsq,
                        const float* __restrict__ nsq, int* frozen, int* block_frozen, unsigned int* done, float* level_q,
-                       int32_t* steps) {
+                       int32_t* steps, QueueSlots q) {
   pdl_launch_dependents();
   pdl_wait();                                       // the partials of this step are complete and visible
   const int l = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -60,7 +65,14 @@ settle_converge_kernel(int n, int L, int nparts, int B, int rows, int step, floa
     if (frozen[bb]) continue;
     bool stop = true;
     for (int ll = 0; ll < L; ++ll) stop = stop && __ldcg(level_q + (size_t)bb * L + ll) <= tol;
-    steps[bb] = step;
+    if (q.slot_img) {
+      const int age = ++q.age[bb];
+      stop = stop || age >= q.max_iters;
+      steps[q.slot_img[bb]] = age;
+      if (stop) { q.pending[bb] = 1; atomicSub(q.unfinished, 1); }
+    } else {
+      steps[bb] = step;
+    }
     if (stop) frozen[bb] = 1;
   }
   __syncthreads();
@@ -76,7 +88,7 @@ settle_converge_kernel(int n, int L, int nparts, int B, int rows, int step, floa
 
 cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
                                    int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, cudaStream_t st,
-                                   int* launches) {
+                                   int* launches, const QueueSlots* q) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(g.L, g.B);
   cfg.blockDim = dim3(SETTLE_THREADS);
@@ -87,7 +99,7 @@ cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const
   cfg.attrs = attr; cfg.numAttrs = 1;
   if (launches) ++*launches;
   return cudaLaunchKernelEx(&cfg, settle_converge_kernel, g.n, g.L, g.nparts, g.B, g.rows, step, tol, dsq, nsq, frozen,
-                            block_frozen, done, level_q, steps);
+                            block_frozen, done, level_q, steps, q ? *q : QueueSlots{});
 }
 
 __device__ __forceinline__ int clamp_steps(int s, int max_steps) { return min(max(s, 0), max_steps); }
@@ -184,6 +196,143 @@ cudaError_t launch_steps_fill(const Geometry& g, int max_steps, const int32_t* s
                                                                          reinterpret_cast<float4*>(states));
   if (launches) ++*launches;
   return cudaGetLastError();
+}
+
+// ---- Glom.settle_queue: N images through B slots.  Slot s holds image slot_img[s]; its rows are rows s*n .. s*n+n-1
+// of every step buffer, exactly as image s's rows in a settle call of batch B.  S_t of the slots lives in the private
+// slab t & 1, the shadows and norm partials in buffer t & 1, as in settle.  A slot whose image stops after step t-1 hands
+// that image's final state (slab t & 1) to state_out in the fill of step t, which then writes the next image's S_0 over
+// it; K1 recomputes group 0 for the blocks that admitted an image (block_fresh), K3 and K2 skip frozen slots as in settle.
+
+template <typename... Params, typename... Args>
+static cudaError_t launch_pdl(void (*kernel)(Params...), dim3 grid, cudaStream_t st, Args... args) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid;
+  cfg.blockDim = dim3(SETTLE_THREADS);
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernels
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kernel, args...);
+}
+
+// One block: every slot empty (frozen, no image), every image queued.
+__global__ void __launch_bounds__(SETTLE_THREADS)
+queue_init_kernel(int B, int nblk, QueueSlots q, int* frozen, int* block_frozen, unsigned int* done) {
+  pdl_launch_dependents();
+  pdl_wait();                                       // the previous call's kernels have stopped reading the workspace
+  for (int s = threadIdx.x; s < B; s += SETTLE_THREADS) {
+    q.slot_img[s] = -1; q.age[s] = 0; q.pending[s] = 0; q.gather_img[s] = -1; q.fresh[s] = 0;
+    frozen[s] = 1;
+  }
+  for (int m = threadIdx.x; m < nblk; m += SETTLE_THREADS) { block_frozen[m] = 1; q.block_fresh[m] = 0; }
+  if (threadIdx.x == 0) { *q.head = 0; *q.unfinished = q.images; *done = 0u; }
+}
+
+cudaError_t launch_queue_init(const Geometry& g, const QueueSlots& q, int* frozen, int* block_frozen, unsigned int* done,
+                              cudaStream_t st, int* launches, Profiler* prof) {
+  ProfScope scope(prof, PROF_PREP, st);
+  if (launches) ++*launches;
+  return launch_pdl(queue_init_kernel, dim3(1), st, g.B, (g.rows + 255) / 256, q, frozen, block_frozen, done);
+}
+
+// One block, before a step.  The open slots (frozen: their image stopped, or empty) are ranked in slot order by a
+// block-wide count; open slot number k takes queued image head + k while there is one (and `admit`), so the assignment
+// does not depend on timing.  An open slot with a pending image hands it over to the fill (gather_img).  Then the
+// per-256-row-block flags: block_frozen = every slot of the block is frozen, block_fresh = one of them took an image.
+__global__ void __launch_bounds__(SETTLE_THREADS)
+queue_schedule_kernel(int n, int B, int rows, int admit, QueueSlots q, int* frozen, int* block_frozen) {
+  pdl_launch_dependents();
+  pdl_wait();                                       // the previous step's convergence launch has set the flags
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  __shared__ int wsum[SETTLE_THREADS / 32];
+  int head = *q.head;
+  for (int base = 0; base < B; base += SETTLE_THREADS) {
+    const int s = base + tid;
+    const bool open = s < B && frozen[s];
+    const unsigned m = __ballot_sync(0xffffffffu, open);
+    if (lane == 0) wsum[warp] = __popc(m);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int w = 0; w < SETTLE_THREADS / 32; ++w) { before += w < warp ? wsum[w] : 0; total += wsum[w]; }
+    if (open) {
+      q.gather_img[s] = q.pending[s] ? q.slot_img[s] : -1;
+      q.pending[s] = 0;
+      const int img = head + before + __popc(m & ((1u << lane) - 1u));
+      const bool take = admit && img < q.images;
+      q.slot_img[s] = take ? img : -1;
+      q.fresh[s] = take;
+      if (take) { q.age[s] = 0; frozen[s] = 0; }
+    } else if (s < B) {
+      q.gather_img[s] = -1;
+      q.fresh[s] = 0;
+    }
+    if (admit) head = min(head + total, q.images);
+    __syncthreads();                                // wsum is reused
+  }
+  if (tid == 0) *q.head = head;
+  const int nblk = (rows + 255) / 256;
+  for (int m = tid; m < nblk; m += SETTLE_THREADS) {
+    const int b0 = m * 256 / n, b1 = (min(rows, m * 256 + 256) - 1) / n;
+    int all = 1, any = 0;
+    for (int bb = b0; bb <= b1; ++bb) { all = all && frozen[bb]; any = any || q.fresh[bb]; }
+    block_frozen[m] = all;
+    q.block_fresh[m] = any;
+  }
+}
+
+cudaError_t launch_queue_schedule(const Geometry& g, const QueueSlots& q, int admit, int* frozen, int* block_frozen,
+                                  cudaStream_t st, int* launches, Profiler* prof) {
+  ProfScope scope(prof, PROF_PREP, st);
+  if (launches) ++*launches;
+  return launch_pdl(queue_schedule_kernel, dim3(1), st, g.n, g.B, g.rows, admit, q, frozen, block_frozen);
+}
+
+constexpr int FILL_ROWS = 8;                        // rows of one slot per block of the fill
+
+// Grid (ceil(n / FILL_ROWS), B), after the schedule.  Block (c, s) covers rows c*FILL_ROWS.. of slot s: first the copy
+// of the handed-over image's final state from the slab into state_out, then (admitted slot) the admitted image's S_0
+// into the same slab rows with prep_state_row, one warp per (row, level), and its token rows cast to bf16.
+__global__ void __launch_bounds__(SETTLE_THREADS)
+queue_fill_kernel(int n, int L, int d, int nparts, int part_w, QueueSlots q, const float* __restrict__ tokens,
+                  const float* __restrict__ pos, const float* __restrict__ state_in, const float* __restrict__ init_levels,
+                  float* __restrict__ state_out, float* slab, __nv_bfloat16* __restrict__ sb, __nv_bfloat16* __restrict__ sp,
+                  float* __restrict__ nsq, __nv_bfloat16* __restrict__ xb) {
+  pdl_launch_dependents();
+  pdl_wait();                                       // the schedule is written, the previous step's K2 has stored S_t
+  const int s = blockIdx.y, i0 = blockIdx.x * FILL_ROWS, ni = min(FILL_ROWS, n - i0);
+  const int gi = q.gather_img[s], fresh = q.fresh[s];
+  const size_t ld = (size_t)L * d, r0 = (size_t)s * n + i0;
+  if (gi >= 0) {
+    const float4* src = reinterpret_cast<const float4*>(slab + r0 * ld);
+    float4* dst = reinterpret_cast<float4*>(state_out + ((size_t)gi * n + i0) * ld);
+    for (size_t k = threadIdx.x; k < (size_t)ni * ld / 4; k += SETTLE_THREADS) dst[k] = src[k];
+  }
+  if (!fresh) return;                               // block-uniform
+  __syncthreads();                                  // the handed-over state is read before S_0 replaces it
+  const int img = q.slot_img[s];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int w = warp; w < ni * L; w += SETTLE_THREADS / 32) {
+    const int i = i0 + w / L, l = w % L;
+    const size_t r = (size_t)s * n + i;
+    const float* src = state_in ? state_in + (((size_t)img * n + i) * L + l) * d : init_levels + (size_t)l * d;
+    prep_state_row(lane, l, d, nparts, part_w, src, pos + (size_t)i * d, slab + (r * L + l) * d, sb + (r * L + l) * d,
+                   l >= 1 ? sp + (r * (L - 1) + (l - 1)) * d : nullptr, nsq + (r * L + l) * nparts);
+  }
+  const float4* tk = reinterpret_cast<const float4*>(tokens + ((size_t)img * n + i0) * d);
+  uint2* xo = reinterpret_cast<uint2*>(xb + r0 * d);
+  for (int k = threadIdx.x; k < ni * d / 4; k += SETTLE_THREADS) xo[k] = cast4_bf16(tk[k]);
+}
+
+cudaError_t launch_queue_fill(const Geometry& g, const QueueSlots& q, const float* tokens, const float* pos,
+                              const float* state_in, const float* init_levels, float* state_out, float* slab,
+                              __nv_bfloat16* sb, __nv_bfloat16* sp, float* nsq, __nv_bfloat16* xb, cudaStream_t st,
+                              int* launches, Profiler* prof) {
+  ProfScope scope(prof, PROF_PREP, st);
+  if (launches) ++*launches;
+  return launch_pdl(queue_fill_kernel, dim3((g.n + FILL_ROWS - 1) / FILL_ROWS, g.B), st, g.n, g.L, g.d, g.nparts, g.part_w,
+                    q, tokens, pos, state_in, init_levels, state_out, slab, sb, sp, nsq, xb);
 }
 
 }  // namespace glom

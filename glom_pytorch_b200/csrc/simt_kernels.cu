@@ -5,6 +5,7 @@
 // Reference semantics (glom_pytorch/glom_pytorch.py): GroupedFeedForward :23-36,
 // ConsensusAttention :56-73, combine :128-129/:141-142, image_to_tokens :94-97.
 #include "engine.h"
+#include "prep_state.cuh"
 #include "ptx.cuh"
 
 namespace glom {
@@ -90,51 +91,14 @@ __global__ void prep_state_kernel(int rows, int n, int L, int d, int nparts, int
   if (warp >= rows * L) return;
   const int r = warp / L, l = warp % L;
   const float* src = state_in ? state_in + ((size_t)r * L + l) * d : init_levels + (size_t)l * d;
-  const float* p = pos + (size_t)(r % n) * d;
-  for (int c = lane * 4; c < d; c += 128) {
-    const float4 v = *reinterpret_cast<const float4*>(src + c);
-    const size_t o = ((size_t)r * L + l) * d + c;
-    if (s32_dst) *reinterpret_cast<float4*>(s32_dst + o) = v;
-    uint2 pk;
-    pk.x = pack_bf16x2(v.x, v.y);
-    pk.y = pack_bf16x2(v.z, v.w);
-    *reinterpret_cast<uint2*>(sb + o) = pk;
-    if (l >= 1) {
-      const float4 q = *reinterpret_cast<const float4*>(p + c);
-      uint2 pq;
-      pq.x = pack_bf16x2(v.x + q.x, v.y + q.y);
-      pq.y = pack_bf16x2(v.z + q.z, v.w + q.w);
-      *reinterpret_cast<uint2*>(sp + ((size_t)r * (L - 1) + (l - 1)) * d + c) = pq;
-    }
-  }
-  // squared-norm partials in exactly the order the GEMM2 epilogue accumulates them (row_chunk_sumsq in
-  // tc_kernels.cu), so a carried-in state continues bit-identically (:123).
-  // (per 32-column chunk: 8 four-column fmaf chains, pairwise tree; chunks added in order)
-  for (int part = 0; part < nparts; ++part) {
-    float ss = 0.f;
-    for (int c0 = 0; c0 < part_w; c0 += 32) {
-      const float4 v = *reinterpret_cast<const float4*>(src + part * part_w + c0 + (lane & 7) * 4);
-      float q = v.x * v.x;
-      q = fmaf(v.y, v.y, q);
-      q = fmaf(v.z, v.z, q);
-      q = fmaf(v.w, v.w, q);
-      q += __shfl_xor_sync(0xffffffffu, q, 1);
-      q += __shfl_xor_sync(0xffffffffu, q, 2);
-      q += __shfl_xor_sync(0xffffffffu, q, 4);
-      ss += q;
-    }
-    if (lane == 0) nsq[((size_t)r * L + l) * nparts + part] = ss;
-  }
+  const size_t o = ((size_t)r * L + l) * d;
+  prep_state_row(lane, l, d, nparts, part_w, src, pos + (size_t)(r % n) * d, s32_dst ? s32_dst + o : nullptr, sb + o,
+                 l >= 1 ? sp + ((size_t)r * (L - 1) + (l - 1)) * d : nullptr, nsq + ((size_t)r * L + l) * nparts);
 }
 
 __global__ void cast_bf16_kernel(size_t n4, const float* __restrict__ src, __nv_bfloat16* __restrict__ dst) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    const float4 v = reinterpret_cast<const float4*>(src)[i];
-    uint2 pk;
-    pk.x = pack_bf16x2(v.x, v.y);
-    pk.y = pack_bf16x2(v.z, v.w);
-    reinterpret_cast<uint2*>(dst)[i] = pk;
-  }
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x)
+    reinterpret_cast<uint2*>(dst)[i] = cast4_bf16(reinterpret_cast<const float4*>(src)[i]);
 }
 
 cudaError_t launch_prep(const Geometry& g, const float* state_in, const float* init_levels, const float* pos,

@@ -69,6 +69,9 @@ struct GemmParams {
   const int* frozen;        // [B] 1: the image has stopped
   const int* block_frozen;  // [num_m] 1: every row of the 256-row block belongs to a stopped image
   float* dsq_out;           // K2: squared-change partials |S_{t+1} - S_t|^2, laid out like nsq_out
+  // K1 of the settle queue (NULL otherwise): [num_m] 1 = the 256-row block holds a slot admitted at this step.  The
+  // launch covers group 0 (z0 = 0) at every step, and only the blocks marked here run its tiles
+  const int* block_fresh;
 };
 
 template <int MODE, int BN>
@@ -161,6 +164,14 @@ __device__ __forceinline__ void tok_chunk(const uint32_t (&v)[32], const float4 
 // SETTLE (K1 / K2 of Glom.settle): tiles of 256-row blocks whose images have all stopped are skipped by every warp role
 // of both CTAs (the same flag, written by an earlier launch and read after pdl_wait, keeps the multicast and empty-barrier
 // protocol in step); K2 stores nothing for rows of stopped images and also writes the squared-change partials.
+// K1 of the settle queue also skips the group-0 tiles of blocks that admitted no image at this step: their group-0
+// hidden activations (tokens only) are still in H from the step that admitted the block's images.
+template <int MODE>
+__device__ __forceinline__ bool settle_skip(const GemmParams& p, const TileInfo& t) {
+  if (p.block_frozen[t.m_blk]) return true;
+  return MODE == 0 && t.z == 0 && p.block_fresh != nullptr && !p.block_fresh[t.m_blk];
+}
+
 template <int MODE, int BN, bool CNT, bool SETTLE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows, d)        K2: H (rows, G*4d)
@@ -224,7 +235,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
       const int blk_skip = (p.m128 - 1) * kbg_n;
       for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
         const TileInfo t = decode_tile<MODE>(p, tile);
-        if constexpr (SETTLE) { if (p.block_frozen[t.m_blk]) continue; }
+        if constexpr (SETTLE) { if (settle_skip<MODE>(p, t)) continue; }
         const CUtensorMap* amap;
         int a_col, b_row;
         if (MODE == 0) {
@@ -293,7 +304,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
     float acc[BN / 2];
     for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
       const TileInfo t = decode_tile<MODE>(p, tile);
-      if constexpr (SETTLE) { if (p.block_frozen[t.m_blk]) continue; }
+      if constexpr (SETTLE) { if (settle_skip<MODE>(p, t)) continue; }
       const int row0 = t.m_blk * 256 + cta_rank * BM + pair * 32;     // first row of this warp pair's 32-row band
       const int rows_left = p.rows - row0;                              // >= 32: whole band valid (warp-uniform)
       uint32_t live = ~0u;                                              // SETTLE, K2: bit r = row row0 + r is stored
@@ -1147,10 +1158,12 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTil
     // of H is written by the call's first step and stays valid; the later steps run the other 2L - 2 groups only.
     // The groups are walked upward from z0, and every H box is stored evict-first: H streams through L2 and must not
     // displace the weights and state shadows that the GEMMs and the consensus kernel re-read
-    p.z0 = (step_index > 0 && g.G > 1) ? 1 : 0;
+    // The settle queue (b.block_fresh) admits images at any step: group 0 is in every launch, and its tiles run only for
+    // the row blocks that admitted an image at this step.
+    p.z0 = (step_index > 0 && g.G > 1 && !b.block_fresh) ? 1 : 0;
     p.num_m = (rows + 255) / 256; p.num_n = 4 * d / 256; p.num_tiles = (g.G - p.z0) * p.num_m * p.num_n;
     p.bias = b.b1; p.m128 = m128;
-    p.frozen = b.frozen; p.block_frozen = b.block_frozen;
+    p.frozen = b.frozen; p.block_frozen = b.block_frozen; p.block_fresh = b.block_fresh;
     ProfScope scope(prof, PROF_GEMM1, st);
     cudaError_t e = launch_gemm<0, 256>(mx, msb, msp, mw1, mh_out, p, num_sms, st);
     if (launches) ++*launches;

@@ -581,3 +581,68 @@ class Glom(nn.Module):
         if tol != tol:
             raise ValueError("tol is NaN")
         return self._column_update(img, levels, needs_grad, max_iters, return_all, tol=tol)
+
+    # ------------------------------------------------------------------ settling a stream of images
+    def settle_queue(self, img, tol, max_iters=None, levels=None, *, slots=32):
+        """Settle N images through ``slots`` batch slots -> ``(levels, steps)``, as ``settle`` returns them for the whole
+        batch.
+
+        Contract: ``levels[i]`` and ``steps[i]`` are bit-identical to ``settle(img, tol, max_iters, levels)`` on the whole
+        N-image batch, and so to ``forward(img, iters=steps[i], levels=same_start)[i]``.  Rows, consensus items and tiles
+        are independent across images, so which slot holds an image, and when, changes no bit.
+
+        The engine keeps ``slots`` images in flight (the batch of each step, clipped to N).  When an image stops, its
+        slot takes the next queued image on the next step, on the GPU, so the throughput follows the mean step count of
+        the images rather than each batch's slowest image.  Arguments, errors and the stopping rule are those of
+        ``settle``: bf16 engine only, inference only, ``max_iters >= 1`` (None = 2L), NaN ``tol`` rejected; no
+        ``return_all`` or ``differentiable``.  ``levels`` (N, n, L, d) or None, result (N, n, L, d) fp32 and ``steps``
+        (N,) int32 on the GPU.
+
+        The tokens of all N images are computed up front by one tokeniser call: N * n * d * 4 bytes (512 MB for 1024
+        images at dim 512 and 256 patches).  The call synchronises once per ``max_iters`` steps to read the number of
+        unfinished images (4 bytes), so it cannot be captured in a CUDA graph."""
+        if self.precision != "bf16":
+            raise RuntimeError("Glom.settle_queue needs precision='bf16' (the fp32 engine has no early stopping)")
+        _require_cuda(img)
+        if self._needs_grad(img, levels):
+            raise RuntimeError("Glom.settle_queue is inference only: call it under torch.no_grad() / torch.inference_mode() "
+                               "or with parameters and inputs that do not require grad")
+        max_iters = self.levels * 2 if max_iters is None else int(max_iters)
+        if max_iters < 1:
+            raise ValueError(f"max_iters must be >= 1, got {max_iters}")
+        tol = float(tol)
+        if tol != tol:
+            raise ValueError("tol is NaN")
+        slots = int(slots)
+        if slots < 1:
+            raise ValueError(f"slots must be >= 1, got {slots}")
+        num, n = self._check_input(img, levels)
+        self._resume = None
+        slots = min(slots, num)
+        tokens = self.tokens(img)                                           # (:114) all N images, one engine call
+        device = tokens.device
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            pos = self.pos_emb.weight[:n].detach().to(torch.float32).contiguous()
+            init = self.init_levels.detach().to(torch.float32).contiguous()
+            state_in = None if levels is None else levels.detach().to(device=device, dtype=torch.float32).contiguous()
+            state_ptr = None if state_in is None else state_in.data_ptr()
+            cfg = self.engine_cfg(n)
+            packed = self._packed_weights(cfg, device, stream)
+            out = torch.empty(num, n, self.levels, self.dim, dtype=torch.float32, device=device)
+            steps = torch.empty(num, dtype=torch.int32, device=device)
+            remaining = torch.empty(1, dtype=torch.int32, device=device)
+            ws = self._get_workspace(_native.settle_queue_workspace_bytes(cfg, slots, max_iters), device)
+            args = (tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(), out.data_ptr(), steps.data_ptr(), num,
+                    slots, max_iters, tol, ws.data_ptr(), ws.numel(), stream)
+            _native.settle_queue_begin(cfg, *args)
+            launches, first = _native.last_launch_count(), 0
+            while True:
+                _native.settle_queue_run(cfg, packed.data_ptr(), *args, first, max_iters, remaining.data_ptr())
+                launches += _native.last_launch_count()
+                first += max_iters
+                if int(remaining.item()) == 0:                              # the only host read
+                    break
+            _native.settle_queue_run(cfg, packed.data_ptr(), *args, first, 0, None)   # the last stopped images' states
+            self.last_launches = launches + _native.last_launch_count() + getattr(self, "_tok_launches", 0)
+        return out, steps

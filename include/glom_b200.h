@@ -165,6 +165,36 @@ GLOM_B200_API int glom_b200_forward_steps(const glom_b200_cfg* cfg, const void* 
                                           int batch, const int32_t* steps, int max_steps, int return_all, void* workspace,
                                           size_t workspace_bytes, void* stream);
 
+/* A queue of images settled through fixed batch slots (Glom.settle_queue).  bf16 engine only.  `images` = N images run
+ * through `slots` = B batch slots: each slot holds one image at a time and, on the step after its image stops, takes the
+ * next queued image (open slots take queued images in slot order, so the assignment is deterministic).  Image i's result
+ * is bit-identical to glom_b200_settle on the whole N-image batch with the same tol and max_iters: state_out[i] = S_k and
+ * steps_out[i] = k, k the first step whose change criterion is <= tol, or max_iters.  The library never synchronises:
+ * the caller loops on the host.
+ *   tokens (N, n, d) fp32 (all images, tokenised up front);  pos (n, d);  state_in (N, n, L, d) or NULL with
+ *   init_levels (L, d) broadcast;  state_out (N, n, L, d) fp32, must not alias state_in;  steps_out (N) int32 device.
+ * _begin initialises the queue state in the workspace (every slot empty, all N images queued).  _run enqueues the global
+ * steps first_step .. first_step + num_steps - 1 (first_step = the number of steps the earlier _run calls of this queue
+ * enqueued), each a slot schedule, a slot fill (the final states of images that stopped at the previous step go to
+ * state_out, S_0 of the admitted images into their slots), the three kernels of a settle step and the stopping rule;
+ * then it copies the number of unfinished images (queued or in a slot) to *remaining_out (device int32, may be NULL).
+ * When that count is 0, a _run with num_steps = 0 enqueues only the final hand-over of the images that stopped at the
+ * last step; after it state_out and steps_out are complete.  A typical loop: begin; do { run(t, max_iters); t += max_iters;
+ * read the count } while (count); run(t, 0).  Every call takes the same arguments.  Argument errors (precision fp32,
+ * images < 1, slots < 1, max_iters < 1, NaN tol, NULL or misaligned steps_out) are reported before any device query.
+ * The workspace (1024-byte aligned) depends on (slots, max_iters) only: the settle workspace of batch `slots`, a second
+ * fp32 state slab and the per-slot queue state; a following glom_b200_forward_resume on it is not valid. */
+GLOM_B200_API int glom_b200_settle_queue_workspace_bytes(const glom_b200_cfg* cfg, int slots, int max_iters, size_t* out_bytes);
+GLOM_B200_API int glom_b200_settle_queue_begin(const glom_b200_cfg* cfg, const float* tokens, const float* pos,
+                                               const float* state_in, const float* init_levels, float* state_out,
+                                               int32_t* steps_out, int images, int slots, int max_iters, float tol,
+                                               void* workspace, size_t workspace_bytes, void* stream);
+GLOM_B200_API int glom_b200_settle_queue_run(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
+                                             const float* pos, const float* state_in, const float* init_levels,
+                                             float* state_out, int32_t* steps_out, int images, int slots, int max_iters,
+                                             float tol, void* workspace, size_t workspace_bytes, void* stream, int first_step,
+                                             int num_steps, int32_t* remaining_out);
+
 /* Tokeniser, the step before the loop: replaces image_to_tokens
  * (glom_pytorch.py:94-97, call :114): patchify 'b c (h p1) (w p2) -> b (h w) (p1 p2 c)'
  * fused with the Linear(3*p*p -> d).
