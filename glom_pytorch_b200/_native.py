@@ -61,8 +61,11 @@ SIGNATURES = {
     "glom_b200_backward_workspace_bytes": (_i32, [_CFG, _i32, _SZP]),
     "glom_b200_backward": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _i32, _i32, _vp, _sz, _vp]),
     "glom_b200_backward_steps": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _vp, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_backward_ex": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _vp, _i32, _i32, _i32, _vp, _sz, _vp]),
     "glom_b200_tokenize_backward_workspace_bytes": (_i32, [_i32, _i32, _i32, _i32, _i32, _SZP]),
     "glom_b200_tokenize_backward": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_tokenize_backward_ex": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz,
+                                              _vp]),
     "glom_b200_profile_begin": (_i32, []),
     "glom_b200_profile_end": (_i32, [ctypes.POINTER(ctypes.c_double), _I32P, _i32]),
     "glom_b200_islands": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp, _vp]),
@@ -240,14 +243,18 @@ def backward_workspace_bytes(cfg, batch):
 
 
 def backward(cfg, weight_ptrs, tokens_ptr, pos_ptr, states_ptr, grad_out_ptr, grad_ptrs, batch, iters, grad_all,
-             ws_ptr, ws_bytes, stream, steps_ptr=None):
+             ws_ptr, ws_bytes, stream, steps_ptr=None, deterministic=False):
     """weight_ptrs: the 8 reference-layout tensors; grad_ptrs: dict of the Grads fields (None allowed for
     d_state0 / d_init).  With steps_ptr (the forward's (batch,) int32 step vector, iters = max_steps):
-    glom_b200_backward_steps, the backward of forward_steps / settle_all."""
+    glom_b200_backward_steps, the backward of forward_steps / settle_all.  deterministic: glom_b200_backward_ex with
+    its fixed-order reductions (bit-reproducible gradients)."""
     w = WeightsRef(ctypes.sizeof(WeightsRef), *weight_ptrs)
     g = Grads(ctypes.sizeof(Grads), *[grad_ptrs.get(k) for k, _ in Grads._fields_[1:]])
     lib = load()
-    if steps_ptr is None:
+    if deterministic:
+        rc = lib.glom_b200_backward_ex(ctypes.byref(cfg), ctypes.byref(w), tokens_ptr, pos_ptr, states_ptr, grad_out_ptr,
+                                       ctypes.byref(g), batch, steps_ptr, iters, int(grad_all), 1, ws_ptr, ws_bytes, stream)
+    elif steps_ptr is None:
         rc = lib.glom_b200_backward(ctypes.byref(cfg), ctypes.byref(w), tokens_ptr, pos_ptr, states_ptr, grad_out_ptr,
                                     ctypes.byref(g), batch, iters, int(grad_all), ws_ptr, ws_bytes, stream)
     else:
@@ -262,8 +269,13 @@ def tokenize_backward_workspace_bytes(batch, h, w, patch, need_d_img):
 
 
 def tokenize_backward(img_ptr, weight_ptr, d_tokens_ptr, d_weight_ptr, d_bias_ptr, d_img_ptr, batch, h, w, patch, dim,
-                      ws_ptr, ws_bytes, stream):
-    """Tokeniser backward; d_* pointers may be None (skipped); outputs are accumulated into."""
+                      ws_ptr, ws_bytes, stream, deterministic=False):
+    """Tokeniser backward; d_* pointers may be None (skipped); outputs are accumulated into.  deterministic:
+    glom_b200_tokenize_backward_ex, d_bias by a fixed-order column sum."""
+    if deterministic:
+        check(load().glom_b200_tokenize_backward_ex(img_ptr, weight_ptr, d_tokens_ptr, d_weight_ptr, d_bias_ptr, d_img_ptr,
+                                                    batch, h, w, patch, dim, 1, ws_ptr, ws_bytes, stream))
+        return
     check(load().glom_b200_tokenize_backward(img_ptr, weight_ptr, d_tokens_ptr, d_weight_ptr, d_bias_ptr, d_img_ptr, batch, h, w,
                                              patch, dim, ws_ptr, ws_bytes, stream))
 

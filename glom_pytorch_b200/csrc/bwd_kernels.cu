@@ -302,6 +302,119 @@ __global__ void init_grad_kernel(int rows, int L, int d, const float* __restrict
   atomicAdd(dinit + i, acc);
 }
 
+// ---- the deterministic backward's reductions (BackwardArgs::deterministic): no floating-point atomics, and every sum
+// runs in an order fixed by the shapes alone -- never by the grid size, the SM count or the order blocks run in.
+// colsum_acc_kernel and init_grad_kernel as one fixed-order column sum: out[c] += sum_r src[r * row_stride + c], out2 as
+// in colsum_acc_kernel, the same frozen rows skipped.  One block owns 32 columns and every row: thread (x, y) sums rows
+// y, y + 32, ... of its column in order, then row y = 0 adds the 32 slice sums in slice order.
+__global__ void __launch_bounds__(1024) colsum_det_kernel(int rows, int cols, long long row_stride,
+                                                          const float* __restrict__ src, float* __restrict__ out,
+                                                          float* __restrict__ out2, int cols2,
+                                                          const int32_t* __restrict__ steps, int t, int n) {
+  const int c = blockIdx.x * 32 + threadIdx.x, y = threadIdx.y;
+  __shared__ float red[32][33];
+  float acc = 0.f;
+  if (c < cols) {
+#pragma unroll 4
+    for (int r = y; r < rows; r += 32)
+      if (!steps || __ldg(steps + r / n) > t) acc += src[(long long)r * row_stride + c];
+  }
+  red[y][threadIdx.x] = acc;
+  __syncthreads();
+  if (y == 0 && c < cols) {
+    float s = red[0][threadIdx.x];
+#pragma unroll
+    for (int i = 1; i < 32; ++i) s += red[i][threadIdx.x];
+    out[c] += s;
+    if (out2 && c < cols2) out2[c] += s;
+  }
+}
+static cudaError_t colsum(bool det, int rows, int cols, long long row_stride, const float* src, float* out, float* out2,
+                          int cols2, const int32_t* steps, int t, int n, cudaStream_t st, int* launches) {
+  if (det)
+    colsum_det_kernel<<<(cols + 31) / 32, dim3(32, 32), 0, st>>>(rows, cols, row_stride, src, out, out2, cols2, steps, t, n);
+  else
+    colsum_acc_kernel<<<dim3((cols + 31) / 32, 16), 256, 0, st>>>(rows, cols, row_stride, src, out, out2, cols2, steps, t, n);
+  if (launches) ++*launches;
+  return cudaGetLastError();
+}
+// After BW_DX<DET>: ds[r, l + 1] += dx_td[r, l] for the top-down groups l = 0 .. L-2, and dpos[i] += the sum of
+// dx_td[b n + i, l] over images b, and groups l within an image.  Block = 32 float4 columns x 8 image slices of one
+// position i: slice y takes images y, y + 8, ... in order, then slice 0 adds the 8 slice sums in slice order.  Images
+// frozen at reverse step t (steps[b] <= t) are skipped: BW_DX skipped their row blocks and wrote nothing for them
+__global__ void __launch_bounds__(256) dx_td_reduce_kernel(int B, int n, int L, int d, const float* __restrict__ dx_td,
+                                                           float* __restrict__ ds, float* __restrict__ dpos,
+                                                           const int32_t* __restrict__ steps, int t) {
+  const int d4 = d / 4, chunks = (d4 + 31) / 32;
+  const int i = blockIdx.x / chunks, c4 = (blockIdx.x % chunks) * 32 + threadIdx.x, y = threadIdx.y;
+  __shared__ float4 red[8][32];
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (c4 < d4) {
+    for (int b = y; b < B; b += 8) {
+      if (steps && __ldg(steps + b) <= t) continue;
+      const size_t r = (size_t)b * n + i;
+      const float4* src = reinterpret_cast<const float4*>(dx_td) + r * (L - 1) * d4 + c4;
+      float4* dst = reinterpret_cast<float4*>(ds) + (r * L + 1) * d4 + c4;
+#pragma unroll 4
+      for (int l = 0; l < L - 1; ++l) {
+        const float4 v = src[(size_t)l * d4];
+        float4 o = dst[(size_t)l * d4];
+        o.x += v.x; o.y += v.y; o.z += v.z; o.w += v.w;
+        dst[(size_t)l * d4] = o;
+        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+      }
+    }
+  }
+  red[y][threadIdx.x] = acc;
+  __syncthreads();
+  if (y == 0 && c4 < d4) {
+    float4 s = red[0][threadIdx.x];
+#pragma unroll
+    for (int k = 1; k < 8; ++k) { const float4 v = red[k][threadIdx.x]; s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w; }
+    float4* p = reinterpret_cast<float4*>(dpos) + (size_t)i * d4 + c4;
+    float4 o = *p;
+    o.x += s.x; o.y += s.y; o.z += s.z; o.w += s.w;
+    *p = o;
+  }
+}
+// After BW_DH<DET>: d_*_b1[g, j] += the sum over 32-row bands k of part[g][k][j].  Block = 32 float4 columns x 16 band
+// slices: slice y takes bands y, y + 16, ... in order, then slice 0 adds the 16 slice sums in slice order.  A band whose
+// rows all belong to images frozen at reverse step t is skipped: BW_DH wrote nothing there when it skipped the band's
+// 128-row block, and exact zeros otherwise
+__global__ void __launch_bounds__(512) bias_partials_kernel(int G, int nbands, int rows, int n, int d,
+                                                            const float* __restrict__ part, float* __restrict__ d_bu_b1,
+                                                            float* __restrict__ d_td_b1, const int32_t* __restrict__ steps,
+                                                            int t) {
+  const int q = blockIdx.x * 32 + threadIdx.x, y = threadIdx.y;     // q: float4 column of the (G, 4d) bias gradients
+  __shared__ float4 red[16][32];
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (q < G * d) {
+    const float4* src = reinterpret_cast<const float4*>(part) + (size_t)(q / d) * nbands * d + q % d;
+    for (int k = y; k < nbands; k += 16) {
+      if (steps) {
+        const int r1 = min(32 * k + 32, rows);
+        bool live = false;
+        for (int b = 32 * k / n; b <= (r1 - 1) / n && !live; ++b) live = __ldg(steps + b) > t;
+        if (!live) continue;
+      }
+      const float4 v = src[(size_t)k * d];
+      acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+    }
+  }
+  red[y][threadIdx.x] = acc;
+  __syncthreads();
+  if (y == 0 && q < G * d) {
+    float4 s = red[0][threadIdx.x];
+#pragma unroll
+    for (int k = 1; k < 16; ++k) { const float4 v = red[k][threadIdx.x]; s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w; }
+    const int g = q / d;
+    float4* p = reinterpret_cast<float4*>(((g & 1) ? d_td_b1 : d_bu_b1) + (size_t)(g >> 1) * 4 * d) + q % d;
+    float4 o = *p;
+    o.x += s.x; o.y += s.y; o.z += s.z; o.w += s.w;
+    *p = o;
+  }
+}
+
 // =====================================================================================
 // Tokeniser backward (image_to_tokens: Rearrange + Linear, glom_pytorch.py:94-97) -- fp32 on CUDA cores
 //   d_weight (d, 3p^2) += dTok^T . patches,  d_bias (d) += column sums of dTok,
@@ -337,7 +450,8 @@ size_t tokenize_backward_workspace_bytes(int B, int H, int W, int p, int need_di
 }
 
 cudaError_t tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight, float* d_bias,
-                              float* d_img, int B, int H, int W, int p, int d, void* workspace, cudaStream_t st, int* launches) {
+                              float* d_img, int B, int H, int W, int p, int d, void* workspace, cudaStream_t st, int* launches,
+                              int deterministic) {
   const int rows = B * (H / p) * (W / p), k3 = 3 * p * p;
   float* patches = static_cast<float*>(workspace);
   float* dpatches = reinterpret_cast<float*>(static_cast<char*>(workspace) + align_up((size_t)rows * k3 * sizeof(float), 1024));
@@ -357,12 +471,9 @@ cudaError_t tokenize_backward(const float* img, const float* weight, const float
     q.alpha = 1.f; q.beta = 1.f; q.bias = nullptr;
     if ((e = gemm_f32(q, 1, st, launches)) != cudaSuccess) return e;
   }
-  if (d_bias) {
-    dim3 grid((d + 31) / 32, 16);
-    colsum_acc_kernel<<<grid, 256, 0, st>>>(rows, d, (long long)d, d_tokens, d_bias);
-    if (launches) ++*launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  }
+  if (d_bias && (e = colsum(deterministic != 0, rows, d, (long long)d, d_tokens, d_bias, nullptr, 0, nullptr, 0, 1, st,
+                            launches)) != cudaSuccess)
+    return e;
   if (d_img) {
     // dpatches (rows, k3) = dTok (rows x d) . W (d x k3)
     GemmF32 q{};
@@ -422,6 +533,11 @@ BackwardLayout backward_layout(const Geometry& g, int precision) {
     w.khatb_off = take((size_t)g.rows * g.L * g.d * 2);
     w.ab_off = take((size_t)g.B * g.L * g.n * g.n * 2);
     w.dsimb_off = take((size_t)g.B * g.L * g.n * g.n * 2);
+    // deterministic backward: BW_DH's bias partials [G][ceil(R/32)][4d] fp32 go to the fp32 pre / h / dh buffers, which
+    // this path leaves unused; only shapes with very few rows per group need a region of their own.  (Its top-down dx
+    // buffer (R, L-1, d) fp32 is dkhat, dead once normalize_bwd_kernel has run.)
+    const size_t part = (size_t)g.G * ((g.rows + 31) / 32) * 4 * g.d * 4;
+    w.b1part_off = part <= w.xp_off - w.pre_off ? w.pre_off : take(part);
   }
   w.total = off;
   return w;
@@ -480,13 +596,11 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
       // dW2 += DY^T h                                     (d x 4d)
       q = GemmF32{d, h4, R, 1, Mat{DY.p, 1, ld, 0, 0}, Mat{hb, h4, 1, 0, 0}, MatOut{dw2 + (size_t)l * d * h4, h4, 1, 0, 0}, 1.f, 1.f, nullptr};
       CK(gemm_f32(q, 1, st, launches));
-      colsum_acc_kernel<<<dim3((d + 31) / 32, 16), 256, 0, st>>>(R, d, ld, DY.p, db2 + (size_t)l * d);
-      CKL();
+      CK(colsum(a.deterministic != 0, R, d, ld, DY.p, db2 + (size_t)l * d, nullptr, 0, nullptr, 0, 1, st, launches));
       // dW1 += dpre^T X                                   (4d x d)
       q = GemmF32{h4, d, R, 1, Mat{dh, 1, h4, 0, 0}, Mat{X.p, X.s_row, 1, 0, 0}, MatOut{dw1 + (size_t)l * h4 * d, d, 1, 0, 0}, 1.f, 1.f, nullptr};
       CK(gemm_f32(q, 1, st, launches));
-      colsum_acc_kernel<<<dim3((h4 + 31) / 32, 16), 256, 0, st>>>(R, h4, h4, dh, db1 + (size_t)l * h4);
-      CKL();
+      CK(colsum(a.deterministic != 0, R, h4, h4, dh, db1 + (size_t)l * h4, nullptr, 0, nullptr, 0, 1, st, launches));
       // dX = dpre W1                                      (R x d)
       q = GemmF32{R, d, h4, 1, Mat{dh, h4, 1, 0, 0}, Mat{W1, d, 1, 0, 0}, MatOut{dx, d, 1, 0, 0}, 1.f, 0.f, nullptr};
       CK(gemm_f32(q, 1, st, launches));
@@ -630,6 +744,9 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
     m.d_tokens = a.d_tokens; m.d_pos = a.d_pos;
     m.d_bu_w1 = a.d_bu_w1; m.d_bu_w2 = a.d_bu_w2; m.d_td_w1 = a.d_td_w1; m.d_td_w2 = a.d_td_w2;
     m.d_bu_b1 = a.d_bu_b1; m.d_td_b1 = a.d_td_b1;
+    m.deterministic = a.deterministic;
+    m.dx_td = reinterpret_cast<float*>(ws + wl.dkhat_off);
+    m.b1_part = reinterpret_cast<float*>(ws + wl.b1part_off);
     pack_bwd_weights_kernel<<<sm_count() * 8, 256, 0, st>>>(g.d, g.L, a.bu_w1, a.bu_b1, a.bu_w2, a.td_w1, a.td_b1, a.td_w2,
                                                      const_cast<__nv_bfloat16*>(m.w1p), const_cast<__nv_bfloat16*>(m.w2t),
                                                      const_cast<__nv_bfloat16*>(m.w1t), const_cast<float*>(m.b1p));
@@ -699,9 +816,16 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
       m.ds = ds;
       m.steps = steps; m.t = t;
       if (int r = mlp_backward_tc(g, m, enc, num_sms, st, launches, err, errlen)) return r;
-      colsum_acc_kernel<<<dim3((g.L * g.d + 31) / 32, 16), 256, 0, st>>>(g.rows, g.L * g.d, (long long)g.L * g.d, gs, a.d_bu_b2,
-                                                                         a.d_td_b2, (g.L - 1) * g.d, steps, t, g.n);
-      CKLI();
+      if (a.deterministic) {     // what the default DH / DX epilogues reduce with atomics, in a fixed order
+        bias_partials_kernel<<<(g.G * g.d + 31) / 32, dim3(32, 16), 0, st>>>(g.G, (g.rows + 31) / 32, g.rows, g.n, g.d,
+                                                                             m.b1_part, a.d_bu_b1, a.d_td_b1, steps, t);
+        CKLI();
+        dx_td_reduce_kernel<<<g.n * ((g.d / 4 + 31) / 32), dim3(32, 8), 0, st>>>(g.B, g.n, g.L, g.d, m.dx_td, ds, a.d_pos,
+                                                                                  steps, t);
+        CKLI();
+      }
+      CKI(colsum(a.deterministic != 0, g.rows, g.L * g.d, (long long)g.L * g.d, gs, a.d_bu_b2, a.d_td_b2, (g.L - 1) * g.d,
+                 steps, t, g.n, st, launches));
     }
     gin = ds;
     gextra = grad_all ? a.grad_out + (size_t)t * state : nullptr;
@@ -713,7 +837,9 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
       add_kernel<<<nblk(state), 256, 0, st>>>(state, part, a.d_state0);
       CKLI();
     }
-    if (a.d_init) {
+    if (a.d_init && a.deterministic) {
+      CKI(colsum(true, g.rows, g.L * g.d, (long long)g.L * g.d, part, a.d_init, nullptr, 0, nullptr, 0, 1, st, launches));
+    } else if (a.d_init) {
       init_grad_kernel<<<dim3((g.L * g.d + 255) / 256, 64), 256, 0, st>>>(g.rows, g.L, g.d, part, a.d_init);
       CKLI();
     }

@@ -222,12 +222,15 @@ struct BackwardArgs {
   // outputs, ACCUMULATED into (caller zero-initialises); d_state0 / d_init: exactly one is non-NULL
   float *d_tokens, *d_pos, *d_state0, *d_init;
   float *d_bu_w1, *d_bu_b1, *d_bu_w2, *d_bu_b2, *d_td_w1, *d_td_b1, *d_td_w2, *d_td_b2;
+  // 1: every reduction runs in an order fixed by the shapes (no floating-point atomics): bit-reproducible gradients
+  int deterministic;
 };
 struct BackwardLayout {
   size_t g_off, gs_off, ds_off, khat_off, dkhat_off, rnorm_off, pre_off, h_off, dh_off, xp_off, dx_off, attn_off,
       dattn_off;
   // bf16 (tensor-core) MLP backward only
   size_t xb_off, sb_off, sp_off, gsb_off, w1p_off, w2t_off, w1t_off, b1p_off, bpre_off, bh_off, bdpre_off;
+  size_t b1part_off;     // deterministic backward: BW_DH's bias partials (normally inside the unused fp32 pre / h / dh)
   size_t khatb_off, ab_off, dsimb_off;     // bf16 khat (state-like), probabilities and scaled dsim (Z, n, n)
   size_t blocked_bytes;
   size_t total;
@@ -246,6 +249,10 @@ struct MlpBwdTc {
   // steps[b] <= t have gs = 0 at reverse step t, so row blocks made only of such rows are skipped
   const int32_t* steps;
   int t;
+  // deterministic (1): no atomics.  DX stores the top-down groups' dx into dx_td (R, L-1, d) and DH the 32-row column
+  // sums of dpre into b1_part [G][ceil(R/32)][4d]; the caller reduces both afterwards (backward_run)
+  int deterministic;
+  float *dx_td, *b1_part;
 };
 int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches,
                     char* err, size_t errlen);
@@ -261,8 +268,10 @@ int attn_bwd_gemm_tc(const Geometry& g, const void* a_src, int a_state, int a_mn
 BackwardLayout backward_layout(const Geometry& g, int precision);
 // tokeniser backward (fp32, CUDA cores; bwd_kernels.cu): any of d_weight / d_bias / d_img may be NULL; all ACCUMULATED into
 size_t tokenize_backward_workspace_bytes(int B, int H, int W, int p, int need_dimg);
+// deterministic: d_bias by a fixed-order column sum instead of atomics (d_weight / d_img have no atomics)
 cudaError_t tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight, float* d_bias,
-                              float* d_img, int B, int H, int W, int p, int d, void* workspace, cudaStream_t st, int* launches);
+                              float* d_img, int B, int H, int W, int p, int d, void* workspace, cudaStream_t st, int* launches,
+                              int deterministic = 0);
 // steps (nullable, device memory): per-image step counts; image b is the identity at every reverse step t >= steps[b]
 int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int iters, int grad_all, const int32_t* steps,
                  void* workspace, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen);

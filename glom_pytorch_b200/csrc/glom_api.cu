@@ -690,9 +690,9 @@ GLOM_B200_API int glom_b200_tokenize_backward_workspace_bytes(int batch, int hei
   return 0;
 }
 
-GLOM_B200_API int glom_b200_tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight,
-                                              float* d_bias, float* d_img, int batch, int height, int width, int patch, int dim,
-                                              void* workspace, size_t workspace_bytes, void* stream) {
+static int tokenize_backward_impl(const float* img, const float* weight, const float* d_tokens, float* d_weight,
+                                  float* d_bias, float* d_img, int batch, int height, int width, int patch, int dim,
+                                  int deterministic, void* workspace, size_t workspace_bytes, void* stream) {
   if (!img || !weight || !d_tokens) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
   if (batch < 1 || patch < 1 || dim < 1 || height < patch || width < patch || height % patch || width % patch)
     return fail(GLOM_B200_ERR_INVALID, "image %dx%d is not a positive multiple of patch %d", height, width, patch);
@@ -703,9 +703,26 @@ GLOM_B200_API int glom_b200_tokenize_backward(const float* img, const float* wei
     return fail(GLOM_B200_ERR_WORKSPACE, "tokeniser backward workspace: need %zu bytes, got %zu", need, workspace_bytes);
   g_launches = 0;
   const cudaError_t e = tokenize_backward(img, weight, d_tokens, d_weight, d_bias, d_img, batch, height, width, patch, dim,
-                                          workspace, static_cast<cudaStream_t>(stream), &g_launches);
+                                          workspace, static_cast<cudaStream_t>(stream), &g_launches, deterministic);
   if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "tokeniser backward: %s", cudaGetErrorString(e));
   return 0;
+}
+
+GLOM_B200_API int glom_b200_tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight,
+                                              float* d_bias, float* d_img, int batch, int height, int width, int patch, int dim,
+                                              void* workspace, size_t workspace_bytes, void* stream) {
+  return tokenize_backward_impl(img, weight, d_tokens, d_weight, d_bias, d_img, batch, height, width, patch, dim, 0,
+                                workspace, workspace_bytes, stream);
+}
+
+GLOM_B200_API int glom_b200_tokenize_backward_ex(const float* img, const float* weight, const float* d_tokens,
+                                                 float* d_weight, float* d_bias, float* d_img, int batch, int height,
+                                                 int width, int patch, int dim, int deterministic, void* workspace,
+                                                 size_t workspace_bytes, void* stream) {
+  if (deterministic != 0 && deterministic != 1)
+    return fail(GLOM_B200_ERR_INVALID, "tokenize_backward_ex: deterministic must be 0 or 1 (got %d)", deterministic);
+  return tokenize_backward_impl(img, weight, d_tokens, d_weight, d_bias, d_img, batch, height, width, patch, dim,
+                                deterministic, workspace, workspace_bytes, stream);
 }
 
 GLOM_B200_API int glom_b200_backward_workspace_bytes(const glom_b200_cfg* cfg, int batch, size_t* out_bytes) {
@@ -718,7 +735,8 @@ GLOM_B200_API int glom_b200_backward_workspace_bytes(const glom_b200_cfg* cfg, i
 // glom_b200_backward (steps == NULL) and glom_b200_backward_steps (per-image step counts, iters = max_steps)
 static int backward_impl(const glom_b200_cfg* cfg, const glom_b200_weights_ref* w, const float* tokens, const float* pos,
                          const float* states, const float* grad_out, const glom_b200_grads* gr, int batch, int iters,
-                         const int32_t* steps, int grad_all, void* workspace, size_t workspace_bytes, void* stream) {
+                         const int32_t* steps, int grad_all, void* workspace, size_t workspace_bytes, void* stream,
+                         int deterministic = 0) {
   if (int r = check_cfg(cfg)) return r;
   if (batch < 1 || iters < 0) return fail(GLOM_B200_ERR_INVALID, "batch must be >= 1 and iters >= 0");
   if (!w || w->struct_size != sizeof(glom_b200_weights_ref) || !gr || gr->struct_size != sizeof(glom_b200_grads))
@@ -741,6 +759,7 @@ static int backward_impl(const glom_b200_cfg* cfg, const glom_b200_weights_ref* 
   a.d_tokens = gr->d_tokens; a.d_pos = gr->d_pos; a.d_state0 = gr->d_state0; a.d_init = gr->d_init;
   a.d_bu_w1 = gr->d_bu_w1; a.d_bu_b1 = gr->d_bu_b1; a.d_bu_w2 = gr->d_bu_w2; a.d_bu_b2 = gr->d_bu_b2;
   a.d_td_w1 = gr->d_td_w1; a.d_td_b1 = gr->d_td_b1; a.d_td_w2 = gr->d_td_w2; a.d_td_b2 = gr->d_td_b2;
+  a.deterministic = deterministic;
   g_launches = 0;
   char msg[400] = "";
   if (int r = backward_run(g, a, cfg->precision, iters, grad_all, steps, workspace, g_encode, di.sms,
@@ -766,6 +785,19 @@ GLOM_B200_API int glom_b200_backward_steps(const glom_b200_cfg* cfg, const glom_
   if (max_steps < 0) return fail(GLOM_B200_ERR_INVALID, "backward_steps: max_steps must be >= 0 (got %d)", max_steps);
   return backward_impl(cfg, w, tokens, pos, states, grad_out, gr, batch, max_steps, steps, grad_all, workspace,
                        workspace_bytes, stream);
+}
+
+GLOM_B200_API int glom_b200_backward_ex(const glom_b200_cfg* cfg, const glom_b200_weights_ref* w, const float* tokens,
+                                        const float* pos, const float* states, const float* grad_out,
+                                        const glom_b200_grads* gr, int batch, const int32_t* steps, int max_steps,
+                                        int grad_all, int deterministic, void* workspace, size_t workspace_bytes,
+                                        void* stream) {
+  if (deterministic != 0 && deterministic != 1)
+    return fail(GLOM_B200_ERR_INVALID, "backward_ex: deterministic must be 0 or 1 (got %d)", deterministic);
+  if (steps && reinterpret_cast<uintptr_t>(steps) % 4) return fail(GLOM_B200_ERR_INVALID, "backward_ex: steps must be 4-byte aligned");
+  if (steps && max_steps < 0) return fail(GLOM_B200_ERR_INVALID, "backward_ex: max_steps must be >= 0 (got %d)", max_steps);
+  return backward_impl(cfg, w, tokens, pos, states, grad_out, gr, batch, max_steps, steps, grad_all, workspace,
+                       workspace_bytes, stream, deterministic);
 }
 
 GLOM_B200_API int glom_b200_islands(const float* states, int slabs, int side_h, int side_w, int levels, int dim, float threshold,

@@ -8,6 +8,8 @@
 // All four use the forward's pipeline structure (tc_kernels.cu): 256 x 256 tiles dealt to pairs of CTAs that compute 128
 // rows each, a TMA producer warp feeding 128B-swizzled smem stages, two wgmma consumer warpgroups with register
 // accumulators that run the epilogue, bounded mbarrier waits.  The attention backward, reductions and the scatter of dx stay on CUDA cores (bwd_kernels.cu).
+// The deterministic backward (MlpBwdTc::deterministic) runs the DET instantiations of DH and DX, whose epilogues store
+// what the default ones add with red.add atomics (see BwdParams::dx_td / b1_part and DESIGN.md).
 #include "tc_common.cuh"
 
 #include <stdio.h>
@@ -68,6 +70,13 @@ struct BwdParams {
   // the problems of such images
   const int32_t* steps;
   int t;
+  // deterministic instantiations (DET): BW_DX stores the top-down groups' dx tiles into dx_td (R, L-1, d) instead of
+  // reducing them into ds / d_pos, and BW_DH stores each warp's 32-row column sum of dpre into b1_part
+  // [G][nbands = ceil(R / 32)][4d] instead of reducing it into d_*_b1; CUDA-core kernels of bwd_kernels.cu then reduce
+  // both in a fixed order
+  float* dx_td;
+  float* b1_part;
+  int nbands;
 };
 
 // rows [r0, r0 + nr) below p.rows all belong to images frozen at this step (an empty range counts as frozen).  Every warp
@@ -140,7 +149,7 @@ __device__ __forceinline__ void normal_cdf_pdf(float x, float& cdf, float& pdf) 
   pdf = tail * hz;
 }
 
-template <int MODE>
+template <int MODE, bool DET = false>
 __global__ void __launch_bounds__(THREADS, 1)
 bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb           DH: gsb (R, L*d)   DX: dpre blocks   DW: gsb
                 const __grid_constant__ CUtensorMap map_a1,   // PRE: Sb                                              DW: dpre blocks
@@ -359,7 +368,19 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
               }
             }
           } else if (MODE == BW_DX) {
-            if (row < p.rows) {
+            if constexpr (DET) {
+              // every element below has one writer in this launch: group 0 owns d_tokens, bottom-up group 2l owns level
+              // l-1 of ds (top-down groups no longer add there), top-down group 2l+1 owns slice l of dx_td
+              const int lg = t.g >> 1;
+              if (row < p.rows && (t.g & 1)) {
+                *reinterpret_cast<float4*>(p.dx_td + ((size_t)row * (p.L - 1) + lg) * p.d + col) = acc;
+              } else if (row < p.rows) {
+                float* dst = t.g == 0 ? p.d_tokens + (size_t)row * p.d + col : p.ds + ((size_t)row * p.L + lg - 1) * p.d + col;
+                float4 o = *reinterpret_cast<const float4*>(dst);
+                o.x += acc.x; o.y += acc.y; o.z += acc.z; o.w += acc.w;
+                *reinterpret_cast<float4*>(dst) = o;
+              }
+            } else if (row < p.rows) {
               // several groups (and, for pos, all images) add into the same element: reduce in L2, no dx round trip
               const int lg = t.g >> 1;
               if (t.g == 0) {
@@ -406,9 +427,15 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
             colsum[e] += __shfl_xor_sync(0xffffffffu, colsum[e], 8);
             colsum[e] += __shfl_xor_sync(0xffffffffu, colsum[e], 16);
           }
-          if (rsub == 0)
+          if constexpr (DET) {
+            // deterministic: the band's partial goes to its own slot, reduced over bands in order by bias_partials_kernel
+            if (rsub == 0 && row0 < p.rows)
+              *reinterpret_cast<float4*>(p.b1_part + ((size_t)t.g * p.nbands + row0 / 32) * 4 * p.d + col) =
+                  make_float4(colsum[0], colsum[1], colsum[2], colsum[3]);
+          } else if (rsub == 0) {
             red_add_f32x4(((t.g & 1) ? p.d_td_b1 : p.d_bu_b1) + (size_t)(t.g >> 1) * 4 * p.d + col,
                           make_float4(colsum[0], colsum[1], colsum[2], colsum[3]));
+          }
         }
         __syncwarp();
         named_bar_sync(1 + quad, 64);                                   // staging tile free for the next step
@@ -432,11 +459,11 @@ bool map2d_box(EncodeTiledFn enc, CUtensorMap* m, const void* base, uint64_t row
   return true;
 }
 
-template <int MODE>
+template <int MODE, bool DET = false>
 cudaError_t launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& b0,
                    const CUtensorMap& b1, const CUtensorMap& b2, const BwdParams& p, int num_sms, cudaStream_t st) {
   static SmemOptIn optin;
-  if (cudaError_t e = optin.ensure(bwd_gemm_kernel<MODE>, SMEM_BYTES)) return e;
+  if (cudaError_t e = optin.ensure(bwd_gemm_kernel<MODE, DET>, SMEM_BYTES)) return e;
   const int max_pairs = num_sms / 2;
   const int pairs = p.num_tiles < max_pairs ? p.num_tiles : max_pairs;
   cudaLaunchConfig_t cfg{};
@@ -448,7 +475,7 @@ cudaError_t launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorM
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, bwd_gemm_kernel<MODE>, a0, a1, a2, b0, b1, b2, p);
+  return cudaLaunchKernelEx(&cfg, bwd_gemm_kernel<MODE, DET>, a0, a1, a2, b0, b1, b2, p);
 }
 
 bool map3d_box(EncodeTiledFn enc, CUtensorMap* m, const void* base, uint64_t inner, uint64_t rows, uint64_t batches,
@@ -529,17 +556,20 @@ int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int
   p.d_bu_w1 = a.d_bu_w1; p.d_bu_w2 = a.d_bu_w2; p.d_td_w1 = a.d_td_w1; p.d_td_w2 = a.d_td_w2;
   p.d_bu_b1 = a.d_bu_b1; p.d_td_b1 = a.d_td_b1;
   p.steps = a.steps; p.t = a.t;
+  p.dx_td = a.dx_td; p.b1_part = a.b1_part; p.nbands = (rows + 31) / 32;
   const int nm = (rows + 255) / 256;
   cudaError_t e;
   p.num_tiles = G * nm * (4 * d / BN);
   e = launch<BW_PRE>(mxb, msb, msp, mw1p, mw1p, mw1p, p, num_sms, st);
   if (launches) ++*launches;
   if (e != cudaSuccess) { snprintf(err, errlen, "bwd pre launch: %s", cudaGetErrorString(e)); return -3; }
-  e = launch<BW_DH>(mgs, mgs, mgs, mw2t, mw2t, mw2t, p, num_sms, st);
+  e = a.deterministic ? launch<BW_DH, true>(mgs, mgs, mgs, mw2t, mw2t, mw2t, p, num_sms, st)
+                      : launch<BW_DH>(mgs, mgs, mgs, mw2t, mw2t, mw2t, p, num_sms, st);
   if (launches) ++*launches;
   if (e != cudaSuccess) { snprintf(err, errlen, "bwd dh launch: %s", cudaGetErrorString(e)); return -3; }
   p.num_tiles = G * nm * (d / BN);
-  e = launch<BW_DX>(mdpre128, mdpre128, mdpre128, mw1t, mw1t, mw1t, p, num_sms, st);
+  e = a.deterministic ? launch<BW_DX, true>(mdpre128, mdpre128, mdpre128, mw1t, mw1t, mw1t, p, num_sms, st)
+                      : launch<BW_DX>(mdpre128, mdpre128, mdpre128, mw1t, mw1t, mw1t, p, num_sms, st);
   if (launches) ++*launches;
   if (e != cudaSuccess) { snprintf(err, errlen, "bwd dx launch: %s", cudaGetErrorString(e)); return -3; }
   p.num_tiles = G * 2 * (d / 256) * (4 * d / BN);

@@ -15,8 +15,10 @@ fallback -- inputs on other devices raise.  Under autograd the loop is a ``torch
 is ``glom_b200_backward`` (bf16 engine: the MLP and consensus GEMMs of the reverse pass on wgmma tensor cores, the
 softmax / normalisation / bias reductions in fp32 on CUDA cores; fp32 engine: everything fp32 on CUDA cores): the
 forward keeps S_0..S_T and the reverse pass recomputes each step's intermediates (README.md:58-90 training use).
-The backward is once-differentiable and accumulates with ``red.add`` atomics, so gradients are reproducible only up
-to fp32 summation order.
+The backward is once-differentiable.  By default it accumulates some sums with ``red.add`` atomics, so gradients are
+reproducible only up to fp32 summation order; under ``torch.use_deterministic_algorithms(True)`` (read when the
+backward runs, ``warn_only`` included) it reduces in an order fixed by the shapes instead, and the gradients are
+bit-identical from run to run on the same GPU model and build (DESIGN.md, "Deterministic backward").
 
 Packed weights: the MLP weights are repacked (one small kernel) on EVERY call while ``self.training``; in eval mode
 the packed copy is cached and keyed on each parameter's ``(data_ptr, _version)`` and dropped by ``load_state_dict``,
@@ -187,7 +189,8 @@ class _ColumnUpdate(torch.autograd.Function):
             _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
                              grad_out.data_ptr(), ptrs, b, iters, ctx.return_all, ws.data_ptr(), ws.numel(),
                              torch.cuda.current_stream(device).cuda_stream,
-                             None if ctx.steps is None else ctx.steps.data_ptr())
+                             None if ctx.steps is None else ctx.steps.data_ptr(),
+                             deterministic=torch.are_deterministic_algorithms_enabled())
         return (None, None, None, None, None, g["d_tokens"], g["d_pos"], g["d_state0"] if ctx.want_state0 else None,
                 g["d_init"], *[g[k] for k in names])
 
@@ -229,7 +232,8 @@ class _Tokenize(torch.autograd.Function):
             _native.tokenize_backward(img.data_ptr(), wt.data_ptr(), d_tokens.data_ptr(),
                                       None if d_w is None else d_w.data_ptr(), None if d_b is None else d_b.data_ptr(),
                                       None if d_i is None else d_i.data_ptr(), b, h, w, p, module.dim,
-                                      ws.data_ptr(), ws.numel(), torch.cuda.current_stream(device).cuda_stream)
+                                      ws.data_ptr(), ws.numel(), torch.cuda.current_stream(device).cuda_stream,
+                                      deterministic=torch.are_deterministic_algorithms_enabled())
         return None, d_i, d_w, d_b
 
 

@@ -263,6 +263,18 @@ GLOM_B200_API int glom_b200_backward_steps(const glom_b200_cfg* cfg, const glom_
                                            const float* tokens, const float* pos, const float* states, const float* grad_out,
                                            const glom_b200_grads* grads, int batch, const int32_t* steps, int max_steps,
                                            int grad_all, void* workspace, size_t workspace_bytes, void* stream);
+/* glom_b200_backward (steps == NULL, iters = max_steps) or glom_b200_backward_steps (steps != NULL), with
+ * deterministic = 1: bit-reproducible gradients.  No floating-point atomics run: every sum that the default path
+ * accumulates with red.add / atomicAdd (the tensor-core MLP backward's dL/dS_t, dL/dpos and first-layer bias gradients,
+ * the bias column sums, d_init) is computed in an order fixed by the shapes alone, independent of the grid and of the
+ * SM count, so the same inputs give the same bits on every run on the same GPU model and build.  deterministic = 0 is
+ * exactly the default entry points.  Same workspace as glom_b200_backward.  Argument errors (deterministic not 0 or 1,
+ * misaligned steps, max_steps < 0, and those of glom_b200_backward) are reported before any device query. */
+GLOM_B200_API int glom_b200_backward_ex(const glom_b200_cfg* cfg, const glom_b200_weights_ref* weights,
+                                        const float* tokens, const float* pos, const float* states, const float* grad_out,
+                                        const glom_b200_grads* grads, int batch, const int32_t* steps, int max_steps,
+                                        int grad_all, int deterministic, void* workspace, size_t workspace_bytes,
+                                        void* stream);
 
 /* Backward of glom_b200_tokenize (image_to_tokens, glom_pytorch.py:94-97; SURVEY 8 rows f1 + f2), fp32 on CUDA cores:
  *   d_weight (dim, 3 patch^2) += d_tokens^T . patches,   d_bias (dim) += column sums of d_tokens,
@@ -274,6 +286,13 @@ GLOM_B200_API int glom_b200_tokenize_backward_workspace_bytes(int batch, int hei
 GLOM_B200_API int glom_b200_tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight,
                                               float* d_bias, float* d_img, int batch, int height, int width, int patch, int dim,
                                               void* workspace, size_t workspace_bytes, void* stream);
+/* glom_b200_tokenize_backward with deterministic = 1: d_bias by a fixed-order column sum instead of atomics (d_weight
+ * and d_img never use atomics), so all three are bit-reproducible.  deterministic must be 0 or 1 (checked before any
+ * device query); same workspace. */
+GLOM_B200_API int glom_b200_tokenize_backward_ex(const float* img, const float* weight, const float* d_tokens,
+                                                 float* d_weight, float* d_bias, float* d_img, int batch, int height,
+                                                 int width, int patch, int dim, int deterministic, void* workspace,
+                                                 size_t workspace_bytes, void* stream);
 
 /* Per-kernel device timing for the roofline report (bench.py).  Between _begin and _end every
  * kernel the forward/tokenize calls of THIS thread enqueue is bracketed by CUDA events on the
