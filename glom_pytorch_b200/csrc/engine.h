@@ -180,6 +180,11 @@ cudaError_t launch_steps_schedule(const Geometry& g, int t, int max_steps, const
 cudaError_t launch_steps_fill(const Geometry& g, int max_steps, const int32_t* steps, float* states, cudaStream_t st,
                               int* launches);
 
+// fp32 consensus (attn_f32_kernel): a block of 16 queries keeps their rows (16 x dim) and logits (16 x n) as fp32 in
+// shared memory, within the 227 KB a block may opt in to: dim + n <= 3632
+constexpr int kAttnF32Queries = 16;
+constexpr int kAttnF32MaxDimPlusN = (int)((227 * 1024) / (kAttnF32Queries * sizeof(float)));
+
 struct F32Buffers {
   const float* s_in;  float* s_out;
   const float* x;  const float* pos;

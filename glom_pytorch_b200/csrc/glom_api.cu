@@ -479,6 +479,10 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
                         const SettleRun* settle, const int32_t* steps) {
   if (int r = check_cfg(cfg)) return r;
   if (batch < 1 || iters < 0) return fail(GLOM_B200_ERR_INVALID, "batch must be >= 1 and iters >= 0");
+  if (cfg->precision == GLOM_B200_FP32 && cfg->dim + cfg->n > kAttnF32MaxDimPlusN)
+    return fail(GLOM_B200_ERR_INVALID,
+                "fp32 consensus keeps %d (dim + n) floats per block in shared memory: dim + n must be <= %d (got %d)",
+                kAttnF32Queries, kAttnF32MaxDimPlusN, cfg->dim + cfg->n);
   if (!packed_weights || !tokens || !pos || !state_out) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
   if (!state_in && !init_levels) return fail(GLOM_B200_ERR_INVALID, "need state_in or init_levels");
   if (state_in == state_out) return fail(GLOM_B200_ERR_INVALID, "state_out must not alias state_in");

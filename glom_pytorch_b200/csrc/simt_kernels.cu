@@ -242,7 +242,7 @@ __global__ void __launch_bounds__(256) sgemm_kernel(SgemmParams q) {
 // =====================================================================================
 // fp32 consensus attention (glom_pytorch.py:56-73).  Block = (image b, level l, 16 queries).
 // =====================================================================================
-constexpr int AQ = 16;
+constexpr int AQ = kAttnF32Queries;
 __device__ __forceinline__ void store_consensus(float* p, float v) { *p = v; }
 __device__ __forceinline__ void store_consensus(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 // OutT = float: the fp32 engine.  OutT = bf16: the bf16 engine's path for more columns than the tensor-core kernel
@@ -314,14 +314,29 @@ __global__ void __launch_bounds__(256) attn_f32_kernel(int n, int L, int d, int 
     for (int j = lane; j < n; j += 32) sim[qi * n + j] *= inv;
   }
   __syncthreads();
-  for (int c = threadIdx.x; c < d; c += 256) {                                   // P.V (:72)
-    float acc[AQ];
+  // P.V (:72), summed in blocks of 32 keys whose partial sums go into a compensated (Kahan) total: the rounding error
+  // is that of a 32-term sum at any n.  One running sum over all keys let it grow linearly in n when the keys are equal
+  // (every step from init_levels): 1.4e-5 relative on S_1 at n = 3600
+  for (int c = threadIdx.x; c < d; c += 256) {
+    float acc[AQ], comp[AQ];
 #pragma unroll
-    for (int i = 0; i < AQ; ++i) acc[i] = 0.f;
-    for (int j = 0; j < n; ++j) {
-      const float v = s[((img + j) * L + l) * d + c];
+    for (int i = 0; i < AQ; ++i) acc[i] = comp[i] = 0.f;
+    for (int j0 = 0; j0 < n; j0 += 32) {
+      const int j1 = min(j0 + 32, n);
+      float part[AQ];
 #pragma unroll
-      for (int i = 0; i < AQ; ++i) acc[i] = fmaf(sim[i * n + j], v, acc[i]);
+      for (int i = 0; i < AQ; ++i) part[i] = 0.f;
+      for (int j = j0; j < j1; ++j) {
+        const float v = s[((img + j) * L + l) * d + c];
+#pragma unroll
+        for (int i = 0; i < AQ; ++i) part[i] = fmaf(sim[i * n + j], v, part[i]);
+      }
+#pragma unroll
+      for (int i = 0; i < AQ; ++i) {
+        const float y = part[i] - comp[i], t = acc[i] + y;
+        comp[i] = (t - acc[i]) - y;
+        acc[i] = t;
+      }
     }
 #pragma unroll
     for (int i = 0; i < AQ; ++i)
@@ -332,7 +347,7 @@ __global__ void __launch_bounds__(256) attn_f32_kernel(int n, int L, int d, int 
 template <typename OutT>
 static cudaError_t launch_attn_simt(const Geometry& g, const float* s, OutT* c, cudaStream_t st, int* launches) {
   const size_t smem = (size_t)(AQ * g.d + AQ * g.n) * sizeof(float);
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
+  if (g.d + g.n > kAttnF32MaxDimPlusN) return cudaErrorInvalidValue;     // forward_impl rejects this shape up front
   static SmemOptIn optin;
   if (smem > 48 * 1024) {
     cudaError_t e = optin.ensure(attn_f32_kernel<OutT>, smem);

@@ -27,8 +27,9 @@ the packed copy is cached and keyed on each parameter's ``(data_ptr, _version)``
 
 Engine-only knob (keyword-only, additive): ``precision`` = ``"bf16"`` (default; wgmma tensor cores,
 bf16 operands, fp32 accumulate and fp32 state -- the arithmetic of the reference under
-``torch.autocast(dtype=torch.bfloat16)``) or ``"fp32"`` (CUDA-core path matching the reference's fp32
-forward to ~1e-5).
+``torch.autocast(dtype=torch.bfloat16)``) or ``"fp32"`` (CUDA-core path: each step within 8e-7 relative, per
+kernel tile, of the same step in float64 from the same state; tests/test_cuda_core_oracle.py).  The fp32 engine needs
+dim + n <= 3632 (its consensus keeps a block's 16 query rows and logits in shared memory).
 """
 from math import sqrt
 

@@ -6,7 +6,8 @@ that it uses every host core the way the reference's own torch/oneDNN path does.
 arm (``kind: "port"``) ONLY when the unmodified reference package is not importable on the box
 (``$GLOM_REF_PATH`` -> ``baseline/_ref`` -> ``/root/reference``); ``tests/test_oracle_golden.py`` checks it against
 the same golden fixtures as the numpy oracle.  ``column_step`` is the loop body as a differentiable float64-capable
-function; ``grads_at_states`` and ``step_backward_bf16`` are the backward references of ``tests/test_backward_oracle.py``,
+function and ``hidden_activations`` its MLPs' hidden layer (``tests/test_cuda_core_oracle.py``);
+``grads_at_states`` and ``step_backward_bf16`` are the backward references of ``tests/test_backward_oracle.py``,
 ``step_forward_bf16`` the one-step forward reference of ``tests/test_forward_oracle.py``, ``settle_change``,
 ``settle_ratio`` and ``settle_rule`` the settle references of ``tests/test_settle_oracle.py``.
 Only ``tests/`` and ``bench.py``'s CPU legs may import this module.
@@ -118,6 +119,23 @@ def grads_at_states(P, tokens, pos, states, cot, *, return_all, steps=None, atte
             g = g + cot[t]
     acc["d_state0"] = g
     return acc
+
+
+def hidden_activations(P, tokens, pos, levels):
+    """The MLPs' hidden activations of one step in float64: (2L-1, B*n, 4d), group g = 2l the bottom-up MLP of level l
+    (input tokens for l = 0, else levels[:, :, l-1]), g = 2l+1 the top-down MLP of level l (input levels[:, :, l+1] +
+    pos), H_g = gelu(A_g W1_g^T + b1_g) with the exact-erf GELU (:27-33, :134-136).  This is the engine's group order."""
+    P = {k: _f64(P[k]) for k in MLP_KEYS}
+    tokens, pos, levels = _f64(tokens), _f64(pos), _f64(levels)
+    B, n, L, d = levels.shape
+    w1 = [P["bottom_up.net.1.weight"].reshape(L, 4 * d, d), P["top_down.net.1.weight"].reshape(L - 1, 4 * d, d)]
+    b1 = [P["bottom_up.net.1.bias"].reshape(L, 4 * d), P["top_down.net.1.bias"].reshape(L - 1, 4 * d)]
+    H = []
+    for g in range(2 * L - 1):
+        net, l = g & 1, g >> 1
+        a = levels[:, :, l + 1] + pos[None] if net else (tokens if l == 0 else levels[:, :, l - 1])
+        H.append(F.gelu(a.reshape(B * n, d) @ w1[net][l].T + b1[net][l]))
+    return torch.stack(H)
 
 
 def patchify(img, p):
