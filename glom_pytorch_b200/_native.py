@@ -52,6 +52,11 @@ SIGNATURES = {
     "glom_b200_settle_queue_begin": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _sz, _vp]),
     "glom_b200_settle_queue_run": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _vp, _sz, _vp,
                                           _i32, _i32, _vp]),
+    "glom_b200_settle_video_workspace_bytes": (_i32, [_CFG, _i32, _i32, _SZP]),
+    "glom_b200_settle_video_begin": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _sz,
+                                            _vp]),
+    "glom_b200_settle_video_run": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _sz,
+                                          _vp, _i32, _i32, _vp]),
     "glom_b200_forward_steps_workspace_bytes": (_i32, [_CFG, _i32, _i32, _i32, _SZP]),
     "glom_b200_forward_steps": (_i32, [_CFG, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _sz, _vp]),
     "glom_b200_tokenize_workspace_bytes": (_i32, [_i32, _i32, _i32, _i32, _i32, _i32, _SZP]),
@@ -228,6 +233,26 @@ def settle_queue_run(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_pt
     check(load().glom_b200_settle_queue_run(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr,
                                             out_ptr, steps_ptr, images, slots, max_iters, float(tol), ws_ptr, ws_bytes,
                                             stream, first_step, num_steps, remaining_ptr))
+
+
+def settle_video_workspace_bytes(cfg, slots, max_iters):
+    return _bytes("glom_b200_settle_video_workspace_bytes", ctypes.byref(cfg), slots, max_iters)
+
+
+def settle_video_begin(cfg, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, steps_ptr, streams, frames, slots,
+                       max_iters, tol, ws_ptr, ws_bytes, stream):
+    """glom_b200_settle_video_begin: every slot empty, all `streams` queued (enqueued on `stream`)."""
+    check(load().glom_b200_settle_video_begin(ctypes.byref(cfg), tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr,
+                                              steps_ptr, streams, frames, slots, max_iters, float(tol), ws_ptr, ws_bytes,
+                                              stream))
+
+
+def settle_video_run(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, steps_ptr, streams, frames,
+                     slots, max_iters, tol, ws_ptr, ws_bytes, stream, first_step, num_steps, remaining_ptr):
+    """glom_b200_settle_video_run: as settle_queue_run; the count is of unfinished frames."""
+    check(load().glom_b200_settle_video_run(ctypes.byref(cfg), packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr,
+                                            out_ptr, steps_ptr, streams, frames, slots, max_iters, float(tol), ws_ptr,
+                                            ws_bytes, stream, first_step, num_steps, remaining_ptr))
 
 
 def forward_steps(cfg, packed_ptr, tokens_ptr, pos_ptr, state_in_ptr, init_ptr, out_ptr, batch, steps_ptr, max_steps,

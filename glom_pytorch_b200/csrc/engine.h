@@ -86,29 +86,31 @@ struct SettleLayout {
 };
 SettleLayout settle_layout(const Geometry& g, int max_iters, int return_all = 0);
 
-// Glom.settle_queue (bf16 engine): B = slots.  The settle workspace for (slots, max_iters), whose fp32 slab is slab 0 of
-// the two private slabs that hold S_t of the slots (slab t & 1), followed by slab 1 and the per-slot queue state
+// Glom.settle_queue and Glom.settle_video (bf16 engine): B = slots.  The settle workspace for (slots, max_iters), whose
+// fp32 slab is slab 0 of the two private slabs that hold S_t of the slots (slab t & 1), followed by slab 1 and the
+// per-slot queue state.  settle_video's images are its frames, stream-major: image i = stream * frames + frame.
 struct QueueLayout {
   SettleLayout settle;
   size_t slab_off[2];      // (B, n, L, d) f32 each
-  size_t queue_off;        // initialised by glom_b200_settle_queue_begin:
+  size_t queue_off;        // initialised by glom_b200_settle_queue_begin / glom_b200_settle_video_begin:
   size_t slot_img_off;     //   [B] int   image in the slot, -1: none
   size_t age_off;          //   [B] int   steps the slot's image has run
   size_t pending_off;      //   [B] int   1: the image stopped; its final state waits in the slab for the next fill
   size_t gather_off;       //   [B] int   this step's fill hands the slot's final state to this image, -1: none
   size_t fresh_off;        //   [B] int   1: the slot admitted an image at this step
   size_t block_fresh_off;  //   [ceil(rows/256)] int   1: the block holds a slot admitted at this step
-  size_t head_off;         //   [1] int   next queued image
+  size_t head_off;         //   [1] int   next queued stream (settle_queue: image)
   size_t unfinished_off;   //   [1] int   images queued or in flight
   size_t queue_bytes;
   size_t total;
 };
 QueueLayout queue_layout(const Geometry& g, int max_iters);
 
-// device pointers into the queue state (QueueLayout), images = N; all NULL for Glom.settle
+// device pointers into the queue state (QueueLayout), images = N (settle_video: streams * frames); frames = 1 for
+// settle_queue; all NULL for Glom.settle
 struct QueueSlots {
   int *slot_img, *age, *pending, *gather_img, *fresh, *block_fresh, *head, *unfinished;
-  int images, max_iters;
+  int images, frames, max_iters;
 };
 
 // ---- launchers (return cudaError_t of the launch; all asynchronous on `st`) -----------------
@@ -155,11 +157,13 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTil
 cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
                                    int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, cudaStream_t st,
                                    int* launches, const QueueSlots* q = nullptr);
-// Glom.settle_queue (settle_kernels.cu).  init: the queue state of a new call (every slot empty, N images queued).
-// schedule, before step t: each finished or empty slot, in slot order, hands its stopped image over to the fill and,
-// when `admit` and the queue is not empty, takes the next queued image; writes frozen / block_frozen / block_fresh.
+// Glom.settle_queue / Glom.settle_video (settle_kernels.cu).  init: the queue state of a new call (every slot empty, all
+// images queued).  schedule, before step t: each finished or empty slot, in slot order, hands its stopped image over to
+// the fill and, when `admit`, takes the next frame of its stream (settle_video) or else, while the queue is not empty,
+// frame 0 of the next queued stream (settle_queue: the next queued image); writes frozen / block_frozen / block_fresh.
 // fill, after the schedule: the handed-over images' final states from slab (S_t of the slots) into state_out, then S_0
-// of each admitted image into slab, its bf16 shadows sb / sp and norm partials nsq, and its bf16 token rows xb.
+// of each admitted image into slab (a continuing stream's S_0 is already there), its bf16 shadows sb / sp and norm
+// partials nsq, and its bf16 token rows xb.
 cudaError_t launch_queue_init(const Geometry& g, const QueueSlots& q, int* frozen, int* block_frozen, unsigned int* done,
                               cudaStream_t st, int* launches, Profiler* prof);
 cudaError_t launch_queue_schedule(const Geometry& g, const QueueSlots& q, int admit, int* frozen, int* block_frozen,

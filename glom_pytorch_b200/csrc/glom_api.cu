@@ -340,38 +340,48 @@ GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void*
   return r;
 }
 
-// glom_b200_settle_queue_*: the arguments shared by _begin and _run, checked in the same order as settle's
+// glom_b200_settle_queue_* and glom_b200_settle_video_*: the arguments shared by _begin and _run, checked in the same
+// order as settle's.  settle_queue queues `items` = N images (frames = 1); settle_video queues `items` = S streams of
+// `frames` frames each, and its images are the S * frames frames.
+struct QueueMode { const char* name; const char* items; };
+static const QueueMode kQueue{"settle_queue", "images"}, kVideo{"settle_video", "streams"};
+
 struct QueueArgs {
+  const QueueMode& mode;
   const glom_b200_cfg* cfg; const float *tokens, *pos, *state_in, *init_levels; float* state_out; int32_t* steps_out;
-  int images, slots, max_iters; float tol; void* workspace; size_t workspace_bytes; void* stream;
+  int items, frames, slots, max_iters; float tol; void* workspace; size_t workspace_bytes; void* stream;
 };
 
-static int check_queue_sizes(const glom_b200_cfg* cfg, int images, int slots, int max_iters) {
+static int check_queue_sizes(const QueueMode& m, const glom_b200_cfg* cfg, int items, int frames, int slots, int max_iters) {
   if (int r = check_cfg(cfg)) return r;
-  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "settle_queue: bf16 engine only (precision fp32 given)");
-  if (images < 1) return fail(GLOM_B200_ERR_INVALID, "settle_queue: images must be >= 1 (got %d)", images);
-  if (slots < 1) return fail(GLOM_B200_ERR_INVALID, "settle_queue: slots must be >= 1 (got %d)", slots);
-  if (max_iters < 1) return fail(GLOM_B200_ERR_INVALID, "settle_queue: max_iters must be >= 1 (got %d)", max_iters);
+  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "%s: bf16 engine only (precision fp32 given)", m.name);
+  if (items < 1) return fail(GLOM_B200_ERR_INVALID, "%s: %s must be >= 1 (got %d)", m.name, m.items, items);
+  if (frames < 1) return fail(GLOM_B200_ERR_INVALID, "%s: frames must be >= 1 (got %d)", m.name, frames);
+  if ((int64_t)items * frames > INT32_MAX)
+    return fail(GLOM_B200_ERR_INVALID, "%s: %s x frames must be < 2^31 (got %d x %d)", m.name, m.items, items, frames);
+  if (slots < 1) return fail(GLOM_B200_ERR_INVALID, "%s: slots must be >= 1 (got %d)", m.name, slots);
+  if (max_iters < 1) return fail(GLOM_B200_ERR_INVALID, "%s: max_iters must be >= 1 (got %d)", m.name, max_iters);
   return 0;
 }
 
 // -> 0 and the geometry / layout of the slots, after every argument check and the device query
 static int check_queue(const QueueArgs& a, Geometry* g, QueueLayout* ql, DeviceInfo* di) {
-  if (int r = check_queue_sizes(a.cfg, a.images, a.slots, a.max_iters)) return r;
-  if (a.tol != a.tol) return fail(GLOM_B200_ERR_INVALID, "settle_queue: tol is NaN");
-  if (int r = check_steps_ptr("settle_queue", "steps_out", a.steps_out)) return r;
-  if (!a.tokens || !a.pos || !a.state_out) return fail(GLOM_B200_ERR_INVALID, "settle_queue: a required pointer is NULL");
-  if (!a.state_in && !a.init_levels) return fail(GLOM_B200_ERR_INVALID, "settle_queue: need state_in or init_levels");
-  if (a.state_in == a.state_out) return fail(GLOM_B200_ERR_INVALID, "settle_queue: state_out must not alias state_in");
-  if (reinterpret_cast<uintptr_t>(a.workspace) % 1024) return fail(GLOM_B200_ERR_INVALID, "settle_queue: workspace must be 1024-byte aligned");
+  const char* fn = a.mode.name;
+  if (int r = check_queue_sizes(a.mode, a.cfg, a.items, a.frames, a.slots, a.max_iters)) return r;
+  if (a.tol != a.tol) return fail(GLOM_B200_ERR_INVALID, "%s: tol is NaN", fn);
+  if (int r = check_steps_ptr(fn, "steps_out", a.steps_out)) return r;
+  if (!a.tokens || !a.pos || !a.state_out) return fail(GLOM_B200_ERR_INVALID, "%s: a required pointer is NULL", fn);
+  if (!a.state_in && !a.init_levels) return fail(GLOM_B200_ERR_INVALID, "%s: need state_in or init_levels", fn);
+  if (a.state_in == a.state_out) return fail(GLOM_B200_ERR_INVALID, "%s: state_out must not alias state_in", fn);
+  if (reinterpret_cast<uintptr_t>(a.workspace) % 1024) return fail(GLOM_B200_ERR_INVALID, "%s: workspace must be 1024-byte aligned", fn);
   if (reinterpret_cast<uintptr_t>(a.tokens) % 16 || reinterpret_cast<uintptr_t>(a.pos) % 16 ||
       reinterpret_cast<uintptr_t>(a.state_out) % 16 || reinterpret_cast<uintptr_t>(a.state_in) % 16 ||
       reinterpret_cast<uintptr_t>(a.init_levels) % 16)
-    return fail(GLOM_B200_ERR_INVALID, "settle_queue: tensor pointers must be 16-byte aligned");
+    return fail(GLOM_B200_ERR_INVALID, "%s: tensor pointers must be 16-byte aligned", fn);
   *g = make_geometry(a.cfg, a.slots);
   *ql = queue_layout(*g, a.max_iters);
   if (!a.workspace || a.workspace_bytes < ql->total)
-    return fail(GLOM_B200_ERR_WORKSPACE, "settle_queue workspace: need %zu bytes, got %zu", ql->total, a.workspace_bytes);
+    return fail(GLOM_B200_ERR_WORKSPACE, "%s workspace: need %zu bytes, got %zu", fn, ql->total, a.workspace_bytes);
   return device_info(di);
 }
 
@@ -386,7 +396,8 @@ static QueueSlots queue_slots(const QueueArgs& a, const QueueLayout& ql) {
   q.block_fresh = reinterpret_cast<int*>(ws + ql.block_fresh_off);
   q.head = reinterpret_cast<int*>(ws + ql.head_off);
   q.unfinished = reinterpret_cast<int*>(ws + ql.unfinished_off);
-  q.images = a.images;
+  q.images = a.items * a.frames;
+  q.frames = a.frames;
   q.max_iters = a.max_iters;
   return q;
 }
@@ -400,7 +411,7 @@ static int queue_begin(const QueueArgs& a) {
                                           reinterpret_cast<int*>(ws + ql.settle.block_frozen_off),
                                           reinterpret_cast<unsigned int*>(ws + ql.settle.done_off),
                                           static_cast<cudaStream_t>(a.stream), &g_launches, &g_prof);
-  if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle_queue init launch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "%s init launch: %s", a.mode.name, cudaGetErrorString(e));
   g_err[0] = 0;
   return 0;
 }
@@ -409,13 +420,14 @@ static int queue_begin(const QueueArgs& a) {
 // the schedule and fill of step first_step without admissions, i.e. the hand-over of the images that stopped last.
 static int queue_run(const QueueArgs& a, const void* packed_weights, int first_step, int num_steps, int32_t* remaining_out) {
   Geometry g{}; QueueLayout ql{}; DeviceInfo di{};
-  if (int r = check_queue_sizes(a.cfg, a.images, a.slots, a.max_iters)) return r;
+  const char* fn = a.mode.name;
+  if (int r = check_queue_sizes(a.mode, a.cfg, a.items, a.frames, a.slots, a.max_iters)) return r;
   if (!packed_weights || reinterpret_cast<uintptr_t>(packed_weights) % 1024)
-    return fail(GLOM_B200_ERR_INVALID, "settle_queue: packed weights NULL or not 1024-byte aligned");
+    return fail(GLOM_B200_ERR_INVALID, "%s: packed weights NULL or not 1024-byte aligned", fn);
   if (first_step < 0 || num_steps < 0)
-    return fail(GLOM_B200_ERR_INVALID, "settle_queue: first_step and num_steps must be >= 0 (got %d, %d)", first_step, num_steps);
+    return fail(GLOM_B200_ERR_INVALID, "%s: first_step and num_steps must be >= 0 (got %d, %d)", fn, first_step, num_steps);
   if (reinterpret_cast<uintptr_t>(remaining_out) % 4)
-    return fail(GLOM_B200_ERR_INVALID, "settle_queue: remaining_out must be 4-byte aligned");
+    return fail(GLOM_B200_ERR_INVALID, "%s: remaining_out must be 4-byte aligned", fn);
   if (int r = check_queue(a, &g, &ql, &di)) return r;
   const WorkspaceLayout& wl = ql.settle.fwd;
   const PackedLayout pl = packed_layout(g.d, g.L, GLOM_B200_BF16);
@@ -439,7 +451,7 @@ static int queue_run(const QueueArgs& a, const void* packed_weights, int first_s
     if (e == cudaSuccess)
       e = launch_queue_fill(g, q, a.tokens, a.pos, a.state_in, a.init_levels, a.state_out, slab[p], sb[p], sp[p], nsq[p], xb, st,
                             &g_launches, &g_prof);
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle_queue slot launch before step %d: %s", t, cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "%s slot launch before step %d: %s", fn, t, cudaGetErrorString(e));
     if (num_steps == 0) break;
     Bf16Buffers b{};
     b.s32_in = slab[p]; b.s32_out = slab[p ^ 1]; b.s32_in_bcast = 0;
@@ -458,15 +470,15 @@ static int queue_run(const QueueArgs& a, const void* packed_weights, int first_s
     b.frozen = frozen; b.block_frozen = block_frozen; b.dsq_out = dsq; b.block_fresh = q.block_fresh;
     char msg[400] = "";
     const int r = step_bf16(g, b, t, g_encode, di.sms, st, &g_launches, msg, sizeof(msg), &g_prof);
-    if (r) return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "settle_queue step %d: %s", t, msg);
+    if (r) return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "%s step %d: %s", fn, t, msg);
     e = launch_settle_converge(g, t + 1, a.tol, dsq, b.nsq_out, frozen, block_frozen,
                                reinterpret_cast<unsigned int*>(ws + ql.settle.done_off),
                                reinterpret_cast<float*>(ws + ql.settle.level_q_off), a.steps_out, st, &g_launches, &q);
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle_queue convergence launch after step %d: %s", t, cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "%s convergence launch after step %d: %s", fn, t, cudaGetErrorString(e));
   }
   if (remaining_out) {
     const cudaError_t e = cudaMemcpyAsync(remaining_out, q.unfinished, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle_queue count copy: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "%s count copy: %s", fn, cudaGetErrorString(e));
     ++g_launches;
   }
   g_err[0] = 0;
@@ -614,19 +626,23 @@ static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, co
 }
 
 // Glom.settle_queue: N images through `slots` batch slots, see include/glom_b200.h
-GLOM_B200_API int glom_b200_settle_queue_workspace_bytes(const glom_b200_cfg* cfg, int slots, int max_iters, size_t* out_bytes) {
-  if (int r = check_queue_sizes(cfg, 1, slots, max_iters)) return r;
+static int queue_workspace_bytes(const QueueMode& m, const glom_b200_cfg* cfg, int slots, int max_iters, size_t* out_bytes) {
+  if (int r = check_queue_sizes(m, cfg, 1, 1, slots, max_iters)) return r;
   if (!out_bytes) return fail(GLOM_B200_ERR_INVALID, "out_bytes is NULL");
   *out_bytes = queue_layout(make_geometry(cfg, slots), max_iters).total;
   return 0;
+}
+
+GLOM_B200_API int glom_b200_settle_queue_workspace_bytes(const glom_b200_cfg* cfg, int slots, int max_iters, size_t* out_bytes) {
+  return queue_workspace_bytes(kQueue, cfg, slots, max_iters, out_bytes);
 }
 
 GLOM_B200_API int glom_b200_settle_queue_begin(const glom_b200_cfg* cfg, const float* tokens, const float* pos,
                                                const float* state_in, const float* init_levels, float* state_out,
                                                int32_t* steps_out, int images, int slots, int max_iters, float tol,
                                                void* workspace, size_t workspace_bytes, void* stream) {
-  return queue_begin({cfg, tokens, pos, state_in, init_levels, state_out, steps_out, images, slots, max_iters, tol, workspace,
-                      workspace_bytes, stream});
+  return queue_begin({kQueue, cfg, tokens, pos, state_in, init_levels, state_out, steps_out, images, 1, slots, max_iters, tol,
+                      workspace, workspace_bytes, stream});
 }
 
 GLOM_B200_API int glom_b200_settle_queue_run(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
@@ -634,8 +650,30 @@ GLOM_B200_API int glom_b200_settle_queue_run(const glom_b200_cfg* cfg, const voi
                                              float* state_out, int32_t* steps_out, int images, int slots, int max_iters,
                                              float tol, void* workspace, size_t workspace_bytes, void* stream, int first_step,
                                              int num_steps, int32_t* remaining_out) {
-  return queue_run({cfg, tokens, pos, state_in, init_levels, state_out, steps_out, images, slots, max_iters, tol, workspace,
-                    workspace_bytes, stream}, packed_weights, first_step, num_steps, remaining_out);
+  return queue_run({kQueue, cfg, tokens, pos, state_in, init_levels, state_out, steps_out, images, 1, slots, max_iters, tol,
+                    workspace, workspace_bytes, stream}, packed_weights, first_step, num_steps, remaining_out);
+}
+
+// Glom.settle_video: S streams of F frames through `slots` batch slots, see include/glom_b200.h
+GLOM_B200_API int glom_b200_settle_video_workspace_bytes(const glom_b200_cfg* cfg, int slots, int max_iters, size_t* out_bytes) {
+  return queue_workspace_bytes(kVideo, cfg, slots, max_iters, out_bytes);
+}
+
+GLOM_B200_API int glom_b200_settle_video_begin(const glom_b200_cfg* cfg, const float* tokens, const float* pos,
+                                               const float* state_in, const float* init_levels, float* state_out,
+                                               int32_t* steps_out, int streams, int frames, int slots, int max_iters,
+                                               float tol, void* workspace, size_t workspace_bytes, void* stream) {
+  return queue_begin({kVideo, cfg, tokens, pos, state_in, init_levels, state_out, steps_out, streams, frames, slots, max_iters,
+                      tol, workspace, workspace_bytes, stream});
+}
+
+GLOM_B200_API int glom_b200_settle_video_run(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
+                                             const float* pos, const float* state_in, const float* init_levels,
+                                             float* state_out, int32_t* steps_out, int streams, int frames, int slots,
+                                             int max_iters, float tol, void* workspace, size_t workspace_bytes, void* stream,
+                                             int first_step, int num_steps, int32_t* remaining_out) {
+  return queue_run({kVideo, cfg, tokens, pos, state_in, init_levels, state_out, steps_out, streams, frames, slots, max_iters,
+                    tol, workspace, workspace_bytes, stream}, packed_weights, first_step, num_steps, remaining_out);
 }
 
 static int tok_kp(int patch) { return (3 * patch * patch + 63) / 64 * 64; }

@@ -1,7 +1,8 @@
 // Glom.settle on CUDA cores: the per-image stopping rule applied after every step, and the final gather of the images
 // whose last state sits in the workspace's half of the ping-pong.  Also the per-image step counts of
 // glom_b200_forward_steps: the flags of each step from the given counts, and the return_all fill of stopped images' slabs.
-// And Glom.settle_queue's slot kernels: queue initialisation, the slot schedule and the slot fill of every step.
+// And the slot kernels of Glom.settle_queue and Glom.settle_video: queue initialisation, the slot schedule and the slot
+// fill of every step.
 #include "engine.h"
 #include "prep_state.cuh"
 #include "ptx.cuh"
@@ -203,6 +204,9 @@ cudaError_t launch_steps_fill(const Geometry& g, int max_steps, const int32_t* s
 // slab t & 1, the shadows and norm partials in buffer t & 1, as in settle.  A slot whose image stops after step t-1 hands
 // that image's final state (slab t & 1) to state_out in the fill of step t, which then writes the next image's S_0 over
 // it; K1 recomputes group 0 for the blocks that admitted an image (block_fresh), K3 and K2 skip frozen slots as in settle.
+// Glom.settle_video runs the same kernels with q.frames = F > 1: the images are the frames i = stream * F + f, a slot
+// whose frame f < F - 1 stops takes frame f + 1 of its own stream, and that frame's S_0 is the slot's own S_k (the
+// settle_queue call is the case F = 1, where no slot continues).
 
 template <typename... Params, typename... Args>
 static cudaError_t launch_pdl(void (*kernel)(Params...), dim3 grid, cudaStream_t st, Args... args) {
@@ -237,38 +241,42 @@ cudaError_t launch_queue_init(const Geometry& g, const QueueSlots& q, int* froze
   return launch_pdl(queue_init_kernel, dim3(1), st, g.B, (g.rows + 255) / 256, q, frozen, block_frozen, done);
 }
 
-// One block, before a step.  The open slots (frozen: their image stopped, or empty) are ranked in slot order by a
-// block-wide count; open slot number k takes queued image head + k while there is one (and `admit`), so the assignment
-// does not depend on timing.  An open slot with a pending image hands it over to the fill (gather_img).  Then the
-// per-256-row-block flags: block_frozen = every slot of the block is frozen, block_fresh = one of them took an image.
+// One block, before a step.  The open slots (frozen: their image stopped, or empty) hand a pending image over to the fill
+// (gather_img).  With `admit`, an open slot whose frame f < F - 1 stopped takes frame f + 1 of the same stream; the other
+// open slots are ranked in slot order by a block-wide count, and number k takes frame 0 of queued stream head + k while
+// there is one, so the assignment does not depend on timing.  Then the per-256-row-block flags: block_frozen = every slot
+// of the block is frozen, block_fresh = one of them took a frame.
 __global__ void __launch_bounds__(SETTLE_THREADS)
 queue_schedule_kernel(int n, int B, int rows, int admit, QueueSlots q, int* frozen, int* block_frozen) {
   pdl_launch_dependents();
   pdl_wait();                                       // the previous step's convergence launch has set the flags
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int streams = q.images / q.frames;
   __shared__ int wsum[SETTLE_THREADS / 32];
   int head = *q.head;
   for (int base = 0; base < B; base += SETTLE_THREADS) {
     const int s = base + tid;
     const bool open = s < B && frozen[s];
-    const unsigned m = __ballot_sync(0xffffffffu, open);
+    const int gi = open && q.pending[s] ? q.slot_img[s] : -1;
+    const bool next = admit && gi >= 0 && gi % q.frames != q.frames - 1;
+    const unsigned m = __ballot_sync(0xffffffffu, open && !next);
     if (lane == 0) wsum[warp] = __popc(m);
     __syncthreads();
     int before = 0, total = 0;
     for (int w = 0; w < SETTLE_THREADS / 32; ++w) { before += w < warp ? wsum[w] : 0; total += wsum[w]; }
     if (open) {
-      q.gather_img[s] = q.pending[s] ? q.slot_img[s] : -1;
+      q.gather_img[s] = gi;
       q.pending[s] = 0;
-      const int img = head + before + __popc(m & ((1u << lane) - 1u));
-      const bool take = admit && img < q.images;
-      q.slot_img[s] = take ? img : -1;
+      const int stream = head + before + __popc(m & ((1u << lane) - 1u));
+      const bool take = next || (admit && stream < streams);
+      q.slot_img[s] = next ? gi + 1 : take ? stream * q.frames : -1;
       q.fresh[s] = take;
       if (take) { q.age[s] = 0; frozen[s] = 0; }
     } else if (s < B) {
       q.gather_img[s] = -1;
       q.fresh[s] = 0;
     }
-    if (admit) head = min(head + total, q.images);
+    if (admit) head = min(head + total, streams);
     __syncthreads();                                // wsum is reused
   }
   if (tid == 0) *q.head = head;
@@ -293,7 +301,10 @@ constexpr int FILL_ROWS = 8;                        // rows of one slot per bloc
 
 // Grid (ceil(n / FILL_ROWS), B), after the schedule.  Block (c, s) covers rows c*FILL_ROWS.. of slot s: first the copy
 // of the handed-over image's final state from the slab into state_out, then (admitted slot) the admitted image's S_0
-// into the same slab rows with prep_state_row, one warp per (row, level), and its token rows cast to bf16.
+// into the same slab rows with prep_state_row, one warp per (row, level), and its token rows cast to bf16.  Frame 0 of a
+// stream starts from state_in[stream] or init_levels.  A later frame's S_0 is the previous frame's final state, already
+// in the slab rows: prep_state_row recomputes the shadows and norm partials from it in place, as the prologue of a
+// settle call given that state as `levels` does.
 __global__ void __launch_bounds__(SETTLE_THREADS)
 queue_fill_kernel(int n, int L, int d, int nparts, int part_w, QueueSlots q, const float* __restrict__ tokens,
                   const float* __restrict__ pos, const float* __restrict__ state_in, const float* __restrict__ init_levels,
@@ -311,13 +322,14 @@ queue_fill_kernel(int n, int L, int d, int nparts, int part_w, QueueSlots q, con
   }
   if (!fresh) return;                               // block-uniform
   __syncthreads();                                  // the handed-over state is read before S_0 replaces it
-  const int img = q.slot_img[s];
+  const int img = q.slot_img[s], stream = img / q.frames, cont = img % q.frames != 0;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int w = warp; w < ni * L; w += SETTLE_THREADS / 32) {
     const int i = i0 + w / L, l = w % L;
     const size_t r = (size_t)s * n + i;
-    const float* src = state_in ? state_in + (((size_t)img * n + i) * L + l) * d : init_levels + (size_t)l * d;
-    prep_state_row(lane, l, d, nparts, part_w, src, pos + (size_t)i * d, slab + (r * L + l) * d, sb + (r * L + l) * d,
+    float* row = slab + (r * L + l) * d;
+    const float* src = cont ? row : state_in ? state_in + (((size_t)stream * n + i) * L + l) * d : init_levels + (size_t)l * d;
+    prep_state_row(lane, l, d, nparts, part_w, src, pos + (size_t)i * d, cont ? nullptr : row, sb + (r * L + l) * d,
                    l >= 1 ? sp + (r * (L - 1) + (l - 1)) * d : nullptr, nsq + (r * L + l) * nparts);
   }
   const float4* tk = reinterpret_cast<const float4*>(tokens + ((size_t)img * n + i0) * d);

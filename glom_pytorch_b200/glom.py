@@ -31,7 +31,7 @@ bf16 operands, fp32 accumulate and fp32 state -- the arithmetic of the reference
 kernel tile, of the same step in float64 from the same state; tests/test_cuda_core_oracle.py).  The fp32 engine needs
 dim + n <= 3632 (its consensus keeps a block's 16 query rows and logits in shared memory).
 """
-from math import sqrt
+from math import prod, sqrt
 
 import operator
 import weakref
@@ -606,11 +606,54 @@ class Glom(nn.Module):
         The tokens of all N images are computed up front by one tokeniser call: N * n * d * 4 bytes (512 MB for 1024
         images at dim 512 and 256 patches).  The call synchronises once per ``max_iters`` steps to read the number of
         unfinished images (4 bytes), so it cannot be captured in a CUDA graph."""
+        tol, max_iters, slots = self._slot_args("settle_queue", img, levels, tol, max_iters, slots)
+        num, n = self._check_input(img, levels)
+        self._resume = None
+        tokens = self.tokens(img)                                           # (:114) all N images, one engine call
+        return self._settle_slots("settle_queue", tokens, levels, (num,), n, tol, max_iters, min(slots, num))
+
+    def settle_video(self, frames, tol, max_iters=None, levels=None, *, slots=32):
+        """Settle S video streams frame by frame -> ``(levels, steps)``, each frame starting from the levels its stream's
+        previous frame settled at.  ``frames`` is (S, F, 3, H, W); ``levels`` (S, n, L, d) or None (``init_levels``) is
+        the start of each stream's frame 0.  Result: ``levels`` (S, F, n, L, d) fp32 and ``steps`` (S, F) int32 on the GPU.
+
+        Contract: ``(levels[s, f], steps[s, f])`` are bit-identical to the host loop
+        ``lv = levels; for f in range(F): lv, st = settle(frames[:, f], tol, max_iters, levels=lv)`` at index s, and so
+        to ``forward(frames[:, f], iters=steps[:, f], levels=<frame f-1's levels>)[s]``.  So F = 1 is ``settle_queue`` on
+        ``frames[:, 0]``, and a long clip can be settled in chunks: ``settle_video(frames[:, k:], levels=out[:, k-1])``
+        continues ``out = settle_video(frames[:, :k])`` with the same bits as one call over all F frames.
+
+        The engine keeps ``slots`` streams in flight (clipped to S).  When a frame stops, its slot takes the stream's
+        next frame on the next step, on the GPU, starting from the state the slot already holds; after the last frame it
+        takes the next queued stream.  A static stream thus runs ahead of one with a cut instead of waiting for it at
+        every frame.  Arguments, errors and the stopping rule are those of ``settle_queue``: bf16 engine only, inference
+        only, ``max_iters >= 1`` (None = 2L), NaN ``tol`` rejected, ``slots >= 1``; no ``return_all`` or
+        ``differentiable``.  The tokens of all S * F frames are computed up front by one tokeniser call, and the call
+        reads the number of unfinished frames once per ``max_iters`` steps (4 bytes)."""
+        tol, max_iters, slots = self._slot_args("settle_video", frames, levels, tol, max_iters, slots)
+        p = self.patch_size
+        if frames.dim() != 5 or frames.shape[2] != 3 or frames.shape[3] % p or frames.shape[4] % p:
+            raise RuntimeError(f"frames {tuple(frames.shape)} is not (S, F, 3, H, W) with H, W multiples of {p}")
+        num, num_frames = frames.shape[0], frames.shape[1]
+        if num < 1 or num_frames < 1:
+            raise RuntimeError(f"frames {tuple(frames.shape)} needs at least one stream and one frame")
+        flat = frames.reshape((num * num_frames,) + tuple(frames.shape[2:]))
+        _, n = self._check_input(flat)
+        if levels is not None and tuple(levels.shape) != (num, n, self.levels, self.dim):
+            raise RuntimeError(f"levels must have shape {(num, n, self.levels, self.dim)}, got {tuple(levels.shape)}")
+        self._resume = None
+        tokens = self.tokens(flat)                                          # (:114) all S * F frames, one engine call
+        out, steps = self._settle_slots("settle_video", tokens, levels, (num, num_frames), n, tol, max_iters,
+                                        min(slots, num))
+        return out.view(num, num_frames, n, self.levels, self.dim), steps.view(num, num_frames)
+
+    def _slot_args(self, name, img, levels, tol, max_iters, slots):
+        """The argument checks of settle_queue / settle_video -> (tol, max_iters, slots)."""
         if self.precision != "bf16":
-            raise RuntimeError("Glom.settle_queue needs precision='bf16' (the fp32 engine has no early stopping)")
+            raise RuntimeError(f"Glom.{name} needs precision='bf16' (the fp32 engine has no early stopping)")
         _require_cuda(img)
         if self._needs_grad(img, levels):
-            raise RuntimeError("Glom.settle_queue is inference only: call it under torch.no_grad() / torch.inference_mode() "
+            raise RuntimeError(f"Glom.{name} is inference only: call it under torch.no_grad() / torch.inference_mode() "
                                "or with parameters and inputs that do not require grad")
         max_iters = self.levels * 2 if max_iters is None else int(max_iters)
         if max_iters < 1:
@@ -621,11 +664,14 @@ class Glom(nn.Module):
         slots = int(slots)
         if slots < 1:
             raise ValueError(f"slots must be >= 1, got {slots}")
-        num, n = self._check_input(img, levels)
-        self._resume = None
-        slots = min(slots, num)
-        tokens = self.tokens(img)                                           # (:114) all N images, one engine call
+        return tol, max_iters, slots
+
+    def _settle_slots(self, name, tokens, levels, counts, n, tol, max_iters, slots):
+        """The host loop of glom_b200_<name>_begin / _run: settle_queue with counts = (N,), settle_video with counts =
+        (S, F) and tokens stream-major.  -> (out (prod(counts), n, L, d), steps (prod(counts),))."""
         device = tokens.device
+        images = prod(counts)
+        begin, run = getattr(_native, name + "_begin"), getattr(_native, name + "_run")
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
             pos = self.pos_emb.weight[:n].detach().to(torch.float32).contiguous()
@@ -634,20 +680,20 @@ class Glom(nn.Module):
             state_ptr = None if state_in is None else state_in.data_ptr()
             cfg = self.engine_cfg(n)
             packed = self._packed_weights(cfg, device, stream)
-            out = torch.empty(num, n, self.levels, self.dim, dtype=torch.float32, device=device)
-            steps = torch.empty(num, dtype=torch.int32, device=device)
+            out = torch.empty(images, n, self.levels, self.dim, dtype=torch.float32, device=device)
+            steps = torch.empty(images, dtype=torch.int32, device=device)
             remaining = torch.empty(1, dtype=torch.int32, device=device)
-            ws = self._get_workspace(_native.settle_queue_workspace_bytes(cfg, slots, max_iters), device)
-            args = (tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(), out.data_ptr(), steps.data_ptr(), num,
-                    slots, max_iters, tol, ws.data_ptr(), ws.numel(), stream)
-            _native.settle_queue_begin(cfg, *args)
+            ws = self._get_workspace(getattr(_native, name + "_workspace_bytes")(cfg, slots, max_iters), device)
+            args = (tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(), out.data_ptr(), steps.data_ptr(),
+                    *counts, slots, max_iters, tol, ws.data_ptr(), ws.numel(), stream)
+            begin(cfg, *args)
             launches, first = _native.last_launch_count(), 0
             while True:
-                _native.settle_queue_run(cfg, packed.data_ptr(), *args, first, max_iters, remaining.data_ptr())
+                run(cfg, packed.data_ptr(), *args, first, max_iters, remaining.data_ptr())
                 launches += _native.last_launch_count()
                 first += max_iters
                 if int(remaining.item()) == 0:                              # the only host read
                     break
-            _native.settle_queue_run(cfg, packed.data_ptr(), *args, first, 0, None)   # the last stopped images' states
+            run(cfg, packed.data_ptr(), *args, first, 0, None)              # the last stopped images' states
             self.last_launches = launches + _native.last_launch_count() + getattr(self, "_tok_launches", 0)
         return out, steps

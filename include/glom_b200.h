@@ -195,6 +195,31 @@ GLOM_B200_API int glom_b200_settle_queue_run(const glom_b200_cfg* cfg, const voi
                                              float tol, void* workspace, size_t workspace_bytes, void* stream, int first_step,
                                              int num_steps, int32_t* remaining_out);
 
+/* Video streams settled frame by frame through fixed batch slots (Glom.settle_video).  bf16 engine only.  `streams` = S
+ * streams of `frames` = F frames each; frame i = s * F + f is an image of the queue above.  A slot holds one stream at a
+ * time: on the step after its frame f < F - 1 stops, it takes frame f + 1 of the same stream, whose S_0 is frame f's
+ * final state; after the stream's last frame it takes frame 0 of the next queued stream (open slots take queued streams
+ * in slot order).  Frame (s, f)'s result is bit-identical to glom_b200_settle on the S-stream batch of frame f, started
+ * from frame f - 1's results (frame 0: from state_in or init_levels): state_out[s * F + f] = S_k, steps_out[s * F + f] = k.
+ *   tokens (S * F, n, d) fp32, stream-major (all frames, tokenised up front);  pos (n, d);  state_in (S, n, L, d), the
+ *   start of each stream's frame 0, or NULL with init_levels (L, d) broadcast;  state_out (S * F, n, L, d) fp32, must not
+ *   alias state_in;  steps_out (S * F) int32 device.
+ * _begin and _run, the host loop, the workspace (the same size as settle_queue's for the same slots and max_iters) and the
+ * unfinished count (of frames) are those of glom_b200_settle_queue_*.  Within max_iters steps every frame in flight
+ * stops, so every round of the loop makes progress.  Argument errors (precision fp32, streams < 1, frames < 1,
+ * streams * frames >= 2^31, slots < 1, max_iters < 1, NaN tol, NULL or misaligned steps_out, NULL or misaligned tensor
+ * pointers, state_out aliasing state_in) are reported before any device query. */
+GLOM_B200_API int glom_b200_settle_video_workspace_bytes(const glom_b200_cfg* cfg, int slots, int max_iters, size_t* out_bytes);
+GLOM_B200_API int glom_b200_settle_video_begin(const glom_b200_cfg* cfg, const float* tokens, const float* pos,
+                                               const float* state_in, const float* init_levels, float* state_out,
+                                               int32_t* steps_out, int streams, int frames, int slots, int max_iters,
+                                               float tol, void* workspace, size_t workspace_bytes, void* stream);
+GLOM_B200_API int glom_b200_settle_video_run(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
+                                             const float* pos, const float* state_in, const float* init_levels,
+                                             float* state_out, int32_t* steps_out, int streams, int frames, int slots,
+                                             int max_iters, float tol, void* workspace, size_t workspace_bytes, void* stream,
+                                             int first_step, int num_steps, int32_t* remaining_out);
+
 /* Tokeniser, the step before the loop: replaces image_to_tokens
  * (glom_pytorch.py:94-97, call :114): patchify 'b c (h p1) (w p2) -> b (h w) (p1 p2 c)'
  * fused with the Linear(3*p*p -> d).
