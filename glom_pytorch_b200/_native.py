@@ -67,6 +67,9 @@ SIGNATURES = {
     "glom_b200_backward": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _i32, _i32, _vp, _sz, _vp]),
     "glom_b200_backward_steps": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _vp, _i32, _i32, _vp, _sz, _vp]),
     "glom_b200_backward_ex": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _vp, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "glom_b200_backward_implicit_workspace_bytes": (_i32, [_CFG, _i32, _SZP]),
+    "glom_b200_backward_implicit": (_i32, [_CFG, _W, _vp, _vp, _vp, _vp, _G, _i32, _i32, _f32, _i32, _vp, _vp, _vp, _sz,
+                                           _vp]),
     "glom_b200_tokenize_backward_workspace_bytes": (_i32, [_i32, _i32, _i32, _i32, _i32, _SZP]),
     "glom_b200_tokenize_backward": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _sz, _vp]),
     "glom_b200_tokenize_backward_ex": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _sz,
@@ -287,6 +290,23 @@ def backward(cfg, weight_ptrs, tokens_ptr, pos_ptr, states_ptr, grad_out_ptr, gr
                                           grad_out_ptr, ctypes.byref(g), batch, steps_ptr, iters, int(grad_all), ws_ptr,
                                           ws_bytes, stream)
     check(rc)
+
+
+def backward_implicit_workspace_bytes(cfg, batch):
+    return _bytes("glom_b200_backward_implicit_workspace_bytes", ctypes.byref(cfg), batch)
+
+
+def backward_implicit(cfg, weight_ptrs, tokens_ptr, pos_ptr, state_ptr, grad_out_ptr, grad_ptrs, batch, adjoint_iters,
+                      adjoint_tol, adjoint_steps_ptr, adjoint_q_ptr, ws_ptr, ws_bytes, stream, deterministic=False):
+    """glom_b200_backward_implicit: the implicit gradients of the settled state at state_ptr given its cotangent;
+    grad_ptrs as in backward, with d_state0 / d_init absent or None.  adjoint_steps_ptr -> (batch,) int32 device words,
+    adjoint_q_ptr -> (batch, L) fp32 device words or None."""
+    w = WeightsRef(ctypes.sizeof(WeightsRef), *weight_ptrs)
+    g = Grads(ctypes.sizeof(Grads), *[grad_ptrs.get(k) for k, _ in Grads._fields_[1:]])
+    check(load().glom_b200_backward_implicit(ctypes.byref(cfg), ctypes.byref(w), tokens_ptr, pos_ptr, state_ptr,
+                                             grad_out_ptr, ctypes.byref(g), batch, adjoint_iters, float(adjoint_tol),
+                                             int(bool(deterministic)), adjoint_steps_ptr, adjoint_q_ptr, ws_ptr, ws_bytes,
+                                             stream))
 
 
 def tokenize_backward_workspace_bytes(batch, h, w, patch, need_d_img):

@@ -9,6 +9,9 @@
 // are small element-wise / row-reduction kernels.  With precision fp32 (or dim % 256 != 0) this file is the whole
 // backward; with precision bf16 `backward_run` sends the MLP and consensus GEMMs to the tensor cores (`mlp_backward_tc`,
 // `attn_bwd_gemm_tc`) and keeps the softmax / normalisation / bias reductions here.
+// Also the implicit gradients of a settled state (`backward_implicit_run`): the adjoint iteration u = g + J^T u at S*,
+// one-step backward_run calls that linearise once and then run only the cotangent-dependent stages, each image stopped
+// by settle's convergence kernel, and one parameter pass.
 #include "engine.h"
 #include "ptx.cuh"
 
@@ -593,18 +596,21 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
       CK(gemm_f32(q, 1, st, launches));
       gelu_bwd_kernel<<<nblk((size_t)R * h4), 256, 0, st>>>((size_t)R * h4, pre, hb, dh);   // dh := dpre
       CKL();
-      // dW2 += DY^T h                                     (d x 4d)
-      q = GemmF32{d, h4, R, 1, Mat{DY.p, 1, ld, 0, 0}, Mat{hb, h4, 1, 0, 0}, MatOut{dw2 + (size_t)l * d * h4, h4, 1, 0, 0}, 1.f, 1.f, nullptr};
-      CK(gemm_f32(q, 1, st, launches));
-      CK(colsum(a.deterministic != 0, R, d, ld, DY.p, db2 + (size_t)l * d, nullptr, 0, nullptr, 0, 1, st, launches));
-      // dW1 += dpre^T X                                   (4d x d)
-      q = GemmF32{h4, d, R, 1, Mat{dh, 1, h4, 0, 0}, Mat{X.p, X.s_row, 1, 0, 0}, MatOut{dw1 + (size_t)l * h4 * d, d, 1, 0, 0}, 1.f, 1.f, nullptr};
-      CK(gemm_f32(q, 1, st, launches));
-      CK(colsum(a.deterministic != 0, R, h4, h4, dh, db1 + (size_t)l * h4, nullptr, 0, nullptr, 0, 1, st, launches));
+      if (!a.state_only) {
+        // dW2 += DY^T h                                     (d x 4d)
+        q = GemmF32{d, h4, R, 1, Mat{DY.p, 1, ld, 0, 0}, Mat{hb, h4, 1, 0, 0}, MatOut{dw2 + (size_t)l * d * h4, h4, 1, 0, 0}, 1.f, 1.f, nullptr};
+        CK(gemm_f32(q, 1, st, launches));
+        CK(colsum(a.deterministic != 0, R, d, ld, DY.p, db2 + (size_t)l * d, nullptr, 0, nullptr, 0, 1, st, launches));
+        // dW1 += dpre^T X                                   (4d x d)
+        q = GemmF32{h4, d, R, 1, Mat{dh, 1, h4, 0, 0}, Mat{X.p, X.s_row, 1, 0, 0}, MatOut{dw1 + (size_t)l * h4 * d, d, 1, 0, 0}, 1.f, 1.f, nullptr};
+        CK(gemm_f32(q, 1, st, launches));
+        CK(colsum(a.deterministic != 0, R, h4, h4, dh, db1 + (size_t)l * h4, nullptr, 0, nullptr, 0, 1, st, launches));
+      }
       // dX = dpre W1                                      (R x d)
       q = GemmF32{R, d, h4, 1, Mat{dh, h4, 1, 0, 0}, Mat{W1, d, 1, 0, 0}, MatOut{dx, d, 1, 0, 0}, 1.f, 0.f, nullptr};
       CK(gemm_f32(q, 1, st, launches));
       if (net == 0 && l == 0) {
+        if (a.state_only) continue;     // the tokens are no state
         add_kernel<<<nblk((size_t)R * d), 256, 0, st>>>((size_t)R * d, dx, a.d_tokens);
         CKL();
       } else if (net == 0) {
@@ -613,6 +619,7 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
       } else {
         add_into_level_kernel<<<nblk((size_t)R * d), 256, 0, st>>>(R, L, d, l + 1, dx, ds);
         CKL();
+        if (a.state_only) continue;
         pos_grad_kernel<<<nblk((size_t)n * d), 256, 0, st>>>(g.B, n, d, dx, a.d_pos);
         CKL();
       }
@@ -620,7 +627,7 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
   }
 
   // ---- consensus attention (:56-73), all (image, level) problems batched (fp32 path)
-  if (!attn_on_tc) {
+  if (!attn_on_tc && !a.skip_attn) {
     float* khat = reinterpret_cast<float*>(ws + wl.khat_off);
     float* dkhat = reinterpret_cast<float*>(ws + wl.dkhat_off);
     float* rnorm = reinterpret_cast<float*>(ws + wl.rnorm_off);
@@ -729,8 +736,7 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
   float* gs = reinterpret_cast<float*>(ws + wl.gs_off);
   MlpBwdTc m{};
   if (tc) {
-    __nv_bfloat16* xb = reinterpret_cast<__nv_bfloat16*>(ws + wl.xb_off);
-    m.xb = xb;
+    m.xb = reinterpret_cast<__nv_bfloat16*>(ws + wl.xb_off);
     m.sb = reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off);
     m.sp = reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off);
     m.gsb = reinterpret_cast<__nv_bfloat16*>(ws + wl.gsb_off);
@@ -747,12 +753,15 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
     m.deterministic = a.deterministic;
     m.dx_td = reinterpret_cast<float*>(ws + wl.dkhat_off);
     m.b1_part = reinterpret_cast<float*>(ws + wl.b1part_off);
+    m.skip_pre = a.relin; m.skip_dw = a.state_only;
+  }
+  if (tc && !a.relin) {     // the weights and tokens of this call (relin: still in the workspace)
     pack_bwd_weights_kernel<<<sm_count() * 8, 256, 0, st>>>(g.d, g.L, a.bu_w1, a.bu_b1, a.bu_w2, a.td_w1, a.td_b1, a.td_w2,
                                                      const_cast<__nv_bfloat16*>(m.w1p), const_cast<__nv_bfloat16*>(m.w2t),
                                                      const_cast<__nv_bfloat16*>(m.w1t), const_cast<float*>(m.b1p));
     CKLI();
     const size_t n4 = (size_t)g.rows * g.d / 4;
-    cast_bf16_rows<<<nblk(n4), 256, 0, st>>>(n4, a.tokens, xb);
+    cast_bf16_rows<<<nblk(n4), 256, 0, st>>>(n4, a.tokens, const_cast<__nv_bfloat16*>(m.xb));
     CKLI();
     if (g.rows % 128) {     // rows of the last 128-row block beyond R are read as K entries of the dW GEMMs: keep them zero
       CKI(cudaMemsetAsync(m.h, 0, wl.blocked_bytes, st));
@@ -773,14 +782,19 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
     CKI(backward_step(g, a, s_t, gin, gextra, ds, ws, wl, tc, attn_tc, steps, t, kept != nullptr, st,
                       launches));   // scale (+ the fp32 MLP / attention backward)
     if (tc) {
-      bwd_shadows_kernel<<<nblk(state / 4), 256, 0, st>>>(g.rows, g.n, g.L, g.d, s_t, gs, a.pos,
-                                                          const_cast<__nv_bfloat16*>(m.sb), const_cast<__nv_bfloat16*>(m.sp),
-                                                          const_cast<__nv_bfloat16*>(m.gsb), kept, t);
+      if (a.relin) {      // sb / sp hold this state's shadows: only the cotangent changes (frozen rows: gs = 0 -> gsb = 0)
+        cast_bf16_rows<<<nblk(state / 4), 256, 0, st>>>(state / 4, gs, const_cast<__nv_bfloat16*>(m.gsb));
+      } else {
+        bwd_shadows_kernel<<<nblk(state / 4), 256, 0, st>>>(g.rows, g.n, g.L, g.d, s_t, gs, a.pos,
+                                                            const_cast<__nv_bfloat16*>(m.sb), const_cast<__nv_bfloat16*>(m.sp),
+                                                            const_cast<__nv_bfloat16*>(m.gsb), kept, t);
+      }
       CKLI();
       // ---- consensus attention backward: the five (n x n x d) GEMM families on tensor cores, softmax in fp32.  With
       // per-image step counts, the problems / rows of images frozen at step t are skipped in every launch (their
       // contribution to ds is an exact zero); the buffers they would have written are left stale and read by no one.
-      if (attn_tc) {
+      // relin: khat / rnorm / khat_b and the probabilities A / a_b of this state are already there
+      if (attn_tc && !a.skip_attn) {
         float* khat = reinterpret_cast<float*>(ws + wl.khat_off);
         float* dkhat = reinterpret_cast<float*>(ws + wl.dkhat_off);
         float* rnorm = reinterpret_cast<float*>(ws + wl.rnorm_off);
@@ -793,13 +807,16 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
         const float scale = 1.0f / sqrtf((float)d);
         const int wblocks = (g.rows * g.L * 32 + 255) / 256, rblocks = (Z * n * 32 + 255) / 256;
         const FrozenRows frozen{steps, t, n * g.L};
-        normalize_rows_kernel<<<wblocks, 256, 0, st>>>(g.rows * g.L, d, s_t, khat, rnorm, khat_b, frozen);
-        CKLI();
-        // logits = Q Khat^T (scaled inside the softmax), dA = dC V^T
-        if (int r = attn_bwd_gemm_tc(g, m.sb, 1, 0, khat_b, 1, 0, n, d, 0, A, steps, t, enc, num_sms, st, launches, err,
-                                     errlen)) return r;
-        attn_softmax_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, a_b, frozen);
-        CKLI();
+        if (!a.relin) {
+          normalize_rows_kernel<<<wblocks, 256, 0, st>>>(g.rows * g.L, d, s_t, khat, rnorm, khat_b, frozen);
+          CKLI();
+          // logits = Q Khat^T (scaled inside the softmax)
+          if (int r = attn_bwd_gemm_tc(g, m.sb, 1, 0, khat_b, 1, 0, n, d, 0, A, steps, t, enc, num_sms, st, launches, err,
+                                       errlen)) return r;
+          attn_softmax_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, a_b, frozen);
+          CKLI();
+        }
+        // dA = dC V^T
         if (int r = attn_bwd_gemm_tc(g, m.gsb, 1, 0, m.sb, 1, 0, n, d, 0, dA, steps, t, enc, num_sms, st, launches, err,
                                      errlen)) return r;
         attn_softmax_bwd_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, scale, dsim_b,
@@ -816,15 +833,17 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
       m.ds = ds;
       m.steps = steps; m.t = t;
       if (int r = mlp_backward_tc(g, m, enc, num_sms, st, launches, err, errlen)) return r;
-      if (a.deterministic) {     // what the default DH / DX epilogues reduce with atomics, in a fixed order
+      if (a.deterministic && !a.state_only) {     // what the default DH / DX epilogues reduce with atomics, in a fixed order
         bias_partials_kernel<<<(g.G * g.d + 31) / 32, dim3(32, 16), 0, st>>>(g.G, (g.rows + 31) / 32, g.rows, g.n, g.d,
                                                                              m.b1_part, a.d_bu_b1, a.d_td_b1, steps, t);
         CKLI();
+      }
+      if (a.deterministic) {
         dx_td_reduce_kernel<<<g.n * ((g.d / 4 + 31) / 32), dim3(32, 8), 0, st>>>(g.B, g.n, g.L, g.d, m.dx_td, ds, a.d_pos,
                                                                                   steps, t);
         CKLI();
       }
-      CKI(colsum(a.deterministic != 0, g.rows, g.L * g.d, (long long)g.L * g.d, gs, a.d_bu_b2, a.d_td_b2, (g.L - 1) * g.d,
+      if (!a.state_only) CKI(colsum(a.deterministic != 0, g.rows, g.L * g.d, (long long)g.L * g.d, gs, a.d_bu_b2, a.d_td_b2, (g.L - 1) * g.d,
                  steps, t, g.n, st, launches));
     }
     gin = ds;
@@ -844,6 +863,122 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
       CKLI();
     }
   }
+  return 0;
+#undef CKI
+#undef CKLI
+}
+
+// =====================================================================================
+// Implicit gradients through settle: the adjoint iteration u_k = gbar + J^T u_{k-1} at the settled state S*, each image
+// stopped by settle's rule on u, then one parameter pass with cotangent u_K
+// =====================================================================================
+// Before adjoint pass k: the backward's skip vector from the convergence flags, stop[b] = 0 (frozen at step t = 0) for
+// an image whose adjoint has stopped, 1 otherwise
+__global__ void implicit_stop_kernel(int B, const int* __restrict__ frozen, int32_t* __restrict__ stop) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) stop[b] = frozen[b] ? 0 : 1;
+}
+// After the one-step VJP of adjoint pass k (jtu = J^T u_{k-1}): for the rows of running images, u_k = gbar + jtu and the
+// partials |u_k - u_{k-1}|^2, |u_k|^2 per (row, level, part of part_w columns) -- the layout of settle's change / norm
+// partials, for settle_converge_kernel -- in a fixed order: lane c sums its columns c, c + 32, ... of the part in order,
+// then an xor tree.  Rows of stopped images are not touched.  One warp per (row, level)
+__global__ void __launch_bounds__(256) implicit_update_kernel(int nrl, int n, int L, int d, int part_w,
+                                                              const float* __restrict__ gbar, const float* __restrict__ jtu,
+                                                              float* __restrict__ u, float* __restrict__ dsq,
+                                                              float* __restrict__ nsq, const int* __restrict__ frozen) {
+  const int lane = threadIdx.x & 31, nparts = d / part_w, per = part_w / 32;
+  const int warps = (gridDim.x * blockDim.x) >> 5;
+  for (int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < nrl; w += warps) {
+    if (frozen[w / (n * L)]) continue;                // warp-uniform
+    const size_t o = (size_t)w * d;
+    for (int p = 0; p < nparts; ++p) {
+      float a = 0.f, c = 0.f;
+      for (int j = 0; j < per; ++j) {
+        const size_t i = o + (size_t)p * part_w + j * 32 + lane;
+        const float v = gbar[i] + jtu[i], dv = v - u[i];
+        a = fmaf(dv, dv, a);
+        c = fmaf(v, v, c);
+        u[i] = v;
+      }
+#pragma unroll
+      for (int s = 16; s; s >>= 1) {
+        a += __shfl_xor_sync(0xffffffffu, a, s);
+        c += __shfl_xor_sync(0xffffffffu, c, s);
+      }
+      if (lane == 0) { dsq[(size_t)w * nparts + p] = a; nsq[(size_t)w * nparts + p] = c; }
+    }
+  }
+}
+
+ImplicitLayout implicit_layout(const Geometry& g) {
+  ImplicitLayout w{};
+  w.bwd = backward_layout(g, 1);
+  size_t off = w.bwd.total;
+  auto take = [&](size_t bytes) { const size_t o = off; off = align_up(off + bytes, 1024); return o; };
+  const size_t parts = (size_t)g.rows * g.L * g.nparts * 4;
+  w.u_off = take((size_t)g.rows * g.L * g.d * 4);
+  w.dsq_off = take(parts); w.nsq_off = take(parts);
+  w.dtok_off = take((size_t)g.rows * g.d * 4); w.dpos_off = take((size_t)g.n * g.d * 4);
+  w.flags_off = off;
+  w.frozen_off = off; off = align_up(off + (size_t)g.B * 4, 16);
+  w.block_frozen_off = off; off = align_up(off + (size_t)(g.rows + 255) / 256 * 4, 16);
+  w.done_off = off; off = align_up(off + 4, 16);
+  w.level_q_off = off; off = align_up(off + (size_t)g.B * g.L * 4, 16);
+  w.stop_off = off; off += (size_t)g.B * 4;
+  w.flags_bytes = off - w.flags_off;
+  w.total = align_up(off, 1024);
+  return w;
+}
+
+int backward_implicit_run(const Geometry& g, const BackwardArgs& a, int adjoint_iters, float adjoint_tol,
+                          int32_t* adjoint_steps, float* adjoint_q, void* workspace, EncodeTiledFn enc, int num_sms,
+                          cudaStream_t st, int* launches, char* err, size_t errlen) {
+#define CKI(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { snprintf(err, errlen, "backward_implicit: %s", cudaGetErrorString(e_)); return -3; } } while (0)
+#define CKLI() do { if (launches) ++*launches; CKI(cudaGetLastError()); } while (0)
+  const ImplicitLayout il = implicit_layout(g);
+  char* ws = static_cast<char*>(workspace);
+  const size_t state = (size_t)g.rows * g.L * g.d;
+  float* u = reinterpret_cast<float*>(ws + il.u_off);
+  float* dsq = reinterpret_cast<float*>(ws + il.dsq_off);
+  float* nsq = reinterpret_cast<float*>(ws + il.nsq_off);
+  int* frozen = reinterpret_cast<int*>(ws + il.frozen_off);
+  int32_t* stop = reinterpret_cast<int32_t*>(ws + il.stop_off);
+  float* level_q = reinterpret_cast<float*>(ws + il.level_q_off);
+  // a one-step backward_run leaves dL/dS_0 = J^T u in the first slab of its ping-pong
+  const float* jtu = reinterpret_cast<const float*>(ws + il.bwd.ds_off);
+  CKI(cudaMemsetAsync(ws + il.flags_off, 0, il.flags_bytes, st));
+  CKI(cudaMemsetAsync(adjoint_steps, 0, (size_t)g.B * 4, st));
+  CKI(cudaMemcpyAsync(u, a.grad_out, state * 4, cudaMemcpyDeviceToDevice, st));
+  // adjoint passes: dL/dS only, fixed-order reductions, token / pos rows into scratch
+  BackwardArgs p = a;
+  p.grad_out = u;
+  p.d_state0 = p.d_init = nullptr;
+  p.d_tokens = reinterpret_cast<float*>(ws + il.dtok_off);
+  p.d_pos = reinterpret_cast<float*>(ws + il.dpos_off);
+  p.deterministic = 1;
+  p.state_only = 1;
+  p.skip_attn = 0;
+  const int nrl = g.rows * g.L;
+  const int ublocks = nblk((size_t)nrl * 32);
+  for (int k = 1; k <= adjoint_iters; ++k) {
+    p.relin = k > 1;                                 // pass 1 linearises at S*, for every image (none has stopped)
+    implicit_stop_kernel<<<(g.B + 255) / 256, 256, 0, st>>>(g.B, frozen, stop);
+    CKLI();
+    if (int r = backward_run(g, p, 1, 1, 0, stop, workspace, enc, num_sms, st, launches, err, errlen)) return r;
+    implicit_update_kernel<<<ublocks, 256, 0, st>>>(nrl, g.n, g.L, g.d, g.part_w, a.grad_out, jtu, u, dsq, nsq, frozen);
+    CKLI();
+    CKI(launch_settle_converge(g, k, adjoint_tol, dsq, nsq, frozen, reinterpret_cast<int*>(ws + il.block_frozen_off),
+                               reinterpret_cast<unsigned int*>(ws + il.done_off), level_q, adjoint_steps, st, launches));
+  }
+  // parameter pass: one VJP at S* with cotangent u_K for every image; consensus attention has no parameters
+  BackwardArgs q = a;
+  q.grad_out = u;
+  q.d_state0 = q.d_init = nullptr;
+  q.state_only = 0;
+  q.relin = adjoint_iters > 0;
+  q.skip_attn = 1;
+  if (int r = backward_run(g, q, 1, 1, 0, nullptr, workspace, enc, num_sms, st, launches, err, errlen)) return r;
+  if (adjoint_q) CKI(cudaMemcpyAsync(adjoint_q, level_q, (size_t)g.B * g.L * 4, cudaMemcpyDeviceToDevice, st));
   return 0;
 #undef CKI
 #undef CKLI

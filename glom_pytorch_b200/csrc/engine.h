@@ -233,6 +233,15 @@ struct BackwardArgs {
   float *d_bu_w1, *d_bu_b1, *d_bu_w2, *d_bu_b2, *d_td_w1, *d_td_b1, *d_td_w2, *d_td_b2;
   // 1: every reduction runs in an order fixed by the shapes (no floating-point atomics): bit-reproducible gradients
   int deterministic;
+  // Implicit gradients through settle (backward_implicit_run), all 0 for every other backward.  They apply to a one-step
+  // call (iters = 1) at a state whose linearisation may already sit in the workspace:
+  //   state_only: only dL/dS_t is wanted; no weight / bias / token / pos gradient is computed (the tensor-core DX still
+  //               writes its token / pos rows, so d_tokens / d_pos must point at scratch)
+  //   relin:      the workspace already holds everything of this state and these weights that does not depend on the
+  //               cotangent (packed weights, bf16 tokens and shadows, BW_PRE's pre / h, khat / rnorm / khat_b, A / a_b)
+  //               from an earlier call with relin = 0 and the same state: those stages are skipped
+  //   skip_attn:  the consensus backward (it has no parameters) is skipped: dL/dS_t is incomplete
+  int state_only, relin, skip_attn;
 };
 struct BackwardLayout {
   size_t g_off, gs_off, ds_off, khat_off, dkhat_off, rnorm_off, pre_off, h_off, dh_off, xp_off, dx_off, attn_off,
@@ -262,6 +271,8 @@ struct MlpBwdTc {
   // sums of dpre into b1_part [G][ceil(R/32)][4d]; the caller reduces both afterwards (backward_run)
   int deterministic;
   float *dx_td, *b1_part;
+  // implicit gradients (BackwardArgs::relin / state_only): skip BW_PRE (pre / h already hold this state's), skip BW_DW
+  int skip_pre, skip_dw;
 };
 int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches,
                     char* err, size_t errlen);
@@ -284,6 +295,32 @@ cudaError_t tokenize_backward(const float* img, const float* weight, const float
 // steps (nullable, device memory): per-image step counts; image b is the identity at every reverse step t >= steps[b]
 int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int iters, int grad_all, const int32_t* steps,
                  void* workspace, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen);
+
+// Implicit gradients through settle (glom_b200_backward_implicit, bf16 engine): the backward workspace, followed by
+struct ImplicitLayout {
+  BackwardLayout bwd;
+  size_t u_off;            // (rows, L, d) f32   the adjoint u
+  size_t dsq_off;          // (rows, L, nparts) f32   |u_k - u_{k-1}|^2 partials
+  size_t nsq_off;          // (rows, L, nparts) f32   |u_k|^2 partials
+  size_t dtok_off;         // (rows, d) f32   token gradients of the adjoint passes (discarded)
+  size_t dpos_off;         // (n, d) f32      pos gradients of the adjoint passes (discarded)
+  size_t flags_off;        // zeroed at the start of a call:
+  size_t frozen_off;       //   [B] int            1: the image's adjoint has stopped
+  size_t block_frozen_off; //   [ceil(rows/256)]   (written by the convergence kernel, unused here)
+  size_t done_off;         //   [1] unsigned       blocks of the convergence kernel that have finished
+  size_t level_q_off;      //   [B * L] f32        the per-(image, level) ratios of each image's last adjoint pass
+  size_t stop_off;         //   [B] int32          the backward's skip vector: 0 = stopped, 1 = running (step t = 0)
+  size_t flags_bytes;
+  size_t total;
+};
+ImplicitLayout implicit_layout(const Geometry& g);
+// u_0 = grad_out; u_k = grad_out + J^T u_{k-1} at `state` for the running images, each stopped by settle's rule on u
+// (adjoint_tol) or after adjoint_iters passes; then one VJP at `state` with cotangent u_K into the gradients of `a`
+// (a.states = state, a.grad_out = grad_out; d_state0 / d_init NULL).  adjoint_steps (B) and adjoint_q (B, L, nullable)
+// receive K_b and the last pass's ratios
+int backward_implicit_run(const Geometry& g, const BackwardArgs& a, int adjoint_iters, float adjoint_tol,
+                          int32_t* adjoint_steps, float* adjoint_q, void* workspace, EncodeTiledFn enc, int num_sms,
+                          cudaStream_t st, int* launches, char* err, size_t errlen);
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per device and per function: remember, per device, the
 // largest size already configured for one kernel (one instance of this per kernel template instantiation).

@@ -842,6 +842,64 @@ GLOM_B200_API int glom_b200_backward_ex(const glom_b200_cfg* cfg, const glom_b20
                        workspace_bytes, stream, deterministic);
 }
 
+GLOM_B200_API int glom_b200_backward_implicit_workspace_bytes(const glom_b200_cfg* cfg, int batch, size_t* out_bytes) {
+  if (int r = check_cfg(cfg)) return r;
+  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "backward_implicit: bf16 engine only (precision fp32 given)");
+  if (batch < 1 || !out_bytes) return fail(GLOM_B200_ERR_INVALID, "backward_implicit: bad batch/out_bytes");
+  *out_bytes = implicit_layout(make_geometry(cfg, batch)).total;
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_backward_implicit(const glom_b200_cfg* cfg, const glom_b200_weights_ref* w, const float* tokens,
+                                              const float* pos, const float* state, const float* grad_out,
+                                              const glom_b200_grads* gr, int batch, int adjoint_iters, float adjoint_tol,
+                                              int deterministic, int32_t* adjoint_steps_out, float* adjoint_q_out,
+                                              void* workspace, size_t workspace_bytes, void* stream) {
+  if (int r = check_cfg(cfg)) return r;
+  if (cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "backward_implicit: bf16 engine only (precision fp32 given)");
+  if (batch < 1) return fail(GLOM_B200_ERR_INVALID, "backward_implicit: batch must be >= 1 (got %d)", batch);
+  if (adjoint_iters < 0)
+    return fail(GLOM_B200_ERR_INVALID, "backward_implicit: adjoint_iters must be >= 0 (got %d)", adjoint_iters);
+  if (adjoint_tol != adjoint_tol) return fail(GLOM_B200_ERR_INVALID, "backward_implicit: adjoint_tol is NaN");
+  if (deterministic != 0 && deterministic != 1)
+    return fail(GLOM_B200_ERR_INVALID, "backward_implicit: deterministic must be 0 or 1 (got %d)", deterministic);
+  if (int r = check_steps_ptr("backward_implicit", "adjoint_steps_out", adjoint_steps_out)) return r;
+  if (reinterpret_cast<uintptr_t>(adjoint_q_out) % 4)
+    return fail(GLOM_B200_ERR_INVALID, "backward_implicit: adjoint_q_out must be 4-byte aligned");
+  if (!w || w->struct_size != sizeof(glom_b200_weights_ref) || !gr || gr->struct_size != sizeof(glom_b200_grads))
+    return fail(GLOM_B200_ERR_INVALID, "weights / grads struct missing or wrong size");
+  if (!tokens || !pos || !state || !grad_out) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
+  if (!w->bu_w1 || !w->bu_b1 || !w->bu_w2 || !w->td_w1 || !w->td_b1 || !w->td_w2)
+    return fail(GLOM_B200_ERR_INVALID, "a weight pointer is NULL");
+  if (!gr->d_tokens || !gr->d_pos || !gr->d_bu_w1 || !gr->d_bu_b1 || !gr->d_bu_w2 || !gr->d_bu_b2 || !gr->d_td_w1 ||
+      !gr->d_td_b1 || !gr->d_td_w2 || !gr->d_td_b2)
+    return fail(GLOM_B200_ERR_INVALID, "gradient pointers: all MLP/token/pos outputs are needed");
+  if (gr->d_state0 || gr->d_init)
+    return fail(GLOM_B200_ERR_INVALID, "backward_implicit: d_state0 and d_init must be NULL (the fixed point does not "
+                                       "depend on the start state)");
+  DeviceInfo di{};
+  if (int r = device_info(&di)) return r;
+  const Geometry g = make_geometry(cfg, batch);
+  const ImplicitLayout il = implicit_layout(g);
+  if (!workspace || workspace_bytes < il.total || reinterpret_cast<uintptr_t>(workspace) % 1024)
+    return fail(GLOM_B200_ERR_WORKSPACE, "backward_implicit workspace: need %zu bytes 1024-aligned, got %zu", il.total,
+                workspace_bytes);
+  BackwardArgs a{};
+  a.tokens = tokens; a.pos = pos; a.states = state; a.grad_out = grad_out;
+  a.bu_w1 = w->bu_w1; a.bu_b1 = w->bu_b1; a.bu_w2 = w->bu_w2; a.td_w1 = w->td_w1; a.td_b1 = w->td_b1; a.td_w2 = w->td_w2;
+  a.d_tokens = gr->d_tokens; a.d_pos = gr->d_pos;
+  a.d_bu_w1 = gr->d_bu_w1; a.d_bu_b1 = gr->d_bu_b1; a.d_bu_w2 = gr->d_bu_w2; a.d_bu_b2 = gr->d_bu_b2;
+  a.d_td_w1 = gr->d_td_w1; a.d_td_b1 = gr->d_td_b1; a.d_td_w2 = gr->d_td_w2; a.d_td_b2 = gr->d_td_b2;
+  a.deterministic = deterministic;
+  g_launches = 0;
+  char msg[400] = "";
+  if (int r = backward_implicit_run(g, a, adjoint_iters, adjoint_tol, adjoint_steps_out, adjoint_q_out, workspace, g_encode,
+                                    di.sms, static_cast<cudaStream_t>(stream), &g_launches, msg, sizeof(msg)))
+    return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "%s", msg);
+  g_err[0] = 0;
+  return 0;
+}
+
 GLOM_B200_API int glom_b200_islands(const float* states, int slabs, int side_h, int side_w, int levels, int dim, float threshold,
                                     float* cos_right, float* cos_down, float* agreement, int32_t* labels, int32_t* num_islands,
                                     void* stream) {

@@ -560,9 +560,11 @@ int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int
   const int nm = (rows + 255) / 256;
   cudaError_t e;
   p.num_tiles = G * nm * (4 * d / BN);
-  e = launch<BW_PRE>(mxb, msb, msp, mw1p, mw1p, mw1p, p, num_sms, st);
-  if (launches) ++*launches;
-  if (e != cudaSuccess) { snprintf(err, errlen, "bwd pre launch: %s", cudaGetErrorString(e)); return -3; }
+  if (!a.skip_pre) {
+    e = launch<BW_PRE>(mxb, msb, msp, mw1p, mw1p, mw1p, p, num_sms, st);
+    if (launches) ++*launches;
+    if (e != cudaSuccess) { snprintf(err, errlen, "bwd pre launch: %s", cudaGetErrorString(e)); return -3; }
+  }
   e = a.deterministic ? launch<BW_DH, true>(mgs, mgs, mgs, mw2t, mw2t, mw2t, p, num_sms, st)
                       : launch<BW_DH>(mgs, mgs, mgs, mw2t, mw2t, mw2t, p, num_sms, st);
   if (launches) ++*launches;
@@ -572,6 +574,7 @@ int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int
                       : launch<BW_DX>(mdpre128, mdpre128, mdpre128, mw1t, mw1t, mw1t, p, num_sms, st);
   if (launches) ++*launches;
   if (e != cudaSuccess) { snprintf(err, errlen, "bwd dx launch: %s", cudaGetErrorString(e)); return -3; }
+  if (a.skip_dw) return 0;
   p.num_tiles = G * 2 * (d / 256) * (4 * d / BN);
   e = launch<BW_DW>(mgs64, mdpre64, mh64, mxb64, msb64, msp64, p, num_sms, st);
   if (launches) ++*launches;

@@ -19,6 +19,8 @@ The backward is once-differentiable.  By default it accumulates some sums with `
 reproducible only up to fp32 summation order; under ``torch.use_deterministic_algorithms(True)`` (read when the
 backward runs, ``warn_only`` included) it reduces in an order fixed by the shapes instead, and the gradients are
 bit-identical from run to run on the same GPU model and build (DESIGN.md, "Deterministic backward").
+``settle(differentiable="implicit")`` is trained by the implicit gradient of the settled state instead
+(``_SettleImplicit``, ``glom_b200_backward_implicit``; DESIGN.md, "Implicit gradients through settle").
 
 Packed weights: the MLP weights are repacked (one small kernel) on EVERY call while ``self.training``; in eval mode
 the packed copy is cached and keyed on each parameter's ``(data_ptr, _version)`` and dropped by ``load_state_dict``,
@@ -196,6 +198,49 @@ class _ColumnUpdate(torch.autograd.Function):
                 g["d_init"], *[g[k] for k in names])
 
 
+class _SettleImplicit(torch.autograd.Function):
+    """Glom.settle(differentiable="implicit"): forward = glom_b200_settle (the same call as under no_grad), backward =
+    glom_b200_backward_implicit, the implicit-function-theorem gradient of the settled state S* = f(S*).  The graph
+    keeps S*, the tokens, pos and the weights, no trajectory.  The start state and init_levels get no gradient: the
+    fixed point does not depend on where the iteration started.  Outputs (levels, steps); steps is not differentiable."""
+
+    @staticmethod
+    def forward(ctx, module, max_iters, tol, adjoint_tol, adjoint_iters, tokens, pos, state0, init_levels, *weights):
+        tokens, pos = tokens.contiguous(), pos.contiguous()
+        levels, steps = module._run(tokens, pos, state0, init_levels, max_iters, False, tol=tol)
+        ctx.mark_non_differentiable(steps)
+        ctx.module, ctx.adjoint_tol, ctx.adjoint_iters = module, adjoint_tol, adjoint_iters
+        ctx.save_for_backward(tokens, pos, levels, *weights)
+        return levels, steps
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out, *_grad_steps):
+        module = ctx.module
+        tokens, pos, state, *weights = ctx.saved_tensors
+        device = state.device
+        b, n = tokens.shape[0], tokens.shape[1]
+        grad_out = grad_out.to(torch.float32).contiguous()
+        wts = [w.detach().to(torch.float32).contiguous() for w in weights]
+        names = ("d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")
+        g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos)}
+        for k, w in zip(names, wts):
+            g[k] = zeros_like32(w)
+        adj_steps = torch.empty(b, dtype=torch.int32, device=device)
+        adj_q = torch.empty(b, module.levels, dtype=torch.float32, device=device)
+        with torch.cuda.device(device):
+            cfg = module.engine_cfg(n)
+            ws_bytes = _native.backward_implicit_workspace_bytes(cfg, b)
+            ws = module._get_workspace(ws_bytes, device, "_implicit_workspace")      # cached across steps
+            _native.backward_implicit(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(),
+                                      state.data_ptr(), grad_out.data_ptr(), {k: v.data_ptr() for k, v in g.items()}, b,
+                                      ctx.adjoint_iters, ctx.adjoint_tol, adj_steps.data_ptr(), adj_q.data_ptr(),
+                                      ws.data_ptr(), ws.numel(), torch.cuda.current_stream(device).cuda_stream,
+                                      deterministic=torch.are_deterministic_algorithms_enabled())
+        module.last_adjoint = (adj_steps, adj_q)
+        return (None, None, None, None, None, g["d_tokens"], g["d_pos"], None, None, *[g[k] for k in names])
+
+
 def zeros_like32(t):
     return torch.zeros(t.shape, dtype=torch.float32, device=t.device)
 
@@ -262,6 +307,7 @@ class Glom(nn.Module):
         self.__dict__.update(self._empty_scratch())
         self.use_native_tokenizer = True
         self.last_launches = 0
+        self.last_adjoint = None      # settle(differentiable="implicit"): (steps (B,) int32, q (B, L) f32) of the last backward
 
     # ------------------------------------------------------------------ cache hygiene
     @staticmethod
@@ -528,9 +574,10 @@ class Glom(nn.Module):
             raise RuntimeError(f"levels must have shape {(b, n, self.levels, self.dim)}, got {tuple(levels.shape)}")
         return b, n
 
-    def _column_update(self, img, levels, needs_grad, iters, return_all, *, steps=None, tol=None):
+    def _column_update(self, img, levels, needs_grad, iters, return_all, *, steps=None, tol=None, adjoint=None):
         """forward and settle after their own argument checks: check the image and `levels`, take the tokens, and run the
-        engine (`_run`'s arguments), through the autograd Function _ColumnUpdate when gradients are needed."""
+        engine (`_run`'s arguments), through the autograd Function _ColumnUpdate when gradients are needed, or
+        _SettleImplicit with `adjoint` = (adjoint_tol, adjoint_iters) (settle(differentiable="implicit"))."""
         _, n = self._check_input(img, levels)
         if not needs_grad:
             tokens = self._take_staged(img)
@@ -548,11 +595,15 @@ class Glom(nn.Module):
             tokens = lin(self.image_to_tokens[0](img.float()))
         pos = self.pos_emb.weight[:n]                                                            # (:117)
         state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
+        if adjoint is not None:
+            return _SettleImplicit.apply(self, iters, tol, *adjoint, tokens, pos, state0, self.init_levels,
+                                         *self._mlp_params())
         return _ColumnUpdate.apply(self, iters, steps, tol, return_all, tokens, pos, state0, self.init_levels,
                                    *self._mlp_params())
 
     # ------------------------------------------------------------------ inference until the columns settle
-    def settle(self, img, tol, max_iters=None, levels=None, *, return_all=False, differentiable=False):
+    def settle(self, img, tol, max_iters=None, levels=None, *, return_all=False, differentiable=False, adjoint_tol=None,
+               adjoint_iters=None):
         """Run each image's column update until its levels stop changing -> ``(levels, steps)``.
 
         After step k the change of image b is ``max_l sqrt(sum_i |S_k[b,i,l] - S_{k-1}[b,i,l]|^2 / sum_i |S_k[b,i,l]|^2)``
@@ -571,9 +622,37 @@ class Glom(nn.Module):
         running the steps a second time and without a host read of ``steps``.  The returned ``steps`` is not
         differentiable; the backward keeps its own copy.  That path holds all max_iters+1 states in fp32 until the
         backward, with or without ``return_all``: about 1.3 GB at dim 512, 6 levels, 256 patches, batch 32 and
-        max_iters 12.  Without autograd ``differentiable`` changes nothing."""
+        max_iters 12.  Without autograd ``differentiable`` changes nothing.
+
+        ``differentiable="implicit"`` trains the settled state itself instead of the path that reached it: the forward is
+        the plain settle call (``levels`` and ``steps`` bit-identical to it under no_grad) and the graph keeps only S*,
+        the tokens, pos and the weights.  The backward is the implicit-function-theorem gradient of S* = f(S*): with
+        J = df/dS at each image's S* and g = dL/dS*, it iterates ``u_0 = g, u_k = g + J^T u_{k-1}`` per image, stops an
+        image by settle's rule applied to u (``adjoint_tol``, default ``tol``) or after ``adjoint_iters`` passes (default
+        ``max_iters``; 0 gives the one-step "Jacobian-free" gradient), and returns the gradients of one step at S* with
+        cotangent u_K (the MLP weights, pos, the tokens and through them the image and the tokeniser).  ``levels`` and
+        ``init_levels`` get no gradient: the fixed point does not depend on the start.  An image whose adjoint does not
+        converge gets the truncated Neumann sum.  ``self.last_adjoint`` then holds ``(steps, q)`` of that backward:
+        each image's K_b ((B,) int32) and its last pass's per-level ratios ((B, L) float32), on the GPU.  No
+        ``return_all``."""
         if self.precision != "bf16":
             raise RuntimeError("Glom.settle needs precision='bf16' (the fp32 engine has no early stopping)")
+        implicit = isinstance(differentiable, str)
+        if implicit and differentiable != "implicit":
+            raise ValueError(f"differentiable must be False, True or 'implicit', got {differentiable!r}")
+        if not implicit and (adjoint_tol is not None or adjoint_iters is not None):
+            raise ValueError("adjoint_tol / adjoint_iters need differentiable='implicit'")
+        if implicit:
+            if return_all:
+                raise ValueError("differentiable='implicit' has no trajectory to return: return_all must be False")
+            if adjoint_tol is not None:
+                adjoint_tol = float(adjoint_tol)
+                if adjoint_tol != adjoint_tol:
+                    raise ValueError("adjoint_tol is NaN")
+            if adjoint_iters is not None:
+                adjoint_iters = operator.index(adjoint_iters)
+                if adjoint_iters < 0:
+                    raise ValueError(f"adjoint_iters must be >= 0, got {adjoint_iters}")
         _require_cuda(img)
         needs_grad = self._needs_grad(img, levels)
         if needs_grad and not differentiable:
@@ -585,7 +664,10 @@ class Glom(nn.Module):
         tol = float(tol)
         if tol != tol:
             raise ValueError("tol is NaN")
-        return self._column_update(img, levels, needs_grad, max_iters, return_all, tol=tol)
+        adjoint = None
+        if implicit and needs_grad:
+            adjoint = (tol if adjoint_tol is None else adjoint_tol, max_iters if adjoint_iters is None else adjoint_iters)
+        return self._column_update(img, levels, needs_grad, max_iters, return_all, tol=tol, adjoint=adjoint)
 
     # ------------------------------------------------------------------ settling a stream of images
     def settle_queue(self, img, tol, max_iters=None, levels=None, *, slots=32):

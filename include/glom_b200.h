@@ -301,6 +301,30 @@ GLOM_B200_API int glom_b200_backward_ex(const glom_b200_cfg* cfg, const glom_b20
                                         int grad_all, int deterministic, void* workspace, size_t workspace_bytes,
                                         void* stream);
 
+/* Implicit gradients of a settled state (Glom.settle(differentiable="implicit"); bf16 engine only).  `state` (B, n, L, d)
+ * is S*, the levels glom_b200_settle returned, and grad_out its cotangent g.  With J_b = df/dS at image b's S*_b (f: one
+ * column step), each image runs the adjoint iteration
+ *   u_0 = g,   u_k = g + J^T u_{k-1}
+ * and stops at the first k >= 1 where max_l sqrt(sum_i |u_k - u_{k-1}|^2 / sum_i |u_k|^2) <= adjoint_tol (settle's rule
+ * on u: sums over the image's columns, fp32, 0/0 counts as 0, a NaN never stops), or after adjoint_iters passes
+ * (0: u = g).  Then the gradients of the single step f at S* with cotangent u_K (tokens, pos, the eight MLP tensors) are
+ * ACCUMULATED into `grads`, whose d_state0 and d_init must be NULL: the fixed point does not depend on where the
+ * iteration started.  adjoint_steps_out (B) int32 receives K_b, adjoint_q_out (B, L) f32 (nullable) each image's ratios
+ * of its last pass (zeros when adjoint_iters = 0).
+ * The state-only quantities of the step (bf16 shadows, MLP pre-activations, attention probabilities) are computed once;
+ * each adjoint pass runs only the cotangent-dependent stages, with the fixed-order (deterministic) reductions whatever
+ * `deterministic` says, so K_b and q are the same on every run.  The final parameter pass honours `deterministic` as
+ * glom_b200_backward_ex does.  Argument errors (fp32 precision, batch < 1, adjoint_iters < 0, NaN adjoint_tol,
+ * deterministic not 0 or 1, NULL or misaligned adjoint_steps_out, misaligned adjoint_q_out, a NULL required pointer,
+ * non-NULL d_state0 / d_init) are reported before any device query. */
+GLOM_B200_API int glom_b200_backward_implicit_workspace_bytes(const glom_b200_cfg* cfg, int batch, size_t* out_bytes);
+GLOM_B200_API int glom_b200_backward_implicit(const glom_b200_cfg* cfg, const glom_b200_weights_ref* weights,
+                                              const float* tokens, const float* pos, const float* state,
+                                              const float* grad_out, const glom_b200_grads* grads, int batch,
+                                              int adjoint_iters, float adjoint_tol, int deterministic,
+                                              int32_t* adjoint_steps_out, float* adjoint_q_out, void* workspace,
+                                              size_t workspace_bytes, void* stream);
+
 /* Backward of glom_b200_tokenize (image_to_tokens, glom_pytorch.py:94-97; SURVEY 8 rows f1 + f2), fp32 on CUDA cores:
  *   d_weight (dim, 3 patch^2) += d_tokens^T . patches,   d_bias (dim) += column sums of d_tokens,
  *   d_img (B, 3, H, W) += fold(d_tokens . weight).
