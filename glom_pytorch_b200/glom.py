@@ -51,6 +51,13 @@ def _aligned_bytes(nbytes, device, align=1024):
     return raw[off:off + nbytes]
 
 
+def _contiguous16(t):
+    """t contiguous with a 16-byte aligned data_ptr, as the engine's fp32 tensor arguments must be: a contiguous view
+    that starts mid-row of a larger buffer (e.g. ``big.view(-1)[1:1 + k].view(shape)``) is copied."""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
 def _require_cuda(img):
     if not img.is_cuda:
         raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
@@ -154,7 +161,7 @@ class _ColumnUpdate(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, module, iters, steps, tol, return_all, tokens, pos, state0, init_levels, *weights):
-        tokens, pos = tokens.contiguous(), pos.contiguous()
+        tokens, pos = _contiguous16(tokens), _contiguous16(pos)
         states = module._run(tokens, pos, state0, init_levels, iters, True, steps=steps, tol=tol)   # (T+1, B, n, L, d)
         if tol is not None:
             states, steps = states
@@ -175,8 +182,8 @@ class _ColumnUpdate(torch.autograd.Function):
         tokens, pos, states, *weights = ctx.saved_tensors
         device = states.device
         b, n = tokens.shape[0], tokens.shape[1]
-        grad_out = grad_out.to(torch.float32).contiguous()
-        wts = [w.detach().to(torch.float32).contiguous() for w in weights]
+        grad_out = _contiguous16(grad_out.to(torch.float32))
+        wts = [_contiguous16(w.detach().to(torch.float32)) for w in weights]
         zeros = torch.zeros
         g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos),
              "d_state0": zeros(states.shape[1:], dtype=torch.float32, device=device) if ctx.had_state0 else None,
@@ -206,7 +213,7 @@ class _SettleImplicit(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, module, max_iters, tol, adjoint_tol, adjoint_iters, tokens, pos, state0, init_levels, *weights):
-        tokens, pos = tokens.contiguous(), pos.contiguous()
+        tokens, pos = _contiguous16(tokens), _contiguous16(pos)
         levels, steps = module._run(tokens, pos, state0, init_levels, max_iters, False, tol=tol)
         ctx.mark_non_differentiable(steps)
         ctx.module, ctx.adjoint_tol, ctx.adjoint_iters = module, adjoint_tol, adjoint_iters
@@ -220,8 +227,8 @@ class _SettleImplicit(torch.autograd.Function):
         tokens, pos, state, *weights = ctx.saved_tensors
         device = state.device
         b, n = tokens.shape[0], tokens.shape[1]
-        grad_out = grad_out.to(torch.float32).contiguous()
-        wts = [w.detach().to(torch.float32).contiguous() for w in weights]
+        grad_out = _contiguous16(grad_out.to(torch.float32))
+        wts = [_contiguous16(w.detach().to(torch.float32)) for w in weights]
         names = ("d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")
         g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos)}
         for k, w in zip(names, wts):
@@ -474,11 +481,11 @@ class Glom(nn.Module):
             use_resume = (plain and allow_resume and resume is not None and state_in is not None and iters >= 1
                           and self.precision == "bf16" and resume["ref"]() is state_in
                           and state_in._version == resume["version"] and resume["key"] == call_key)
-            tokens = tokens.detach().to(torch.float32).contiguous()
-            pos = pos.detach().to(torch.float32).contiguous()
-            init = init.detach().to(torch.float32).contiguous()
+            tokens = _contiguous16(tokens.detach().to(torch.float32))
+            pos = _contiguous16(pos.detach().to(torch.float32))
+            init = _contiguous16(init.detach().to(torch.float32))
             if state_in is not None:
-                state_in = state_in.detach().to(device=device, dtype=torch.float32).contiguous()
+                state_in = _contiguous16(state_in.detach().to(device=device, dtype=torch.float32))
             state_ptr = None if state_in is None else state_in.data_ptr()
             cfg = self.engine_cfg(n)
             packed = self._packed_weights(cfg, device, stream)
@@ -756,9 +763,9 @@ class Glom(nn.Module):
         begin, run = getattr(_native, name + "_begin"), getattr(_native, name + "_run")
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            pos = self.pos_emb.weight[:n].detach().to(torch.float32).contiguous()
-            init = self.init_levels.detach().to(torch.float32).contiguous()
-            state_in = None if levels is None else levels.detach().to(device=device, dtype=torch.float32).contiguous()
+            pos = _contiguous16(self.pos_emb.weight[:n].detach().to(torch.float32))
+            init = _contiguous16(self.init_levels.detach().to(torch.float32))
+            state_in = None if levels is None else _contiguous16(levels.detach().to(device=device, dtype=torch.float32))
             state_ptr = None if state_in is None else state_in.data_ptr()
             cfg = self.engine_cfg(n)
             packed = self._packed_weights(cfg, device, stream)

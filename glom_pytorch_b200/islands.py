@@ -35,6 +35,8 @@ def islands(states, *, grid=None, threshold=0.9):
     if side_h * side_w != n:
         raise RuntimeError(f"grid {grid} does not tile n = {n}")
     x = states.detach().to(torch.float32).contiguous()
+    if x.data_ptr() % 16:                 # a contiguous view starting mid-row: the kernels load float4
+        x = x.clone()
     slabs = 1
     for v in lead:
         slabs *= v
