@@ -79,6 +79,7 @@ SIGNATURES = {
     "glom_b200_islands": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "glom_b200_clock_probe": (_i32, [_vp, _i32, _vp]),
     "glom_b200_kernel_clocks": (_i32, [_vp, _vp, _vp, _i32, _i32]),
+    "glom_b200_set_sm_count_target": (_i32, [_i32]),
 }
 EXPORTS = tuple(SIGNATURES)
 
@@ -337,6 +338,16 @@ def kernel_clocks(reset=True):
     mhz, ms, wf = (ctypes.c_double * k)(), (ctypes.c_double * k)(), (ctypes.c_double * (6 * k))()
     check(load().glom_b200_kernel_clocks(mhz, ms, wf, k, int(bool(reset))))
     return {PROFILE_KINDS[i]: (mhz[i], ms[i], [round(wf[6 * i + j], 4) for j in range(6)]) for i in range(k) if ms[i] > 0}
+
+
+def set_sm_count_target(sms):
+    """Plan every later launch of this process for at most `sms` SMs (0: the device's own count) -> the previous
+    target.  Grids change, results do not (glom_b200_set_sm_count_target)."""
+    lib = load()
+    prev = lib.glom_b200_set_sm_count_target(int(sms))
+    if prev < 0:
+        raise GlomB200Error(f"glom_b200 error {prev}: {lib.glom_b200_last_error().decode()}")
+    return prev
 
 
 def islands(states_ptr, slabs, side_h, side_w, levels, dim, threshold, cos_right_ptr, cos_down_ptr, agreement_ptr,

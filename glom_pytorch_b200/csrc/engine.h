@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <atomic>
 #include <mutex>
 #include <vector>
 
@@ -343,12 +344,22 @@ struct SmemOptIn {
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// SM count of the current device: grid caps of the grid-stride CUDA-core kernels are a few waves of it
+// glom_b200_set_sm_count_target (glom_api.cu): plan launches for at most this many SMs; 0 = the device's own count
+extern std::atomic<int> g_sm_count_target;
+
+// `device_sms` bounded by the SM-count target
+static inline int planned_sms(int device_sms) {
+  const int t = g_sm_count_target.load(std::memory_order_relaxed);
+  return (t > 0 && t < device_sms) ? t : device_sms;
+}
+
+// SM count of the current device (bounded by the SM-count target): grid caps of the grid-stride CUDA-core kernels are a
+// few waves of it
 static inline int sm_count() {
   int dev = 0, n = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1)
     n = 132;
-  return n;
+  return planned_sms(n);
 }
 
 }  // namespace glom

@@ -160,8 +160,11 @@ static int device_info(DeviceInfo* out) {
   }
   *out = g_dev[dev];
   if (!out->ok) return fail(GLOM_B200_ERR_DEVICE, "device %d is not compute capability 9.x (sm_90a kernels only)", dev);
+  out->sms = planned_sms(out->sms);
   return 0;
 }
+
+std::atomic<int> g_sm_count_target{0};
 
 }  // namespace glom
 
@@ -174,6 +177,12 @@ GLOM_B200_API int glom_b200_abi_version(void) { return GLOM_B200_ABI_VERSION; }
 GLOM_B200_API const char* glom_b200_last_error(void) { return g_err; }
 
 GLOM_B200_API int glom_b200_last_launch_count(void) { return g_launches; }
+
+GLOM_B200_API int glom_b200_set_sm_count_target(int sms) {
+  if (sms < 0 || sms == 1)
+    return fail(GLOM_B200_ERR_INVALID, "SM-count target must be 0 or >= 2 (got %d): a CTA pair needs two SMs", sms);
+  return g_sm_count_target.exchange(sms);
+}
 
 GLOM_B200_API int glom_b200_packed_weight_bytes(const glom_b200_cfg* cfg, size_t* out_bytes) {
   if (int r = check_cfg(cfg)) return r;

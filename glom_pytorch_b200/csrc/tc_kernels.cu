@@ -957,16 +957,23 @@ static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1
   attr[1].id = cudaLaunchAttributeClusterDimension;                     // the pair shares its B tiles (multicast)
   attr[1].val.clusterDim.x = 2; attr[1].val.clusterDim.y = 1; attr[1].val.clusterDim.z = 1;
   // Both CTAs of a cluster need an SM of the same GPC, so fewer than num_sms / 2 pairs may be co-resident; a grid beyond
-  // that would run its last clusters as a second wave.
-  static int max_pairs = 0;
-  if (max_pairs == 0) {
-    cfg.gridDim = dim3(2 * (num_sms / 2));
+  // that would run its last clusters as a second wave.  The co-resident count is a property of the device (queried once
+  // per device for its full SM count); num_sms, which the SM-count target may lower, bounds it on every call.
+  static std::atomic<int> co_resident[64];
+  int dev = 0;
+  if (cudaError_t e = cudaGetDevice(&dev)) return e;
+  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+  int occ = co_resident[dev].load(std::memory_order_relaxed);
+  if (occ == 0) {
+    int dev_sms = 0;
+    if (cudaError_t e = cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, dev)) return e;
+    cfg.gridDim = dim3(2 * (dev_sms / 2));
     cfg.attrs = &attr[1]; cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaError_t e = cudaOccupancyMaxActiveClusters(&n, gemm_kernel<MODE, BN, CNT, SETTLE>, &cfg)) return e;
-    if (n < 1) return cudaErrorInvalidConfiguration;
-    max_pairs = n < num_sms / 2 ? n : num_sms / 2;
+    if (cudaError_t e = cudaOccupancyMaxActiveClusters(&occ, gemm_kernel<MODE, BN, CNT, SETTLE>, &cfg)) return e;
+    if (occ < 1) return cudaErrorInvalidConfiguration;
+    co_resident[dev].store(occ, std::memory_order_relaxed);
   }
+  const int max_pairs = occ < num_sms / 2 ? occ : num_sms / 2;
   cfg.attrs = attr; cfg.numAttrs = 2;
   const int pairs = p.num_tiles < max_pairs ? p.num_tiles : max_pairs;
   cfg.gridDim = dim3(2 * pairs);

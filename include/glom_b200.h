@@ -365,6 +365,13 @@ GLOM_B200_API int glom_b200_islands(const float* states, int slabs, int side_h, 
                                     float* cos_right, float* cos_down, float* agreement, int32_t* labels,
                                     int32_t* num_islands, void* stream);
 
+/* Plan every launch for at most `sms` SMs (0 = the device's own count; larger values are clamped to it).  Persistent
+ * kernels then launch min(work, sms) CTAs (consensus) or min(work, sms / 2, co-resident) pairs (GEMM1, GEMM2, tokeniser,
+ * backward GEMMs), and the grid-stride CUDA-core kernels size their grids from it.  Results do not depend on it: it
+ * lets a test run the grids of a part with fewer SMs (an H100 PCIe, a MIG slice).  Process-wide.  Returns the previous
+ * target, or -1 with glom_b200_last_error() set for sms < 0 or sms == 1 (a pair needs two SMs).  Touches no device. */
+GLOM_B200_API int glom_b200_set_sm_count_target(int sms);
+
 /* Measurement aid (bench.py): one device thread spins for `spin_us` microseconds of %globaltimer and writes
  * {SM cycles elapsed, nanoseconds elapsed} to out_cycles_ns[0..1] (device memory, 16 bytes): cycles / ns is the SM
  * clock in GHz the device actually ran at when the probe executed.  Enqueued on `stream`; the caller synchronises. */
