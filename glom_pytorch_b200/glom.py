@@ -25,7 +25,9 @@ bit-identical from run to run on the same GPU model and build (DESIGN.md, "Deter
 Packed weights: the MLP weights are repacked (one small kernel) on EVERY call while ``self.training``; in eval mode
 the packed copy is cached and keyed on each parameter's ``(data_ptr, _version)`` and dropped by ``load_state_dict``,
 ``.to()`` / ``.cuda()`` / ``.half()``-style ``_apply`` calls and ``invalidate_packed()``.  In-place edits through
-``param.data`` do not bump ``_version``: call ``invalidate_packed()`` after them in eval mode.
+``param.data`` do not bump ``_version``: call ``invalidate_packed()`` after them in eval mode.  A call made under CUDA
+graph capture packs inside its graph into a buffer of its own and uses workspaces no other call touches, so its graph
+reads the parameters at replay and depends on no other call (DESIGN.md, "CUDA graphs and streams").
 
 Engine-only knob (keyword-only, additive): ``precision`` = ``"bf16"`` (default; wgmma tensor cores,
 bf16 operands, fp32 accumulate and fp32 state -- the arithmetic of the reference under
@@ -56,6 +58,17 @@ def _contiguous16(t):
     that starts mid-row of a larger buffer (e.g. ``big.view(-1)[1:1 + k].view(shape)``) is copied."""
     t = t.contiguous()
     return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+def _capturing():
+    """True inside a CUDA graph capture on the current stream.  Such a call may only enqueue: it reads nothing on the
+    host, and it uses buffers of its own that no other call touches (Glom._capture_owned)."""
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
+def _no_capture(what, why):
+    if _capturing():
+        raise RuntimeError(f"{what} cannot be captured in a CUDA graph: {why}")
 
 
 def _require_cuda(img):
@@ -113,42 +126,83 @@ class ConsensusAttention(nn.Module):
             co = torch.stack((hh.reshape(-1), ww.reshape(-1)), -1).float()     # (h w) c
             dist = torch.cdist(co, co)
             self.register_buffer("non_local_mask", (dist > local_consensus_radius)[None])
+        self._mask_key = None
+        self._derive_mask()
 
     def forward(self, *_):
         raise RuntimeError("ConsensusAttention runs inside the fused column update engine; call Glom.forward")
 
     def mask_params(self, n):
         """(mask_side, mask_d2_max) for the engine's analytic mask, derived from the buffer so a
-        loaded state_dict is honoured; raises if the buffer is not a radial mask on the grid."""
+        loaded state_dict is honoured; raises if the buffer is not a radial mask on the grid.  The buffer is checked on
+        the host when it is created, moved, loaded or copied, so this call reads nothing from the device (and may run
+        inside a CUDA graph capture) unless the buffer was edited in place since."""
         if self.local_consensus_radius <= 0:
             return 0, 0
         side = self.num_patches_side
-        mask = self.non_local_mask[0]
         if n != side * side:
             raise RuntimeError(f"local_consensus_radius needs n == num_patches ({side * side}), got {n} "
                                "(the reference's masked_fill_ fails the same way)")
-        key = getattr(self, "_mask_key", None)
-        if key is None or key[0] is not self.non_local_mask or key[2] != self.non_local_mask._version:
-            ar = torch.arange(side, device=mask.device)
-            hh, ww = torch.meshgrid(ar, ar, indexing="ij")
-            co = torch.stack((hh.reshape(-1), ww.reshape(-1)), -1)
-            d2 = ((co[:, None, :] - co[None, :, :]) ** 2).sum(-1)
-            kept = d2[~mask]
-            d2_max = int(kept.max().item()) if kept.numel() else -1
-            if not torch.equal(d2 > d2_max, mask):
-                raise RuntimeError("attention.non_local_mask is not a radius mask on the patch grid")
-            self._mask_key = (self.non_local_mask, d2_max, self.non_local_mask._version)
+        if not self._mask_fresh():
+            _no_capture("a call after an in-place edit of attention.non_local_mask",
+                        "checking the edited mask reads it on the host; make one call outside the capture first")
+            self._derive_mask()
+        if self._mask_key[1] is None:
+            raise RuntimeError("attention.non_local_mask is not a radius mask on the patch grid")
         return side, self._mask_key[1]
 
-    def _load_from_state_dict(self, *args, **kwargs):     # a loaded mask (copied in place) is re-derived
-        self._mask_key = None
-        return super()._load_from_state_dict(*args, **kwargs)
+    def _mask_fresh(self):
+        key = getattr(self, "_mask_key", None)
+        return key is not None and key[0] is self.non_local_mask and key[2] == self.non_local_mask._version
 
-    def __getstate__(self):
+    def _derive_mask(self):
+        """Key the buffer with its d2_max (None if it is not a radius mask on the grid), read from a host copy."""
+        if self.local_consensus_radius <= 0:
+            return
+        side = self.num_patches_side
+        mask = self.non_local_mask[0].cpu()
+        ar = torch.arange(side)
+        hh, ww = torch.meshgrid(ar, ar, indexing="ij")
+        co = torch.stack((hh.reshape(-1), ww.reshape(-1)), -1)
+        d2 = ((co[:, None, :] - co[None, :, :]) ** 2).sum(-1)
+        kept = d2[~mask]
+        d2_max = int(kept.max().item()) if kept.numel() else -1
+        self._mask_key = (self.non_local_mask, d2_max if torch.equal(d2 > d2_max, mask) else None,
+                          self.non_local_mask._version)
+
+    def _apply(self, fn, *args, **kwargs):                 # .to() / .cuda() replace the buffer: its d2_max carries over
+        if self.local_consensus_radius > 0 and not self._mask_fresh():
+            self._derive_mask()
+        out = super()._apply(fn, *args, **kwargs)
+        if self.local_consensus_radius > 0:
+            self._mask_key = (self.non_local_mask, self._mask_key[1], self.non_local_mask._version)
+        return out
+
+    def _load_from_state_dict(self, *args, **kwargs):     # a loaded mask (copied in place) is re-derived
+        out = super()._load_from_state_dict(*args, **kwargs)
+        self._derive_mask()
+        return out
+
+    def __getstate__(self):                               # pickle / deepcopy: the key travels as d2_max alone
         st = super().__getstate__() if hasattr(super(), "__getstate__") else self.__dict__.copy()
         st = dict(st)
         st.pop("_mask_key", None)
+        if self.local_consensus_radius > 0:
+            if not self._mask_fresh():
+                self._derive_mask()
+            st["_mask_d2"] = self._mask_key[1]
         return st
+
+    def __setstate__(self, st):
+        st = dict(st)
+        carried = "_mask_d2" in st
+        d2 = st.pop("_mask_d2", None)
+        super().__setstate__(st)
+        self._mask_key = None
+        if carried:
+            self._mask_key = (self.non_local_mask, d2, self.non_local_mask._version)
+        else:
+            self._derive_mask()
 
 
 class _ColumnUpdate(torch.autograd.Function):
@@ -320,19 +374,30 @@ class Glom(nn.Module):
     @staticmethod
     def _empty_scratch():
         """The device-side caches, empty.  .to() / .cuda() / .float() (parameters are replaced), pickling and deepcopy
-        reset them to this."""
+        reset them to this (.to() keeps the buffers of captured calls: graphs may still use them)."""
         return {"_packed": None,    # (key, tensor)
                 "_scratch": {},     # (slot, device index, stream) -> buffer, grown on demand, reused across calls
                 "_resume": None,    # cross-call persistence: what the workspace still holds about the last returned state
-                "_staged": None}    # tokens of the next frame computed ahead on a side stream (stage_tokens)
+                "_staged": None,    # tokens of the next frame computed ahead on a side stream (stage_tokens)
+                "_captured": []}    # the packed weights and workspaces of calls made under CUDA graph capture
 
     def invalidate_packed(self):
         """Drop the cached packed copy of the MLP weights (needed after in-place ``param.data`` edits in eval mode)."""
         self._packed = None
 
     def _apply(self, fn, *args, **kwargs):
+        captured = self._captured
         self.__dict__.update(self._empty_scratch())
+        self._captured = captured
         return super()._apply(fn, *args, **kwargs)
+
+    def _capture_owned(self, nbytes, device):
+        """A buffer for one call under CUDA graph capture.  Its graph's replays are its only users: the module keeps it
+        for its lifetime, so it is never freed or handed to another call or capture, and graphs captured on one module
+        share nothing (any replay order, or replays on concurrent streams, are safe)."""
+        buf = _aligned_bytes(nbytes, device)
+        self._captured.append(buf)
+        return buf
 
     def _load_from_state_dict(self, *args, **kwargs):      # load_state_dict copies in place: versions bump, but be explicit
         self._packed = None
@@ -369,9 +434,12 @@ class Glom(nn.Module):
     def _packed_weights(self, cfg, device, stream):
         params = self._mlp_params()
         key = (self.precision, (device, stream), tuple((p.data_ptr(), p._version) for p in params))
+        capturing = _capturing()
         # training: parameters change between calls in ways the key cannot always see (optimisers that write through
-        # .data, EMA updates): repack every call (one ~30 us kernel).  eval: cached on (data_ptr, _version).
-        if not self.training and self._packed is not None and self._packed[0] == key:
+        # .data, EMA updates): repack every call (one ~30 us kernel).  eval: cached on (data_ptr, _version).  Under
+        # graph capture the pack is part of the graph, into a buffer of its own: a replay reads the parameters as they
+        # are then, and depends on no other call or graph.
+        if not self.training and not capturing and self._packed is not None and self._packed[0] == key:
             return self._packed[1]
         srcs = []
         for p in params:
@@ -380,18 +448,24 @@ class Glom(nn.Module):
                 t = t.float().contiguous()
             srcs.append(t)
         nbytes = _native.packed_weight_bytes(cfg)
-        if self._packed is not None and self._packed[1].device == device and self._packed[1].numel() == nbytes \
+        if capturing:
+            packed = self._capture_owned(nbytes, device)
+        elif self._packed is not None and self._packed[1].device == device and self._packed[1].numel() == nbytes \
                 and self._packed[0][:2] == key[:2]:
             packed = self._packed[1]            # same stream order as the kernels that read it: safe to overwrite
         else:
             packed = _aligned_bytes(nbytes, device)
         _native.pack_weights(cfg, [t.data_ptr() for t in srcs], packed.data_ptr(), nbytes, stream)
-        self._packed = (key, packed)
+        if not capturing:
+            self._packed = (key, packed)
         return packed
 
     def _get_workspace(self, nbytes, device, slot="_workspace"):
         """Scratch buffer per (purpose, device, stream): two forwards of one module on different streams never share
-        H / C / shadow buffers, and a buffer is only ever reused by work enqueued on the stream that last used it."""
+        H / C / shadow buffers, and a buffer is only ever reused by work enqueued on the stream that last used it.
+        Under graph capture: a fresh buffer that only the graph uses (_capture_owned)."""
+        if _capturing():
+            return self._capture_owned(nbytes, device)
         key = (slot, device.index if device.index is not None else torch.cuda.current_device(),
                torch.cuda.current_stream(device).cuda_stream)
         ws = self._scratch.get(key)
@@ -430,7 +504,10 @@ class Glom(nn.Module):
         """Video / multi-frame use (README.md:94-112): compute image_to_tokens of the NEXT frame now, on a side stream, so
         that it overlaps the tail of the forward call already enqueued for the current frame.  The following
         ``forward(img, ...)`` with this very tensor (unmodified) picks the tokens up instead of tokenising again.
-        No-grad inference only; returns nothing."""
+        No-grad inference only; returns nothing.  Not capturable: it forks to a stream of its own, and a captured forward
+        tokenises inside its graph anyway."""
+        _no_capture("stage_tokens", "it tokenises on a side stream for the next eager forward; a captured forward "
+                                    "tokenises inside its graph")
         if not img.is_cuda:
             raise RuntimeError("stage_tokens needs a CUDA tensor")
         device = img.device
@@ -469,10 +546,17 @@ class Glom(nn.Module):
         * `steps` (glom_b200_forward_steps): image b runs steps[b] steps (steps: the engine's (B,) int32 CUDA tensor,
           iters its maximum).
         * `tol` (glom_b200_settle / _settle_all): up to `iters` steps, each image stopped on the GPU -> (out, steps).
-        After a per-image run the shadows of stopped images are stale: the next forward takes the ordinary prologue."""
+        After a per-image run the shadows of stopped images are stale: the next forward takes the ordinary prologue.
+        Under graph capture the call neither resumes nor leaves a resume record (its workspace is its graph's own), and
+        the record of the last eager call stays valid."""
         device = tokens.device
         b, n = tokens.shape[0], tokens.shape[1]
-        resume, self._resume = self._resume, None
+        capturing = _capturing()
+        resume = None
+        if capturing:
+            allow_resume = False
+        else:
+            resume, self._resume = self._resume, None
         plain = steps is None and tol is None
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
@@ -524,9 +608,15 @@ class Glom(nn.Module):
     def _parse_iters(self, iters, b):
         """-> (iters, steps): a scalar step count and None, or, for a per-image vector whose entries differ, its maximum
         and the vector itself (the caller's tensor, or an int64 CPU tensor made from a list).  Reads min / max of a
-        vector once on the host."""
+        vector once on the host, so under graph capture only an int or a CPU scalar tensor is accepted."""
         if iters is None:
             return self.levels * 2, None                                     # (:112)
+        if _capturing() and (isinstance(iters, (list, tuple))
+                             or isinstance(iters, torch.Tensor) and (iters.dim() > 0 or iters.is_cuda)):
+            raise ValueError("forward(iters=...) with a per-image list or tensor, or a CUDA scalar, reads the step counts "
+                             "on the host, which CUDA graph capture cannot do: capture with an int iters, or let the GPU "
+                             "pick each image's steps with settle(img, tol, levels=..., differentiable=True), which is "
+                             "capturable")
         if isinstance(iters, (list, tuple)):
             try:
                 iters = torch.tensor([operator.index(v) for v in iters], dtype=torch.int64)
@@ -587,7 +677,7 @@ class Glom(nn.Module):
         _SettleImplicit with `adjoint` = (adjoint_tol, adjoint_iters) (settle(differentiable="implicit"))."""
         _, n = self._check_input(img, levels)
         if not needs_grad:
-            tokens = self._take_staged(img)
+            tokens = None if _capturing() else self._take_staged(img)      # a graph tokenises for itself
             if tokens is None:
                 tokens = self.tokens(img)                                    # (:114) engine tokeniser
             return self._run(tokens, self.pos_emb.weight[:n], levels, self.init_levels, iters, return_all, steps=steps,
@@ -738,6 +828,8 @@ class Glom(nn.Module):
 
     def _slot_args(self, name, img, levels, tol, max_iters, slots):
         """The argument checks of settle_queue / settle_video -> (tol, max_iters, slots)."""
+        _no_capture(f"Glom.{name}", "its host loop reads the number of unfinished images between engine calls; capture "
+                                    "settle(img, tol, ...) on fixed batches instead (differentiable=True for training)")
         if self.precision != "bf16":
             raise RuntimeError(f"Glom.{name} needs precision='bf16' (the fp32 engine has no early stopping)")
         _require_cuda(img)

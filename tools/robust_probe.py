@@ -34,7 +34,7 @@ with torch.no_grad():
         g = torch.cuda.CUDAGraph()
         s2 = torch.cuda.Stream(); s2.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s2):
-            b(static_x, iters=2)                    # warm-up on the capture stream (allocations, packed weights)
+            b(static_x, iters=2)                    # eager warm-up on a side stream; the capture packs and allocates its own
         torch.cuda.current_stream().wait_stream(s2)
         with torch.cuda.graph(g):
             static_y = b(static_x, iters=2)
