@@ -91,11 +91,10 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(GemmF32 q) {
   }
 }
 
-static cudaError_t gemm_f32(const GemmF32& q, int batches, cudaStream_t st, int* launches) {
+static int gemm_f32(const GemmF32& q, int batches, Launch& ln) {
   dim3 grid((q.M + 63) / 64, (q.N + 63) / 64, batches);
-  gemm_f32_kernel<<<grid, 256, 0, st>>>(q);
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  gemm_f32_kernel<<<grid, 256, 0, ln.st>>>(q);
+  return ln.launched();
 }
 
 // =====================================================================================
@@ -332,14 +331,14 @@ __global__ void __launch_bounds__(1024) colsum_det_kernel(int rows, int cols, lo
     if (out2 && c < cols2) out2[c] += s;
   }
 }
-static cudaError_t colsum(bool det, int rows, int cols, long long row_stride, const float* src, float* out, float* out2,
-                          int cols2, const int32_t* steps, int t, int n, cudaStream_t st, int* launches) {
+static int colsum(bool det, int rows, int cols, long long row_stride, const float* src, float* out, float* out2, int cols2,
+                  const int32_t* steps, int t, int n, Launch& ln) {
+  cudaStream_t st = ln.st;
   if (det)
     colsum_det_kernel<<<(cols + 31) / 32, dim3(32, 32), 0, st>>>(rows, cols, row_stride, src, out, out2, cols2, steps, t, n);
   else
     colsum_acc_kernel<<<dim3((cols + 31) / 32, 16), 256, 0, st>>>(rows, cols, row_stride, src, out, out2, cols2, steps, t, n);
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  return ln.launched();
 }
 // After BW_DX<DET>: ds[r, l + 1] += dx_td[r, l] for the top-down groups l = 0 .. L-2, and dpos[i] += the sum of
 // dx_td[b n + i, l] over images b, and groups l within an image.  Block = 32 float4 columns x 8 image slices of one
@@ -452,19 +451,17 @@ size_t tokenize_backward_workspace_bytes(int B, int H, int W, int p, int need_di
   return align_up(rk, 1024) * (need_dimg ? 2 : 1);
 }
 
-cudaError_t tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight, float* d_bias,
-                              float* d_img, int B, int H, int W, int p, int d, void* workspace, cudaStream_t st, int* launches,
-                              int deterministic) {
+int tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight, float* d_bias,
+                      float* d_img, int B, int H, int W, int p, int d, void* workspace, Launch& ln, int deterministic) {
+  cudaStream_t st = ln.st;
   const int rows = B * (H / p) * (W / p), k3 = 3 * p * p;
   float* patches = static_cast<float*>(workspace);
   float* dpatches = reinterpret_cast<float*>(static_cast<char*>(workspace) + align_up((size_t)rows * k3 * sizeof(float), 1024));
-  cudaError_t e = cudaSuccess;
   if (d_weight) {
     const size_t total = (size_t)rows * k3;
     const size_t want = (total + 255) / 256;
     patchify_f32_kernel<<<(int)(want < sm_count() * 32 ? want : sm_count() * 32), 256, 0, st>>>(img, patches, B, H, W, p);
-    if (launches) ++*launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    GLOM_TRY(ln.launched());
     // d_weight (d, k3) += dTok^T (d x rows) . patches (rows x k3)
     GemmF32 q{};
     q.M = d; q.N = k3; q.K = rows; q.zdiv = 1;
@@ -472,11 +469,9 @@ cudaError_t tokenize_backward(const float* img, const float* weight, const float
     q.B = {patches, k3, 1, 0, 0};
     q.C = {d_weight, k3, 1, 0, 0};
     q.alpha = 1.f; q.beta = 1.f; q.bias = nullptr;
-    if ((e = gemm_f32(q, 1, st, launches)) != cudaSuccess) return e;
+    GLOM_TRY(gemm_f32(q, 1, ln));
   }
-  if (d_bias && (e = colsum(deterministic != 0, rows, d, (long long)d, d_tokens, d_bias, nullptr, 0, nullptr, 0, 1, st,
-                            launches)) != cudaSuccess)
-    return e;
+  if (d_bias) GLOM_TRY(colsum(deterministic != 0, rows, d, (long long)d, d_tokens, d_bias, nullptr, 0, nullptr, 0, 1, ln));
   if (d_img) {
     // dpatches (rows, k3) = dTok (rows x d) . W (d x k3)
     GemmF32 q{};
@@ -485,14 +480,13 @@ cudaError_t tokenize_backward(const float* img, const float* weight, const float
     q.B = {weight, k3, 1, 0, 0};
     q.C = {dpatches, k3, 1, 0, 0};
     q.alpha = 1.f; q.beta = 0.f; q.bias = nullptr;
-    if ((e = gemm_f32(q, 1, st, launches)) != cudaSuccess) return e;
+    GLOM_TRY(gemm_f32(q, 1, ln));
     const size_t total = (size_t)B * 3 * H * W;
     const size_t want = (total + 255) / 256;
     unpatchify_add_kernel<<<(int)(want < sm_count() * 32 ? want : sm_count() * 32), 256, 0, st>>>(dpatches, d_img, B, H, W, p);
-    if (launches) ++*launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    GLOM_TRY(ln.launched());
   }
-  return cudaSuccess;
+  return 0;
 }
 
 __global__ void cast_bf16_rows(size_t n4, const float* __restrict__ src, __nv_bfloat16* __restrict__ dst) {
@@ -506,8 +500,6 @@ static inline int nblk(size_t total, int block = 256) {
   const size_t want = (total + block - 1) / block;
   return (int)(want < (size_t)sm_count() * 32 ? (want ? want : 1) : (size_t)sm_count() * 32);
 }
-#define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return e_; } while (0)
-#define CKL() do { if (launches) ++*launches; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) return e_; } while (0)
 
 BackwardLayout backward_layout(const Geometry& g, int precision) {
   BackwardLayout w{};
@@ -546,23 +538,36 @@ BackwardLayout backward_layout(const Geometry& g, int precision) {
   return w;
 }
 
+// The buffers of a backward workspace (the bf16 ones: tensor-core path only, see backward_layout)
+struct BackwardBuffers {
+  float *g, *gs, *ds, *khat, *dkhat, *rnorm, *pre, *h, *dh, *xp, *dx, *attn, *dattn;
+  __nv_bfloat16 *xb, *sb, *sp, *gsb, *w1p, *w2t, *w1t, *bpre, *bh, *bdpre, *khat_b, *a_b, *dsim_b;
+  float *b1p, *b1_part;
+};
+static BackwardBuffers backward_buffers(const BackwardLayout& wl, void* workspace) {
+  char* ws = static_cast<char*>(workspace);
+  auto f32 = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
+  auto b16 = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(ws + off); };
+  return {f32(wl.g_off), f32(wl.gs_off), f32(wl.ds_off), f32(wl.khat_off), f32(wl.dkhat_off), f32(wl.rnorm_off),
+          f32(wl.pre_off), f32(wl.h_off), f32(wl.dh_off), f32(wl.xp_off), f32(wl.dx_off), f32(wl.attn_off), f32(wl.dattn_off),
+          b16(wl.xb_off), b16(wl.sb_off), b16(wl.sp_off), b16(wl.gsb_off), b16(wl.w1p_off), b16(wl.w2t_off), b16(wl.w1t_off),
+          b16(wl.bpre_off), b16(wl.bh_off), b16(wl.bdpre_off), b16(wl.khatb_off), b16(wl.ab_off), b16(wl.dsimb_off),
+          f32(wl.b1p_off), f32(wl.b1part_off)};
+}
+
 // One reverse step: given gin = dL/dS_{t+1}, produce ds = dL/dS_t (without the external grad of slab t) and
 // accumulate parameter / token / pos gradients.
-static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const float* s_t, const float* gin,
-                                 const float* gextra, float* ds, char* ws, const BackwardLayout& wl, bool mlp_on_tc,
-                                 bool attn_on_tc, const int32_t* steps, int t, bool gs_kept, cudaStream_t st, int* launches) {
+static int backward_step(const Geometry& g, const BackwardArgs& a, const float* s_t, const float* gin, const float* gextra,
+                         float* ds, const BackwardBuffers& w, bool mlp_on_tc, bool attn_on_tc, const int32_t* steps, int t,
+                         bool gs_kept, Launch& ln) {
   const int R = g.rows, L = g.L, d = g.d, n = g.n, h4 = 4 * g.d;
   const long long ld = (long long)L * d;
-  float* gs = reinterpret_cast<float*>(ws + wl.gs_off);       // (gin + gextra) / c
-  float* pre = reinterpret_cast<float*>(ws + wl.pre_off);
-  float* hb = reinterpret_cast<float*>(ws + wl.h_off);
-  float* dh = reinterpret_cast<float*>(ws + wl.dh_off);
-  float* xp = reinterpret_cast<float*>(ws + wl.xp_off);
-  float* dx = reinterpret_cast<float*>(ws + wl.dx_off);
+  cudaStream_t st = ln.st;
+  float *gs = w.gs /* (gin + gextra) / c */, *pre = w.pre, *hb = w.h, *dh = w.dh, *xp = w.xp, *dx = w.dx;
   const size_t state = (size_t)R * L * d;
   scale_by_contrib_kernel<<<nblk(state), 256, 0, st>>>(state, L, d, gin, gextra, gs, ds, steps, t, (size_t)n * ld / 4,
                                                        gs_kept ? 1 : 0);
-  CKL();
+  GLOM_TRY(ln.launched());
 
   // ---- the two grouped MLPs (:23-36), one group at a time (fp32 path; the bf16 engine runs them on tensor cores)
   for (int net = 0; net < 2 && !mlp_on_tc; ++net) {
@@ -581,7 +586,7 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
       else if (net == 0) X = Mat{s_t + (size_t)(l - 1) * d, ld, 1, 0, 0};
       else {
         add_pos_kernel<<<nblk((size_t)R * d), 256, 0, st>>>(R, n, L, d, l + 1, s_t, a.pos, xp);
-        CKL();
+        GLOM_TRY(ln.launched());
         X = Mat{xp, d, 1, 0, 0};
       }
       const float* W1 = w1 + (size_t)l * h4 * d;       // (4d, d)
@@ -590,80 +595,76 @@ static cudaError_t backward_step(const Geometry& g, const BackwardArgs& a, const
       GemmF32 q{};
       // pre = X W1^T + b1                                 (R x 4d)
       q = GemmF32{R, h4, d, 1, X, Mat{W1, 1, d, 0, 0}, MatOut{pre, h4, 1, 0, 0}, 1.f, 0.f, b1 + (size_t)l * h4};
-      CK(gemm_f32(q, 1, st, launches));
+      GLOM_TRY(gemm_f32(q, 1, ln));
       // dh = DY W2                                        (R x 4d)
       q = GemmF32{R, h4, d, 1, DY, Mat{W2, h4, 1, 0, 0}, MatOut{dh, h4, 1, 0, 0}, 1.f, 0.f, nullptr};
-      CK(gemm_f32(q, 1, st, launches));
+      GLOM_TRY(gemm_f32(q, 1, ln));
       gelu_bwd_kernel<<<nblk((size_t)R * h4), 256, 0, st>>>((size_t)R * h4, pre, hb, dh);   // dh := dpre
-      CKL();
+      GLOM_TRY(ln.launched());
       if (!a.state_only) {
         // dW2 += DY^T h                                     (d x 4d)
         q = GemmF32{d, h4, R, 1, Mat{DY.p, 1, ld, 0, 0}, Mat{hb, h4, 1, 0, 0}, MatOut{dw2 + (size_t)l * d * h4, h4, 1, 0, 0}, 1.f, 1.f, nullptr};
-        CK(gemm_f32(q, 1, st, launches));
-        CK(colsum(a.deterministic != 0, R, d, ld, DY.p, db2 + (size_t)l * d, nullptr, 0, nullptr, 0, 1, st, launches));
+        GLOM_TRY(gemm_f32(q, 1, ln));
+        GLOM_TRY(colsum(a.deterministic != 0, R, d, ld, DY.p, db2 + (size_t)l * d, nullptr, 0, nullptr, 0, 1, ln));
         // dW1 += dpre^T X                                   (4d x d)
         q = GemmF32{h4, d, R, 1, Mat{dh, 1, h4, 0, 0}, Mat{X.p, X.s_row, 1, 0, 0}, MatOut{dw1 + (size_t)l * h4 * d, d, 1, 0, 0}, 1.f, 1.f, nullptr};
-        CK(gemm_f32(q, 1, st, launches));
-        CK(colsum(a.deterministic != 0, R, h4, h4, dh, db1 + (size_t)l * h4, nullptr, 0, nullptr, 0, 1, st, launches));
+        GLOM_TRY(gemm_f32(q, 1, ln));
+        GLOM_TRY(colsum(a.deterministic != 0, R, h4, h4, dh, db1 + (size_t)l * h4, nullptr, 0, nullptr, 0, 1, ln));
       }
       // dX = dpre W1                                      (R x d)
       q = GemmF32{R, d, h4, 1, Mat{dh, h4, 1, 0, 0}, Mat{W1, d, 1, 0, 0}, MatOut{dx, d, 1, 0, 0}, 1.f, 0.f, nullptr};
-      CK(gemm_f32(q, 1, st, launches));
+      GLOM_TRY(gemm_f32(q, 1, ln));
       if (net == 0 && l == 0) {
         if (a.state_only) continue;     // the tokens are no state
         add_kernel<<<nblk((size_t)R * d), 256, 0, st>>>((size_t)R * d, dx, a.d_tokens);
-        CKL();
+        GLOM_TRY(ln.launched());
       } else if (net == 0) {
         add_into_level_kernel<<<nblk((size_t)R * d), 256, 0, st>>>(R, L, d, l - 1, dx, ds);
-        CKL();
+        GLOM_TRY(ln.launched());
       } else {
         add_into_level_kernel<<<nblk((size_t)R * d), 256, 0, st>>>(R, L, d, l + 1, dx, ds);
-        CKL();
+        GLOM_TRY(ln.launched());
         if (a.state_only) continue;
         pos_grad_kernel<<<nblk((size_t)n * d), 256, 0, st>>>(g.B, n, d, dx, a.d_pos);
-        CKL();
+        GLOM_TRY(ln.launched());
       }
     }
   }
 
   // ---- consensus attention (:56-73), all (image, level) problems batched (fp32 path)
   if (!attn_on_tc && !a.skip_attn) {
-    float* khat = reinterpret_cast<float*>(ws + wl.khat_off);
-    float* dkhat = reinterpret_cast<float*>(ws + wl.dkhat_off);
-    float* rnorm = reinterpret_cast<float*>(ws + wl.rnorm_off);
-    float* A = reinterpret_cast<float*>(ws + wl.attn_off);
-    float* dA = reinterpret_cast<float*>(ws + wl.dattn_off);
+    float *khat = w.khat, *dkhat = w.dkhat, *rnorm = w.rnorm, *A = w.attn, *dA = w.dattn;
     const int Z = g.B * L;
     const long long sb = (long long)n * ld, sl = d, nn = (long long)n * n;
     const float scale = 1.0f / sqrtf((float)d);
     const int wblocks = (R * L * 32 + 255) / 256;
     const FrozenRows all_rows{nullptr, 0, 1};           // masked by gs = 0 instead
     normalize_rows_kernel<<<wblocks, 256, 0, st>>>(R * L, d, s_t, khat, rnorm, nullptr, all_rows);
-    CKL();
+    GLOM_TRY(ln.launched());
     GemmF32 q{};
     // sim = scale * Q Khat^T                              (n x n per (b, l))
     q = GemmF32{n, n, d, L, Mat{s_t, ld, 1, sb, sl}, Mat{khat, 1, ld, sb, sl}, MatOut{A, n, 1, nn * L, nn}, 1.f, 0.f, nullptr};
-    CK(gemm_f32(q, Z, st, launches));
+    GLOM_TRY(gemm_f32(q, Z, ln));
     attn_softmax_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, nullptr, all_rows);
-    CKL();
+    GLOM_TRY(ln.launched());
     // dA = dC V^T
     q = GemmF32{n, n, d, L, Mat{gs, ld, 1, sb, sl}, Mat{s_t, 1, ld, sb, sl}, MatOut{dA, n, 1, nn * L, nn}, 1.f, 0.f, nullptr};
-    CK(gemm_f32(q, Z, st, launches));
+    GLOM_TRY(gemm_f32(q, Z, ln));
     // dV: ds += A^T dC
     q = GemmF32{n, d, n, L, Mat{A, 1, n, nn * L, nn}, Mat{gs, ld, 1, sb, sl}, MatOut{ds, ld, 1, sb, sl}, 1.f, 1.f, nullptr};
-    CK(gemm_f32(q, Z, st, launches));
+    GLOM_TRY(gemm_f32(q, Z, ln));
     attn_softmax_bwd_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, 1.f, nullptr, all_rows);
-    CKL();
+    GLOM_TRY(ln.launched());
     // dQ: ds += scale * dsim Khat
     q = GemmF32{n, d, n, L, Mat{dA, n, 1, nn * L, nn}, Mat{khat, ld, 1, sb, sl}, MatOut{ds, ld, 1, sb, sl}, scale, 1.f, nullptr};
-    CK(gemm_f32(q, Z, st, launches));
+    GLOM_TRY(gemm_f32(q, Z, ln));
     // dKhat = scale * dsim^T Q
     q = GemmF32{n, d, n, L, Mat{dA, 1, n, nn * L, nn}, Mat{s_t, ld, 1, sb, sl}, MatOut{dkhat, ld, 1, sb, sl}, scale, 0.f, nullptr};
-    CK(gemm_f32(q, Z, st, launches));
+    GLOM_TRY(gemm_f32(q, Z, ln));
     normalize_bwd_kernel<<<wblocks, 256, 0, st>>>(R * L, d, khat, dkhat, rnorm, ds, all_rows);
-    CKL();
+    GLOM_TRY(ln.launched());
   }
-  return cudaSuccess;
+  return 0;
 }
 
 // =====================================================================================
@@ -723,49 +724,41 @@ __global__ void bwd_shadows_kernel(int rows, int n, int L, int d, const float* _
 }
 
 int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int iters, int grad_all, const int32_t* steps,
-                 void* workspace, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen) {
-#define CKI(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { snprintf(err, errlen, "backward: %s", cudaGetErrorString(e_)); return -3; } } while (0)
-#define CKLI() do { if (launches) ++*launches; CKI(cudaGetLastError()); } while (0)
+                 void* workspace, Launch& ln) {
+  // a failure of a launcher shared with the tokeniser backward, in this call's words
+  auto mine = [&](int r) { return r ? ln.fail(r, "backward: %s", ln.err) : 0; };
   const BackwardLayout wl = backward_layout(g, precision);
+  const BackwardBuffers w = backward_buffers(wl, workspace);
   const bool tc = precision == 1 && g.d % 256 == 0;
   const bool attn_tc = tc && g.n % 8 == 0;      // TMA row pitch of the (Z, n, n) bf16 buffers must be a multiple of 16 B
-  char* ws = static_cast<char*>(workspace);
+  cudaStream_t st = ln.st;
   const size_t state = (size_t)g.rows * g.L * g.d;
   // gradient w.r.t. the state walks backwards through two ping-pong slabs: step t reads (gin + gextra) and writes ds
-  float* slab[2] = {reinterpret_cast<float*>(ws + wl.ds_off), reinterpret_cast<float*>(ws + wl.g_off)};
-  float* gs = reinterpret_cast<float*>(ws + wl.gs_off);
+  float* slab[2] = {w.ds, w.g};
+  float* gs = w.gs;
   MlpBwdTc m{};
   if (tc) {
-    m.xb = reinterpret_cast<__nv_bfloat16*>(ws + wl.xb_off);
-    m.sb = reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off);
-    m.sp = reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off);
-    m.gsb = reinterpret_cast<__nv_bfloat16*>(ws + wl.gsb_off);
-    m.w1p = reinterpret_cast<__nv_bfloat16*>(ws + wl.w1p_off);
-    m.w2t = reinterpret_cast<__nv_bfloat16*>(ws + wl.w2t_off);
-    m.w1t = reinterpret_cast<__nv_bfloat16*>(ws + wl.w1t_off);
-    m.b1p = reinterpret_cast<float*>(ws + wl.b1p_off);
-    m.pre = reinterpret_cast<__nv_bfloat16*>(ws + wl.bpre_off);
-    m.h = reinterpret_cast<__nv_bfloat16*>(ws + wl.bh_off);
-    m.dpre = reinterpret_cast<__nv_bfloat16*>(ws + wl.bdpre_off);
+    m.xb = w.xb; m.sb = w.sb; m.sp = w.sp; m.gsb = w.gsb;
+    m.w1p = w.w1p; m.w2t = w.w2t; m.w1t = w.w1t; m.b1p = w.b1p;
+    m.pre = w.bpre; m.h = w.bh; m.dpre = w.bdpre;
     m.d_tokens = a.d_tokens; m.d_pos = a.d_pos;
     m.d_bu_w1 = a.d_bu_w1; m.d_bu_w2 = a.d_bu_w2; m.d_td_w1 = a.d_td_w1; m.d_td_w2 = a.d_td_w2;
     m.d_bu_b1 = a.d_bu_b1; m.d_td_b1 = a.d_td_b1;
     m.deterministic = a.deterministic;
-    m.dx_td = reinterpret_cast<float*>(ws + wl.dkhat_off);
-    m.b1_part = reinterpret_cast<float*>(ws + wl.b1part_off);
+    m.dx_td = w.dkhat;
+    m.b1_part = w.b1_part;
     m.skip_pre = a.relin; m.skip_dw = a.state_only;
   }
   if (tc && !a.relin) {     // the weights and tokens of this call (relin: still in the workspace)
     pack_bwd_weights_kernel<<<sm_count() * 8, 256, 0, st>>>(g.d, g.L, a.bu_w1, a.bu_b1, a.bu_w2, a.td_w1, a.td_b1, a.td_w2,
-                                                     const_cast<__nv_bfloat16*>(m.w1p), const_cast<__nv_bfloat16*>(m.w2t),
-                                                     const_cast<__nv_bfloat16*>(m.w1t), const_cast<float*>(m.b1p));
-    CKLI();
+                                                     w.w1p, w.w2t, w.w1t, w.b1p);
+    GLOM_TRY(ln.launched("backward"));
     const size_t n4 = (size_t)g.rows * g.d / 4;
-    cast_bf16_rows<<<nblk(n4), 256, 0, st>>>(n4, a.tokens, const_cast<__nv_bfloat16*>(m.xb));
-    CKLI();
+    cast_bf16_rows<<<nblk(n4), 256, 0, st>>>(n4, a.tokens, w.xb);
+    GLOM_TRY(ln.launched("backward"));
     if (g.rows % 128) {     // rows of the last 128-row block beyond R are read as K entries of the dW GEMMs: keep them zero
-      CKI(cudaMemsetAsync(m.h, 0, wl.blocked_bytes, st));
-      CKI(cudaMemsetAsync(m.dpre, 0, wl.blocked_bytes, st));
+      GLOM_TRY(ln.check(cudaMemsetAsync(m.h, 0, wl.blocked_bytes, st), "backward"));
+      GLOM_TRY(ln.check(cudaMemsetAsync(m.dpre, 0, wl.blocked_bytes, st), "backward"));
     }
   }
   // pending upstream gradient of S_{t+1}: gin (+ gextra, the cotangent of that step's own output under return_all)
@@ -779,72 +772,61 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
     // reverse step at which every image is frozen (t >= max(steps), the tail of a settle_all backward) then only passes
     // ds = gin + gextra through; its other launches find no work.
     const int32_t* kept = (steps && t < iters - 1) ? steps : nullptr;
-    CKI(backward_step(g, a, s_t, gin, gextra, ds, ws, wl, tc, attn_tc, steps, t, kept != nullptr, st,
-                      launches));   // scale (+ the fp32 MLP / attention backward)
+    GLOM_TRY(mine(backward_step(g, a, s_t, gin, gextra, ds, w, tc, attn_tc, steps, t, kept != nullptr,
+                                ln)));   // scale (+ the fp32 MLP / attention backward)
     if (tc) {
       if (a.relin) {      // sb / sp hold this state's shadows: only the cotangent changes (frozen rows: gs = 0 -> gsb = 0)
-        cast_bf16_rows<<<nblk(state / 4), 256, 0, st>>>(state / 4, gs, const_cast<__nv_bfloat16*>(m.gsb));
+        cast_bf16_rows<<<nblk(state / 4), 256, 0, st>>>(state / 4, gs, w.gsb);
       } else {
-        bwd_shadows_kernel<<<nblk(state / 4), 256, 0, st>>>(g.rows, g.n, g.L, g.d, s_t, gs, a.pos,
-                                                            const_cast<__nv_bfloat16*>(m.sb), const_cast<__nv_bfloat16*>(m.sp),
-                                                            const_cast<__nv_bfloat16*>(m.gsb), kept, t);
+        bwd_shadows_kernel<<<nblk(state / 4), 256, 0, st>>>(g.rows, g.n, g.L, g.d, s_t, gs, a.pos, w.sb, w.sp, w.gsb, kept, t);
       }
-      CKLI();
+      GLOM_TRY(ln.launched("backward"));
       // ---- consensus attention backward: the five (n x n x d) GEMM families on tensor cores, softmax in fp32.  With
       // per-image step counts, the problems / rows of images frozen at step t are skipped in every launch (their
       // contribution to ds is an exact zero); the buffers they would have written are left stale and read by no one.
       // relin: khat / rnorm / khat_b and the probabilities A / a_b of this state are already there
       if (attn_tc && !a.skip_attn) {
-        float* khat = reinterpret_cast<float*>(ws + wl.khat_off);
-        float* dkhat = reinterpret_cast<float*>(ws + wl.dkhat_off);
-        float* rnorm = reinterpret_cast<float*>(ws + wl.rnorm_off);
-        float* A = reinterpret_cast<float*>(ws + wl.attn_off);
-        float* dA = reinterpret_cast<float*>(ws + wl.dattn_off);
-        __nv_bfloat16* khat_b = reinterpret_cast<__nv_bfloat16*>(ws + wl.khatb_off);
-        __nv_bfloat16* a_b = reinterpret_cast<__nv_bfloat16*>(ws + wl.ab_off);
-        __nv_bfloat16* dsim_b = reinterpret_cast<__nv_bfloat16*>(ws + wl.dsimb_off);
+        float *khat = w.khat, *dkhat = w.dkhat, *rnorm = w.rnorm, *A = w.attn, *dA = w.dattn;
+        __nv_bfloat16 *khat_b = w.khat_b, *a_b = w.a_b, *dsim_b = w.dsim_b;
         const int Z = g.B * g.L, n = g.n, d = g.d;
         const float scale = 1.0f / sqrtf((float)d);
         const int wblocks = (g.rows * g.L * 32 + 255) / 256, rblocks = (Z * n * 32 + 255) / 256;
         const FrozenRows frozen{steps, t, n * g.L};
         if (!a.relin) {
           normalize_rows_kernel<<<wblocks, 256, 0, st>>>(g.rows * g.L, d, s_t, khat, rnorm, khat_b, frozen);
-          CKLI();
+          GLOM_TRY(ln.launched("backward"));
           // logits = Q Khat^T (scaled inside the softmax)
-          if (int r = attn_bwd_gemm_tc(g, m.sb, 1, 0, khat_b, 1, 0, n, d, 0, A, steps, t, enc, num_sms, st, launches, err,
-                                       errlen)) return r;
+          GLOM_TRY(attn_bwd_gemm_tc(g, {w.sb, 1, 0}, {khat_b, 1, 0}, n, d, 0, A, steps, t, ln));
           attn_softmax_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, a_b, frozen);
-          CKLI();
+          GLOM_TRY(ln.launched("backward"));
         }
         // dA = dC V^T
-        if (int r = attn_bwd_gemm_tc(g, m.gsb, 1, 0, m.sb, 1, 0, n, d, 0, dA, steps, t, enc, num_sms, st, launches, err,
-                                     errlen)) return r;
+        GLOM_TRY(attn_bwd_gemm_tc(g, {w.gsb, 1, 0}, {w.sb, 1, 0}, n, d, 0, dA, steps, t, ln));
         attn_softmax_bwd_kernel<<<rblocks, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, scale, dsim_b,
                                                          frozen);
-        CKLI();
+        GLOM_TRY(ln.launched("backward"));
         // dV and dQ in one K-concatenated product: ds += [A^T | scale dsim] [dC ; Khat] ;  dKhat = (scale dsim)^T Q
-        if (int r = attn_bwd_gemm_tc(g, a_b, 0, 1, m.gsb, 1, 1, d, n, 1, ds, steps, t, enc, num_sms, st, launches, err, errlen,
-                                     dsim_b, 0, 0, khat_b, 1, 1)) return r;
-        if (int r = attn_bwd_gemm_tc(g, dsim_b, 0, 1, m.sb, 1, 1, d, n, 2, dkhat, steps, t, enc, num_sms, st, launches, err,
-                                     errlen)) return r;
+        GLOM_TRY(attn_bwd_gemm_tc(g, {a_b, 0, 1}, {w.gsb, 1, 1}, d, n, 1, ds, steps, t, ln, {dsim_b, 0, 0}, {khat_b, 1, 1}));
+        GLOM_TRY(attn_bwd_gemm_tc(g, {dsim_b, 0, 1}, {w.sb, 1, 1}, d, n, 2, dkhat, steps, t, ln));
         normalize_bwd_kernel<<<wblocks, 256, 0, st>>>(g.rows * g.L, d, khat, dkhat, rnorm, ds, frozen);
-        CKLI();
+        GLOM_TRY(ln.launched("backward"));
       }
       m.ds = ds;
       m.steps = steps; m.t = t;
-      if (int r = mlp_backward_tc(g, m, enc, num_sms, st, launches, err, errlen)) return r;
+      GLOM_TRY(mlp_backward_tc(g, m, ln));
       if (a.deterministic && !a.state_only) {     // what the default DH / DX epilogues reduce with atomics, in a fixed order
         bias_partials_kernel<<<(g.G * g.d + 31) / 32, dim3(32, 16), 0, st>>>(g.G, (g.rows + 31) / 32, g.rows, g.n, g.d,
                                                                              m.b1_part, a.d_bu_b1, a.d_td_b1, steps, t);
-        CKLI();
+        GLOM_TRY(ln.launched("backward"));
       }
       if (a.deterministic) {
         dx_td_reduce_kernel<<<g.n * ((g.d / 4 + 31) / 32), dim3(32, 8), 0, st>>>(g.B, g.n, g.L, g.d, m.dx_td, ds, a.d_pos,
                                                                                   steps, t);
-        CKLI();
+        GLOM_TRY(ln.launched("backward"));
       }
-      if (!a.state_only) CKI(colsum(a.deterministic != 0, g.rows, g.L * g.d, (long long)g.L * g.d, gs, a.d_bu_b2, a.d_td_b2, (g.L - 1) * g.d,
-                 steps, t, g.n, st, launches));
+      if (!a.state_only)
+        GLOM_TRY(mine(colsum(a.deterministic != 0, g.rows, g.L * g.d, (long long)g.L * g.d, gs, a.d_bu_b2, a.d_td_b2,
+                             (g.L - 1) * g.d, steps, t, g.n, ln)));
     }
     gin = ds;
     gextra = grad_all ? a.grad_out + (size_t)t * state : nullptr;
@@ -854,18 +836,16 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
     if (!part) continue;
     if (a.d_state0) {
       add_kernel<<<nblk(state), 256, 0, st>>>(state, part, a.d_state0);
-      CKLI();
+      GLOM_TRY(ln.launched("backward"));
     }
     if (a.d_init && a.deterministic) {
-      CKI(colsum(true, g.rows, g.L * g.d, (long long)g.L * g.d, part, a.d_init, nullptr, 0, nullptr, 0, 1, st, launches));
+      GLOM_TRY(mine(colsum(true, g.rows, g.L * g.d, (long long)g.L * g.d, part, a.d_init, nullptr, 0, nullptr, 0, 1, ln)));
     } else if (a.d_init) {
       init_grad_kernel<<<dim3((g.L * g.d + 255) / 256, 64), 256, 0, st>>>(g.rows, g.L, g.d, part, a.d_init);
-      CKLI();
+      GLOM_TRY(ln.launched("backward"));
     }
   }
   return 0;
-#undef CKI
-#undef CKLI
 }
 
 // =====================================================================================
@@ -931,10 +911,9 @@ ImplicitLayout implicit_layout(const Geometry& g) {
 }
 
 int backward_implicit_run(const Geometry& g, const BackwardArgs& a, int adjoint_iters, float adjoint_tol,
-                          int32_t* adjoint_steps, float* adjoint_q, void* workspace, EncodeTiledFn enc, int num_sms,
-                          cudaStream_t st, int* launches, char* err, size_t errlen) {
-#define CKI(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { snprintf(err, errlen, "backward_implicit: %s", cudaGetErrorString(e_)); return -3; } } while (0)
-#define CKLI() do { if (launches) ++*launches; CKI(cudaGetLastError()); } while (0)
+                          int32_t* adjoint_steps, float* adjoint_q, void* workspace, Launch& ln) {
+  const char* const me = "backward_implicit";
+  cudaStream_t st = ln.st;
   const ImplicitLayout il = implicit_layout(g);
   char* ws = static_cast<char*>(workspace);
   const size_t state = (size_t)g.rows * g.L * g.d;
@@ -946,9 +925,9 @@ int backward_implicit_run(const Geometry& g, const BackwardArgs& a, int adjoint_
   float* level_q = reinterpret_cast<float*>(ws + il.level_q_off);
   // a one-step backward_run leaves dL/dS_0 = J^T u in the first slab of its ping-pong
   const float* jtu = reinterpret_cast<const float*>(ws + il.bwd.ds_off);
-  CKI(cudaMemsetAsync(ws + il.flags_off, 0, il.flags_bytes, st));
-  CKI(cudaMemsetAsync(adjoint_steps, 0, (size_t)g.B * 4, st));
-  CKI(cudaMemcpyAsync(u, a.grad_out, state * 4, cudaMemcpyDeviceToDevice, st));
+  GLOM_TRY(ln.check(cudaMemsetAsync(ws + il.flags_off, 0, il.flags_bytes, st), me));
+  GLOM_TRY(ln.check(cudaMemsetAsync(adjoint_steps, 0, (size_t)g.B * 4, st), me));
+  GLOM_TRY(ln.check(cudaMemcpyAsync(u, a.grad_out, state * 4, cudaMemcpyDeviceToDevice, st), me));
   // adjoint passes: dL/dS only, fixed-order reductions, token / pos rows into scratch
   BackwardArgs p = a;
   p.grad_out = u;
@@ -963,12 +942,13 @@ int backward_implicit_run(const Geometry& g, const BackwardArgs& a, int adjoint_
   for (int k = 1; k <= adjoint_iters; ++k) {
     p.relin = k > 1;                                 // pass 1 linearises at S*, for every image (none has stopped)
     implicit_stop_kernel<<<(g.B + 255) / 256, 256, 0, st>>>(g.B, frozen, stop);
-    CKLI();
-    if (int r = backward_run(g, p, 1, 1, 0, stop, workspace, enc, num_sms, st, launches, err, errlen)) return r;
+    GLOM_TRY(ln.launched(me));
+    GLOM_TRY(backward_run(g, p, 1, 1, 0, stop, workspace, ln));
     implicit_update_kernel<<<ublocks, 256, 0, st>>>(nrl, g.n, g.L, g.d, g.part_w, a.grad_out, jtu, u, dsq, nsq, frozen);
-    CKLI();
-    CKI(launch_settle_converge(g, k, adjoint_tol, dsq, nsq, frozen, reinterpret_cast<int*>(ws + il.block_frozen_off),
-                               reinterpret_cast<unsigned int*>(ws + il.done_off), level_q, adjoint_steps, st, launches));
+    GLOM_TRY(ln.launched(me));
+    if (int r = launch_settle_converge(g, k, adjoint_tol, dsq, nsq, frozen, reinterpret_cast<int*>(ws + il.block_frozen_off),
+                                       reinterpret_cast<unsigned int*>(ws + il.done_off), level_q, adjoint_steps, ln))
+      return ln.fail(r, "%s: %s", me, ln.err);
   }
   // parameter pass: one VJP at S* with cotangent u_K for every image; consensus attention has no parameters
   BackwardArgs q = a;
@@ -977,11 +957,9 @@ int backward_implicit_run(const Geometry& g, const BackwardArgs& a, int adjoint_
   q.state_only = 0;
   q.relin = adjoint_iters > 0;
   q.skip_attn = 1;
-  if (int r = backward_run(g, q, 1, 1, 0, nullptr, workspace, enc, num_sms, st, launches, err, errlen)) return r;
-  if (adjoint_q) CKI(cudaMemcpyAsync(adjoint_q, level_q, (size_t)g.B * g.L * 4, cudaMemcpyDeviceToDevice, st));
+  GLOM_TRY(backward_run(g, q, 1, 1, 0, nullptr, workspace, ln));
+  if (adjoint_q) GLOM_TRY(ln.check(cudaMemcpyAsync(adjoint_q, level_q, (size_t)g.B * g.L * 4, cudaMemcpyDeviceToDevice, st), me));
   return 0;
-#undef CKI
-#undef CKLI
 }
 
 }  // namespace glom

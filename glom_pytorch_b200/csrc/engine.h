@@ -3,11 +3,15 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <stdarg.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <stdio.h>
 #include <atomic>
 #include <mutex>
 #include <vector>
+
+#include "../../include/glom_b200.h"
 
 namespace glom {
 
@@ -114,7 +118,7 @@ struct QueueSlots {
   int images, frames, max_iters;
 };
 
-// ---- launchers (return cudaError_t of the launch; all asynchronous on `st`) -----------------
+// ---- launchers (all asynchronous on the context's stream; -> 0 or the GLOM_B200_ERR_* code of the failure) -----------
 struct Bf16Buffers {
   const float* s32_in;  float* s32_out;              // fp32 master state of step t / t+1
   int s32_in_bcast;                                   // 1: s32_in is init_levels (L, d) broadcast over the rows (step 0, no carried state)
@@ -139,25 +143,51 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+// What every host-side launcher needs besides its own operands (the tensor-map encoder, the SM count to plan for, the
+// stream, the optional profiler) and what it reports back: the launches it enqueued and the text of its failure.
+struct Launch {
+  EncodeTiledFn enc; int num_sms; cudaStream_t st; Profiler* prof;
+  int launches;                 // kernels / async copies enqueued through this context
+  char err[400];                // text of the failure
+  // A kernel (or a counted async copy) was enqueued and the runtime answered `e`: count it, then as check()
+  int launched(cudaError_t e, const char* what = nullptr) { ++launches; return check(e, what); }
+  int launched(const char* what = nullptr) { return launched(cudaGetLastError(), what); }     // after kernel<<<...>>>
+  // A runtime call that is no launch.  Failure -> GLOM_B200_ERR_CUDA, err = "[<what>: ]<the runtime's text>"
+  int check(cudaError_t e, const char* what = nullptr) {
+    if (e == cudaSuccess) return 0;
+    return what ? fail(GLOM_B200_ERR_CUDA, "%s: %s", what, cudaGetErrorString(e)) : fail(GLOM_B200_ERR_CUDA, "%s", cudaGetErrorString(e));
+  }
+  // -> code (GLOM_B200_ERR_INVALID: a shape the kernels do not support), err = the message.  The arguments may quote err
+  // itself, to put a context in front of a callee's message
+  int fail(int code, const char* fmt, ...) {
+    char msg[sizeof(err)];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(msg, sizeof(msg), fmt, ap);
+    va_end(ap);
+    snprintf(err, sizeof(err), "%s", msg);
+    return code;
+  }
+};
+#define GLOM_TRY(x) do { if (const int r_ = (x)) return r_; } while (0)
+
 // state prologue: S_0 -> fp32 master copy (dst may equal src => skipped), bf16 shadows, norms, bf16 tokens
-cudaError_t launch_prep(const Geometry& g, const float* state_in, const float* init_levels, const float* pos,
-                        const float* tokens, float* s32_dst, __nv_bfloat16* sb, __nv_bfloat16* sp,
-                        __nv_bfloat16* xb, float* nsq, cudaStream_t st, int* launches, Profiler* prof);
+int launch_prep(const Geometry& g, const float* state_in, const float* init_levels, const float* pos, const float* tokens,
+                float* s32_dst, __nv_bfloat16* sb, __nv_bfloat16* sp, __nv_bfloat16* xb, float* nsq, Launch& ln);
 
 // one Jacobi step on tensor cores, three launches: GEMM1+GELU -> H ; consensus -> C ; GEMM2+combine -> state t+1.
 // step_index: position of the step inside the forward call.  The bottom-up net of level 0 reads the tokens, which do not
 // change during a call (glom_pytorch.py:132-134), so its hidden activations (MLP group 0 of H) are computed by step 0 only
 // and re-read by GEMM2 of the later steps.
-int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTiledFn enc, int num_sms, cudaStream_t st,
-              int* launches, char* err, size_t errlen, Profiler* prof);
+int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, Launch& ln);
 
 // Glom.settle (settle_kernels.cu): the stopping rule after step `step` (one launch), and the copy of the stopped images
 // whose final state is in the workspace slab into state_out (after the last step)
 // settle queue (q != NULL): the rule is applied per running slot, which stops when it holds or its image has run
 // q->max_iters steps; steps[image] = the image's step count
-cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
-                                   int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, cudaStream_t st,
-                                   int* launches, const QueueSlots* q = nullptr);
+int launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
+                           int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, Launch& ln,
+                           const QueueSlots* q = nullptr);
 // Glom.settle_queue / Glom.settle_video (settle_kernels.cu).  init: the queue state of a new call (every slot empty, all
 // images queued).  schedule, before step t: each finished or empty slot, in slot order, hands its stopped image over to
 // the fill and, when `admit`, takes the next frame of its stream (settle_video) or else, while the queue is not empty,
@@ -165,25 +195,21 @@ cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const
 // fill, after the schedule: the handed-over images' final states from slab (S_t of the slots) into state_out, then S_0
 // of each admitted image into slab (a continuing stream's S_0 is already there), its bf16 shadows sb / sp and norm
 // partials nsq, and its bf16 token rows xb.
-cudaError_t launch_queue_init(const Geometry& g, const QueueSlots& q, int* frozen, int* block_frozen, unsigned int* done,
-                              cudaStream_t st, int* launches, Profiler* prof);
-cudaError_t launch_queue_schedule(const Geometry& g, const QueueSlots& q, int admit, int* frozen, int* block_frozen,
-                                  cudaStream_t st, int* launches, Profiler* prof);
-cudaError_t launch_queue_fill(const Geometry& g, const QueueSlots& q, const float* tokens, const float* pos,
-                              const float* state_in, const float* init_levels, float* state_out, float* slab,
-                              __nv_bfloat16* sb, __nv_bfloat16* sp, float* nsq, __nv_bfloat16* xb, cudaStream_t st,
-                              int* launches, Profiler* prof);
+int launch_queue_init(const Geometry& g, const QueueSlots& q, int* frozen, int* block_frozen, unsigned int* done, Launch& ln);
+int launch_queue_schedule(const Geometry& g, const QueueSlots& q, int admit, int* frozen, int* block_frozen, Launch& ln);
+int launch_queue_fill(const Geometry& g, const QueueSlots& q, const float* tokens, const float* pos, const float* state_in,
+                      const float* init_levels, float* state_out, float* slab, __nv_bfloat16* sb, __nv_bfloat16* sp,
+                      float* nsq, __nv_bfloat16* xb, Launch& ln);
 // s0 (nullable): where S_0 is when no step materialised it (the carried state, or init_levels broadcast if s0_bcast);
 // images with steps[b] == 0 are copied from there
-cudaError_t launch_settle_gather(const Geometry& g, int max_iters, const int32_t* steps, const float* slab, float* state_out,
-                                 const float* s0, int s0_bcast, cudaStream_t st, int* launches);
+int launch_settle_gather(const Geometry& g, int max_iters, const int32_t* steps, const float* slab, float* state_out,
+                         const float* s0, int s0_bcast, Launch& ln);
 // glom_b200_forward_steps (settle_kernels.cu): the flags of step t from the given step counts (clamped to [0, max_steps]),
 // one launch before every step; and, for return_all, the copy of slab steps[b] of each image into its slabs
 // steps[b]+1 .. max_steps (after the last step)
-cudaError_t launch_steps_schedule(const Geometry& g, int t, int max_steps, const int32_t* steps, int* frozen, int* block_frozen,
-                                  cudaStream_t st, int* launches);
-cudaError_t launch_steps_fill(const Geometry& g, int max_steps, const int32_t* steps, float* states, cudaStream_t st,
-                              int* launches);
+int launch_steps_schedule(const Geometry& g, int t, int max_steps, const int32_t* steps, int* frozen, int* block_frozen,
+                          Launch& ln);
+int launch_steps_fill(const Geometry& g, int max_steps, const int32_t* steps, float* states, Launch& ln);
 
 // fp32 consensus (attn_f32_kernel): a block of 16 queries keeps their rows (16 x dim) and logits (16 x n) as fp32 in
 // shared memory, within the 227 KB a block may opt in to: dim + n <= 3632
@@ -196,31 +222,28 @@ struct F32Buffers {
   float* h;  float* c;
   const float* w1;  const float* w2;  const float* b1;  const float* b2;
 };
-cudaError_t step_f32(const Geometry& g, const F32Buffers& b, cudaStream_t st, int* launches, Profiler* prof);
-cudaError_t launch_broadcast_init(const Geometry& g, const float* state_in, const float* init_levels, float* dst,
-                                  cudaStream_t st, int* launches, Profiler* prof);
+int step_f32(const Geometry& g, const F32Buffers& b, Launch& ln);
+int launch_broadcast_init(const Geometry& g, const float* state_in, const float* init_levels, float* dst, Launch& ln);
 
-cudaError_t launch_pack(int d, int L, int precision, const float* bu_w1, const float* bu_b1, const float* bu_w2,
-                        const float* bu_b2, const float* td_w1, const float* td_b1, const float* td_w2,
-                        const float* td_b2, void* packed, cudaStream_t st, int* launches);
+int launch_pack(int d, int L, int precision, const float* bu_w1, const float* bu_b1, const float* bu_w2, const float* bu_b2,
+                const float* td_w1, const float* td_b1, const float* td_w2, const float* td_b2, void* packed, Launch& ln);
 
-cudaError_t launch_tokenize(const float* img, const float* w, const float* bias, float* tokens, int B, int H, int W,
-                            int p, int d, cudaStream_t st, int* launches, Profiler* prof);
+int launch_tokenize(const float* img, const float* w, const float* bias, float* tokens, int B, int H, int W, int p, int d,
+                    Launch& ln);
 
 // island analytics on state slabs (islands.cu)
-cudaError_t launch_islands(const float* states, int slabs, int side_h, int side_w, int L, int d, float threshold,
-                           float* cos_right, float* cos_down, float* agreement, int* labels, int* num_islands,
-                           cudaStream_t st, int* launches);
+int launch_islands(const float* states, int slabs, int side_h, int side_w, int L, int d, float threshold, float* cos_right,
+                   float* cos_down, float* agreement, int* labels, int* num_islands, Launch& ln);
 
 cudaError_t launch_clock_probe(unsigned long long* out, unsigned long long spin_ns, cudaStream_t st);
 // (cycles, ns) sampled INSIDE the tensor-core kernels since the last reset, by ProfKind (tc_kernels.cu)
 cudaError_t tc_kernel_clocks(unsigned long long* out /* [PROF_KINDS][8] */, bool reset);
 
 // bf16 tokeniser: patchify + cast (CUDA cores), then the wgmma GEMM
-cudaError_t launch_patchify_bf16(const float* img, const float* w, __nv_bfloat16* patches, __nv_bfloat16* wtok, int B,
-                                 int H, int W, int p, int d, int kp, cudaStream_t st, int* launches);
+int launch_patchify_bf16(const float* img, const float* w, __nv_bfloat16* patches, __nv_bfloat16* wtok, int B, int H, int W,
+                         int p, int d, int kp, Launch& ln);
 int tokenize_tc(const __nv_bfloat16* patches, const __nv_bfloat16* wtok, const float* bias, float* tokens, int rows,
-                int d, int kp, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen);
+                int d, int kp, Launch& ln);
 
 // ---- backward (fp32, CUDA cores; bwd_kernels.cu) ---------------------------------------------------------
 struct BackwardArgs {
@@ -275,27 +298,25 @@ struct MlpBwdTc {
   // implicit gradients (BackwardArgs::relin / state_only): skip BW_PRE (pre / h already hold this state's), skip BW_DW
   int skip_pre, skip_dw;
 };
-int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches,
-                    char* err, size_t errlen);
+int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, Launch& ln);
 
-// (optional trailing arguments: a second product accumulated into the same output tile, see tc_bwd_kernels.cu)
+// One operand of the batched attention-backward GEMM: src is state-like (bf16 (B*n, L*d)) or attention-like (bf16
+// (Z, n, n)); mn: see BwdParams
+struct AttnBwdOperand { const void* src; int state, mn; };
+// (a2 / b2: a second product accumulated into the same output tile, see tc_bwd_kernels.cu; a2.src == NULL: none)
 // steps (nullable): the problems of images with steps[b] <= t are skipped and their output is left as it was
-int attn_bwd_gemm_tc(const Geometry& g, const void* a_src, int a_state, int a_mn, const void* b_src, int b_state, int b_mn,
-                     int N, int K, int out_kind, float* out, const int32_t* steps, int t, EncodeTiledFn enc, int num_sms,
-                     cudaStream_t st, int* launches,
-                     char* err, size_t errlen, const void* a2_src = nullptr, int a2_state = 0, int a2_mn = 0,
-                     const void* b2_src = nullptr, int b2_state = 0, int b2_mn = 0);
+int attn_bwd_gemm_tc(const Geometry& g, AttnBwdOperand a, AttnBwdOperand b, int N, int K, int out_kind, float* out,
+                     const int32_t* steps, int t, Launch& ln, AttnBwdOperand a2 = {}, AttnBwdOperand b2 = {});
 
 BackwardLayout backward_layout(const Geometry& g, int precision);
 // tokeniser backward (fp32, CUDA cores; bwd_kernels.cu): any of d_weight / d_bias / d_img may be NULL; all ACCUMULATED into
 size_t tokenize_backward_workspace_bytes(int B, int H, int W, int p, int need_dimg);
 // deterministic: d_bias by a fixed-order column sum instead of atomics (d_weight / d_img have no atomics)
-cudaError_t tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight, float* d_bias,
-                              float* d_img, int B, int H, int W, int p, int d, void* workspace, cudaStream_t st, int* launches,
-                              int deterministic = 0);
+int tokenize_backward(const float* img, const float* weight, const float* d_tokens, float* d_weight, float* d_bias,
+                      float* d_img, int B, int H, int W, int p, int d, void* workspace, Launch& ln, int deterministic = 0);
 // steps (nullable, device memory): per-image step counts; image b is the identity at every reverse step t >= steps[b]
 int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int iters, int grad_all, const int32_t* steps,
-                 void* workspace, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen);
+                 void* workspace, Launch& ln);
 
 // Implicit gradients through settle (glom_b200_backward_implicit, bf16 engine): the backward workspace, followed by
 struct ImplicitLayout {
@@ -320,8 +341,7 @@ ImplicitLayout implicit_layout(const Geometry& g);
 // (a.states = state, a.grad_out = grad_out; d_state0 / d_init NULL).  adjoint_steps (B) and adjoint_q (B, L, nullable)
 // receive K_b and the last pass's ratios
 int backward_implicit_run(const Geometry& g, const BackwardArgs& a, int adjoint_iters, float adjoint_tol,
-                          int32_t* adjoint_steps, float* adjoint_q, void* workspace, EncodeTiledFn enc, int num_sms,
-                          cudaStream_t st, int* launches, char* err, size_t errlen);
+                          int32_t* adjoint_steps, float* adjoint_q, void* workspace, Launch& ln);
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per device and per function: remember, per device, the
 // largest size already configured for one kernel (one instance of this per kernel template instantiation).

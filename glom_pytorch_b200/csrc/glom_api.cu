@@ -11,8 +11,9 @@
 namespace glom {
 
 static thread_local char g_err[512] = "";
-static thread_local int g_launches = 0;
 static thread_local Profiler g_prof;
+// the launch context of this thread's last launching entry point; glom_b200_last_launch_count reports its count
+static thread_local Launch g_launch{};
 
 static int fail(int code, const char* fmt, ...) {
   va_list ap;
@@ -21,6 +22,8 @@ static int fail(int code, const char* fmt, ...) {
   va_end(ap);
   return code;
 }
+
+static bool misaligned(const void* p, size_t a) { return reinterpret_cast<uintptr_t>(p) % a != 0; }
 
 PackedLayout packed_layout(int d, int L, int precision) {
   const size_t es = precision == GLOM_B200_BF16 ? 2 : 4;
@@ -164,6 +167,14 @@ static int device_info(DeviceInfo* out) {
   return 0;
 }
 
+// The launch context of an entry point whose arguments and device have been checked: the thread's count starts at 0 and
+// stands at what the call enqueued when it returns, failed or not.  sms: DeviceInfo::sms (0: the call plans no
+// tensor-core grid and queried no device)
+static Launch& begin_launch(int sms, void* stream) {
+  g_launch = Launch{g_encode, sms, static_cast<cudaStream_t>(stream), &g_prof, 0, ""};
+  return g_launch;
+}
+
 std::atomic<int> g_sm_count_target{0};
 
 }  // namespace glom
@@ -176,7 +187,7 @@ GLOM_B200_API int glom_b200_abi_version(void) { return GLOM_B200_ABI_VERSION; }
 
 GLOM_B200_API const char* glom_b200_last_error(void) { return g_err; }
 
-GLOM_B200_API int glom_b200_last_launch_count(void) { return g_launches; }
+GLOM_B200_API int glom_b200_last_launch_count(void) { return g_launch.launches; }
 
 GLOM_B200_API int glom_b200_set_sm_count_target(int sms) {
   if (sms < 0 || sms == 1)
@@ -199,11 +210,11 @@ GLOM_B200_API int glom_b200_pack_weights(const glom_b200_cfg* cfg, const glom_b2
     return fail(GLOM_B200_ERR_INVALID, "a weight pointer is NULL");
   const PackedLayout pl = packed_layout(cfg->dim, cfg->levels, cfg->precision);
   if (!packed || packed_bytes < pl.total) return fail(GLOM_B200_ERR_WORKSPACE, "packed buffer: need %zu bytes, got %zu", pl.total, packed_bytes);
-  if (reinterpret_cast<uintptr_t>(packed) % 1024) return fail(GLOM_B200_ERR_INVALID, "packed buffer must be 1024-byte aligned");
-  g_launches = 0;
-  cudaError_t e = launch_pack(cfg->dim, cfg->levels, cfg->precision, w->bu_w1, w->bu_b1, w->bu_w2, w->bu_b2, w->td_w1,
-                              w->td_b1, w->td_w2, w->td_b2, packed, static_cast<cudaStream_t>(stream), &g_launches);
-  if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "pack_weights launch: %s", cudaGetErrorString(e));
+  if (misaligned(packed, 1024)) return fail(GLOM_B200_ERR_INVALID, "packed buffer must be 1024-byte aligned");
+  Launch& ln = begin_launch(0, stream);
+  if (int r = launch_pack(cfg->dim, cfg->levels, cfg->precision, w->bu_w1, w->bu_b1, w->bu_w2, w->bu_b2, w->td_w1, w->td_b1,
+                          w->td_w2, w->td_b2, packed, ln))
+    return fail(r, "pack_weights launch: %s", ln.err);
   return 0;
 }
 
@@ -227,14 +238,193 @@ GLOM_B200_API int glom_b200_workspace_offset(const glom_b200_cfg* cfg, int batch
   }
 }
 
+// ---- what the forward, settle and queue calls share ------------------------------------------------------------------
+
+// The tensor arguments of a forward or queue call, checked in this order.  `pre`: "" or "<entry point>: ".  A forward
+// passes its packed weights (they are required, and aligned like the workspace); the queue calls check theirs themselves
+// (queue_run) or take none (queue_begin): has_packed = false.
+static int check_tensors(const char* pre, bool has_packed, const void* packed_weights, const float* tokens, const float* pos,
+                         const float* state_in, const float* init_levels, const float* state_out, const void* workspace) {
+  if ((has_packed && !packed_weights) || !tokens || !pos || !state_out)
+    return fail(GLOM_B200_ERR_INVALID, "%sa required pointer is NULL", pre);
+  if (!state_in && !init_levels) return fail(GLOM_B200_ERR_INVALID, "%sneed state_in or init_levels", pre);
+  if (state_in == state_out) return fail(GLOM_B200_ERR_INVALID, "%sstate_out must not alias state_in", pre);
+  if (has_packed && (misaligned(packed_weights, 1024) || misaligned(workspace, 1024)))
+    return fail(GLOM_B200_ERR_INVALID, "%spacked weights and workspace must be 1024-byte aligned", pre);
+  if (!has_packed && misaligned(workspace, 1024)) return fail(GLOM_B200_ERR_INVALID, "%sworkspace must be 1024-byte aligned", pre);
+  if (misaligned(tokens, 16) || misaligned(pos, 16) || misaligned(state_out, 16) || misaligned(state_in, 16) ||
+      misaligned(init_levels, 16))
+    return fail(GLOM_B200_ERR_INVALID, "%stensor pointers must be 16-byte aligned", pre);
+  return 0;
+}
+
+// The bf16 engine's buffers inside a forward workspace and a packed-weight buffer: `step` with every field set that does
+// not change from step to step, and the ping-pong halves that set_parity() points its in / out fields at.
+struct StepBuffers {
+  Bf16Buffers step;
+  __nv_bfloat16 *sb[2], *sp[2], *xb;
+  float* nsq[2];
+};
+static StepBuffers bind_step_buffers(const WorkspaceLayout& wl, const PackedLayout& pl, void* workspace,
+                                     const void* packed_weights, const float* pos) {
+  char* ws = static_cast<char*>(workspace);
+  const char* pw = static_cast<const char*>(packed_weights);
+  StepBuffers s{};
+  for (int i = 0; i < 2; ++i) {
+    s.sb[i] = reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off[i]);
+    s.sp[i] = reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off[i]);
+    s.nsq[i] = reinterpret_cast<float*>(ws + wl.nsq_off[i]);
+  }
+  s.xb = reinterpret_cast<__nv_bfloat16*>(ws + wl.xb_off);
+  s.step.xb = s.xb;
+  s.step.h = reinterpret_cast<__nv_bfloat16*>(ws + wl.h_off);
+  s.step.c = reinterpret_cast<__nv_bfloat16*>(ws + wl.c_off);
+  s.step.attn_acc = wl.attn_acc_bytes ? reinterpret_cast<float*>(ws + wl.attn_acc_off) : nullptr;
+  s.step.pos = pos;
+  s.step.w1 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w1_off);
+  s.step.w2 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w2_off);
+  s.step.b1 = reinterpret_cast<const float*>(pw + pl.b1_off);
+  s.step.b2 = reinterpret_cast<const float*>(pw + pl.b2_off);
+  return s;
+}
+// the step reads the shadows / norm partials of buffer p and writes those of the other one
+static void set_parity(StepBuffers& s, int p) {
+  s.step.sb_in = s.sb[p]; s.step.sb_out = s.sb[p ^ 1];
+  s.step.sp_in = s.sp[p]; s.step.sp_out = s.sp[p ^ 1];
+  s.step.nsq_in = s.nsq[p]; s.step.nsq_out = s.nsq[p ^ 1];
+}
+
+// the freeze flags and settle's change partials inside a settle workspace
+struct SettleFlags { int *frozen, *block_frozen; float* dsq; unsigned int* done; float* level_q; };
+static SettleFlags bind_settle_flags(const SettleLayout& sl, void* workspace) {
+  char* ws = static_cast<char*>(workspace);
+  return {reinterpret_cast<int*>(ws + sl.frozen_off), reinterpret_cast<int*>(ws + sl.block_frozen_off),
+          reinterpret_cast<float*>(ws + sl.dsq_off), reinterpret_cast<unsigned int*>(ws + sl.done_off),
+          reinterpret_cast<float*>(ws + sl.level_q_off)};
+}
+
 // glom_b200_settle / glom_b200_settle_all: a forward of max_iters steps (return_all = 0 / 1) that stops each image at the
 // first step whose change criterion is <= tol
 struct SettleRun { float tol; int32_t* steps; };
 
-static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
-                        const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
-                        int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity,
-                        const SettleRun* settle = nullptr, const int32_t* steps = nullptr);
+// One forward call: the operands of glom_b200_forward, and what selects the other forms
+struct ForwardArgs {
+  const glom_b200_cfg* cfg; const void* packed_weights; const float *tokens, *pos, *state_in, *init_levels; float* state_out;
+  int batch, iters, return_all; void* workspace; size_t workspace_bytes; void* stream;
+  int resume_parity = -1;              // glom_b200_forward_resume: the shadow buffer that holds state_in's shadows
+  const SettleRun* settle = nullptr;   // glom_b200_settle / _settle_all
+  const int32_t* steps = nullptr;      // glom_b200_forward_steps: per-image step counts (device memory)
+};
+
+static int forward_impl(const ForwardArgs& a) {
+  const glom_b200_cfg* cfg = a.cfg;
+  const float *state_in = a.state_in, *init_levels = a.init_levels;
+  float* state_out = a.state_out;
+  const int iters = a.iters, return_all = a.return_all;
+  const SettleRun* settle = a.settle;
+  const int32_t* steps = a.steps;
+  if (int r = check_cfg(cfg)) return r;
+  if (a.batch < 1 || iters < 0) return fail(GLOM_B200_ERR_INVALID, "batch must be >= 1 and iters >= 0");
+  if (cfg->precision == GLOM_B200_FP32 && cfg->dim + cfg->n > kAttnF32MaxDimPlusN)
+    return fail(GLOM_B200_ERR_INVALID,
+                "fp32 consensus keeps %d (dim + n) floats per block in shared memory: dim + n must be <= %d (got %d)",
+                kAttnF32Queries, kAttnF32MaxDimPlusN, cfg->dim + cfg->n);
+  if (int r = check_tensors("", true, a.packed_weights, a.tokens, a.pos, state_in, init_levels, state_out, a.workspace)) return r;
+  DeviceInfo di{};
+  if (int r = device_info(&di)) return r;
+  const Geometry g = make_geometry(cfg, a.batch);
+  // settle and forward_steps freeze images: the SETTLE instantiations of the step kernels, driven by per-image flags
+  const bool freeze = settle || steps;
+  const SettleLayout sl = freeze ? settle_layout(g, iters, return_all) : SettleLayout{};
+  const WorkspaceLayout wl = freeze ? sl.fwd : workspace_layout(g, cfg->precision, iters, return_all);
+  const size_t ws_need = freeze ? sl.total : wl.total;
+  if (!a.workspace || a.workspace_bytes < ws_need)
+    return fail(GLOM_B200_ERR_WORKSPACE, "workspace: need %zu bytes, got %zu", ws_need, a.workspace_bytes);
+  const PackedLayout pl = packed_layout(g.d, g.L, cfg->precision);
+  char* ws = static_cast<char*>(a.workspace);
+  Launch& ln = begin_launch(di.sms, a.stream);
+  const size_t slab = (size_t)g.rows * g.L * g.d;
+
+  // where the fp32 master of step t lives
+  float* wslab = reinterpret_cast<float*>(ws + wl.s32_off);
+  auto loc = [&](int t) -> float* {
+    if (return_all) return state_out + (size_t)t * slab;
+    return ((iters - t) % 2 == 0) ? state_out : wslab;
+  };
+
+  if (cfg->precision == GLOM_B200_BF16) {
+    StepBuffers sbuf = bind_step_buffers(wl, pl, a.workspace, a.packed_weights, a.pos);
+    Bf16Buffers& b = sbuf.step;
+    // resumed call (glom_b200_forward_resume): the shadows / norm partials of state_in are the ones the previous call left
+    // in buffer `p0`; the state prologue is skipped and step 0 reads the fp32 master straight from state_in
+    const bool resume = a.resume_parity >= 0;
+    const int p0 = resume ? a.resume_parity : 0;
+    const bool s0_direct = resume || (!return_all && iters >= 1);
+    int prep;
+    if (resume) {
+      prep = launch_prep(g, nullptr, nullptr, a.pos, a.tokens, nullptr, nullptr, nullptr, sbuf.xb, nullptr, ln);
+      if (prep == 0 && return_all)         // slab 0 of the return_all form is S_0 (:126)
+        prep = ln.launched(cudaMemcpyAsync(state_out, state_in, slab * sizeof(float), cudaMemcpyDeviceToDevice, ln.st));
+    } else {
+      // S_0 as an fp32 slab is only materialised when it is part of the result (return_all slab 0, iters == 0): otherwise
+      // step 0 reads the carried state from the caller's tensor, or init_levels broadcast over the rows
+      prep = launch_prep(g, state_in, init_levels, a.pos, a.tokens, s0_direct ? nullptr : loc(0), sbuf.sb[0], sbuf.sp[0], sbuf.xb,
+                         sbuf.nsq[0], ln);
+    }
+    if (prep) return fail(prep, "prep launch: %s", ln.err);
+    // settle: no image has stopped yet.  forward_steps: the schedule kernel writes every flag before each step
+    const SettleFlags fl = freeze ? bind_settle_flags(sl, a.workspace) : SettleFlags{};
+    b.frozen = fl.frozen; b.block_frozen = fl.block_frozen;
+    b.dsq_out = settle ? fl.dsq : nullptr;     // NULL: K2 sums no squared change
+    if (settle) {
+      if (int r = ln.check(cudaMemsetAsync(ws + sl.flags_off, 0, sl.flags_bytes, ln.st)))
+        return fail(r, "settle flags memset: %s", ln.err);
+    }
+    for (int t = 0; t < iters; ++t) {
+      if (steps) {         // images with steps[b] <= t are frozen from step t on (from the start when steps[b] == 0)
+        if (int r = launch_steps_schedule(g, t, iters, steps, fl.frozen, fl.block_frozen, ln))
+          return fail(r, "step schedule launch before step %d: %s", t, ln.err);
+      }
+      b.s32_in = (s0_direct && t == 0) ? (state_in ? state_in : init_levels) : loc(t); b.s32_out = loc(t + 1);
+      b.s32_in_bcast = (s0_direct && t == 0 && !state_in) ? 1 : 0;
+      set_parity(sbuf, (t + p0) & 1);
+      if (int r = step_bf16(g, b, t, ln)) return fail(r, "step %d: %s", t, ln.err);
+      if (settle) {
+        if (int r = launch_settle_converge(g, t + 1, settle->tol, fl.dsq, b.nsq_out, fl.frozen, fl.block_frozen, fl.done,
+                                           fl.level_q, settle->steps, ln))
+          return fail(r, "settle convergence launch after step %d: %s", t, ln.err);
+      }
+    }
+    // settle and forward_steps: return_all slab t of image b must be S_min(t, steps[b]).  Otherwise S_steps[b] is in
+    // loc(steps[b]) and the ones in the workspace slab move to state_out; steps[b] == 0 (forward_steps only) takes S_0,
+    // which step 0 read straight from state_in / init_levels
+    const int32_t* image_steps = settle ? settle->steps : steps;
+    if (image_steps && return_all) {
+      if (int r = launch_steps_fill(g, iters, image_steps, state_out, ln)) return fail(r, "return_all fill launch: %s", ln.err);
+    } else if (image_steps && iters > 0) {
+      if (int r = launch_settle_gather(g, iters, image_steps, wslab, state_out, state_in ? state_in : init_levels,
+                                       state_in ? 0 : 1, ln))
+        return fail(r, "%s gather launch: %s", settle ? "settle" : "step", ln.err);
+    }
+  } else {
+    const char* pw = static_cast<const char*>(a.packed_weights);
+    if (int r = launch_broadcast_init(g, state_in, init_levels, loc(0), ln)) return fail(r, "init launch: %s", ln.err);
+    for (int t = 0; t < iters; ++t) {
+      F32Buffers b{};
+      b.s_in = loc(t); b.s_out = loc(t + 1);
+      b.x = a.tokens; b.pos = a.pos;
+      b.h = reinterpret_cast<float*>(ws + wl.h_off);
+      b.c = reinterpret_cast<float*>(ws + wl.c_off);
+      b.w1 = reinterpret_cast<const float*>(pw + pl.w1_off);
+      b.w2 = reinterpret_cast<const float*>(pw + pl.w2_off);
+      b.b1 = reinterpret_cast<const float*>(pw + pl.b1_off);
+      b.b2 = reinterpret_cast<const float*>(pw + pl.b2_off);
+      if (int r = step_f32(g, b, ln)) return fail(r, "fp32 step %d launch: %s", t, ln.err);
+    }
+  }
+  g_err[0] = 0;
+  return 0;
+}
 
 // The freeze modes: settle / settle_all (bound max_iters >= 1) and forward_steps (bound max_steps >= 0) run the bf16
 // engine's SETTLE step kernels.  Their workspace is the forward's plus the freeze flags (settle_layout).
@@ -259,19 +449,17 @@ static int freeze_workspace_bytes(const FreezeMode& m, const glom_b200_cfg* cfg,
 
 static int check_steps_ptr(const char* fn, const char* arg, const int32_t* steps) {
   if (!steps) return fail(GLOM_B200_ERR_INVALID, "%s: %s is NULL", fn, arg);
-  if (reinterpret_cast<uintptr_t>(steps) % 4) return fail(GLOM_B200_ERR_INVALID, "%s: %s must be 4-byte aligned", fn, arg);
+  if (misaligned(steps, 4)) return fail(GLOM_B200_ERR_INVALID, "%s: %s must be 4-byte aligned", fn, arg);
   return 0;
 }
 
-static int settle_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
-                       const float* state_in, const float* init_levels, float* state_out, int batch, int max_iters,
-                       int return_all, float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes, void* stream) {
-  if (int r = check_freeze(kSettle, cfg, batch, max_iters)) return r;
+static int settle_impl(ForwardArgs a, float tol, int32_t* steps_out) {
+  if (int r = check_freeze(kSettle, a.cfg, a.batch, a.iters)) return r;
   if (tol != tol) return fail(GLOM_B200_ERR_INVALID, "settle: tol is NaN");
   if (int r = check_steps_ptr("settle", "steps_out", steps_out)) return r;
   const SettleRun run{tol, steps_out};
-  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_iters, return_all,
-                      workspace, workspace_bytes, stream, -1, &run);
+  a.settle = &run;
+  return forward_impl(a);
 }
 
 GLOM_B200_API int glom_b200_settle_workspace_bytes(const glom_b200_cfg* cfg, int batch, int max_iters, size_t* out_bytes) {
@@ -296,8 +484,8 @@ GLOM_B200_API int glom_b200_settle_workspace_offset(const glom_b200_cfg* cfg, in
 GLOM_B200_API int glom_b200_settle(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                                    const float* state_in, const float* init_levels, float* state_out, int batch, int max_iters,
                                    float tol, int32_t* steps_out, void* workspace, size_t workspace_bytes, void* stream) {
-  return settle_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_iters, 0, tol, steps_out,
-                     workspace, workspace_bytes, stream);
+  return settle_impl({cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_iters, 0, workspace,
+                      workspace_bytes, stream}, tol, steps_out);
 }
 
 // glom_b200_settle_all: glom_b200_settle with every state kept (the return_all form of forward_steps)
@@ -309,8 +497,8 @@ GLOM_B200_API int glom_b200_settle_all(const glom_b200_cfg* cfg, const void* pac
                                        const float* pos, const float* state_in, const float* init_levels, float* states_out,
                                        int batch, int max_iters, float tol, int32_t* steps_out, void* workspace,
                                        size_t workspace_bytes, void* stream) {
-  return settle_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, states_out, batch, max_iters, 1, tol, steps_out,
-                     workspace, workspace_bytes, stream);
+  return settle_impl({cfg, packed_weights, tokens, pos, state_in, init_levels, states_out, batch, max_iters, 1, workspace,
+                      workspace_bytes, stream}, tol, steps_out);
 }
 
 // glom_b200_forward_steps: a forward of max_steps steps in which image b stops after steps[b] (read on the device only)
@@ -325,15 +513,17 @@ GLOM_B200_API int glom_b200_forward_steps(const glom_b200_cfg* cfg, const void* 
                                           size_t workspace_bytes, void* stream) {
   if (int r = check_freeze(kForwardSteps, cfg, batch, max_steps)) return r;
   if (int r = check_steps_ptr("forward_steps", "steps", steps)) return r;
-  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_steps, return_all ? 1 : 0,
-                      workspace, workspace_bytes, stream, -1, nullptr, steps);
+  ForwardArgs a{cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, max_steps, return_all ? 1 : 0,
+                workspace, workspace_bytes, stream};
+  a.steps = steps;
+  return forward_impl(a);
 }
 
 GLOM_B200_API int glom_b200_forward(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
                       const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
                       int return_all, void* workspace, size_t workspace_bytes, void* stream) {
-  return forward_impl(cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, iters, return_all, workspace,
-                      workspace_bytes, stream, -1);
+  return forward_impl({cfg, packed_weights, tokens, pos, state_in, init_levels, state_out, batch, iters, return_all, workspace,
+                       workspace_bytes, stream});
 }
 
 GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens,
@@ -343,8 +533,10 @@ GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void*
   if (!cfg || cfg->precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "forward_resume: bf16 engine only");
   if (!state_in || (shadow_parity != 0 && shadow_parity != 1) || iters < 1)
     return fail(GLOM_B200_ERR_INVALID, "forward_resume: need state_in, shadow_parity in {0, 1} and iters >= 1");
-  const int r = forward_impl(cfg, packed_weights, tokens, pos, state_in, nullptr, state_out, batch, iters, return_all, workspace,
-                             workspace_bytes, stream, shadow_parity);
+  ForwardArgs a{cfg, packed_weights, tokens, pos, state_in, nullptr, state_out, batch, iters, return_all, workspace,
+                workspace_bytes, stream};
+  a.resume_parity = shadow_parity;
+  const int r = forward_impl(a);
   if (r == 0 && out_shadow_parity) *out_shadow_parity = (shadow_parity + iters) & 1;
   return r;
 }
@@ -352,8 +544,8 @@ GLOM_B200_API int glom_b200_forward_resume(const glom_b200_cfg* cfg, const void*
 // glom_b200_settle_queue_* and glom_b200_settle_video_*: the arguments shared by _begin and _run, checked in the same
 // order as settle's.  settle_queue queues `items` = N images (frames = 1); settle_video queues `items` = S streams of
 // `frames` frames each, and its images are the S * frames frames.
-struct QueueMode { const char* name; const char* items; };
-static const QueueMode kQueue{"settle_queue", "images"}, kVideo{"settle_video", "streams"};
+struct QueueMode { const char* name; const char* pre; const char* items; };
+static const QueueMode kQueue{"settle_queue", "settle_queue: ", "images"}, kVideo{"settle_video", "settle_video: ", "streams"};
 
 struct QueueArgs {
   const QueueMode& mode;
@@ -379,14 +571,8 @@ static int check_queue(const QueueArgs& a, Geometry* g, QueueLayout* ql, DeviceI
   if (int r = check_queue_sizes(a.mode, a.cfg, a.items, a.frames, a.slots, a.max_iters)) return r;
   if (a.tol != a.tol) return fail(GLOM_B200_ERR_INVALID, "%s: tol is NaN", fn);
   if (int r = check_steps_ptr(fn, "steps_out", a.steps_out)) return r;
-  if (!a.tokens || !a.pos || !a.state_out) return fail(GLOM_B200_ERR_INVALID, "%s: a required pointer is NULL", fn);
-  if (!a.state_in && !a.init_levels) return fail(GLOM_B200_ERR_INVALID, "%s: need state_in or init_levels", fn);
-  if (a.state_in == a.state_out) return fail(GLOM_B200_ERR_INVALID, "%s: state_out must not alias state_in", fn);
-  if (reinterpret_cast<uintptr_t>(a.workspace) % 1024) return fail(GLOM_B200_ERR_INVALID, "%s: workspace must be 1024-byte aligned", fn);
-  if (reinterpret_cast<uintptr_t>(a.tokens) % 16 || reinterpret_cast<uintptr_t>(a.pos) % 16 ||
-      reinterpret_cast<uintptr_t>(a.state_out) % 16 || reinterpret_cast<uintptr_t>(a.state_in) % 16 ||
-      reinterpret_cast<uintptr_t>(a.init_levels) % 16)
-    return fail(GLOM_B200_ERR_INVALID, "%s: tensor pointers must be 16-byte aligned", fn);
+  if (int r = check_tensors(a.mode.pre, false, nullptr, a.tokens, a.pos, a.state_in, a.init_levels, a.state_out, a.workspace))
+    return r;
   *g = make_geometry(a.cfg, a.slots);
   *ql = queue_layout(*g, a.max_iters);
   if (!a.workspace || a.workspace_bytes < ql->total)
@@ -414,13 +600,10 @@ static QueueSlots queue_slots(const QueueArgs& a, const QueueLayout& ql) {
 static int queue_begin(const QueueArgs& a) {
   Geometry g{}; QueueLayout ql{}; DeviceInfo di{};
   if (int r = check_queue(a, &g, &ql, &di)) return r;
-  char* ws = static_cast<char*>(a.workspace);
-  g_launches = 0;
-  const cudaError_t e = launch_queue_init(g, queue_slots(a, ql), reinterpret_cast<int*>(ws + ql.settle.frozen_off),
-                                          reinterpret_cast<int*>(ws + ql.settle.block_frozen_off),
-                                          reinterpret_cast<unsigned int*>(ws + ql.settle.done_off),
-                                          static_cast<cudaStream_t>(a.stream), &g_launches, &g_prof);
-  if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "%s init launch: %s", a.mode.name, cudaGetErrorString(e));
+  const SettleFlags fl = bind_settle_flags(ql.settle, a.workspace);
+  Launch& ln = begin_launch(di.sms, a.stream);
+  if (int r = launch_queue_init(g, queue_slots(a, ql), fl.frozen, fl.block_frozen, fl.done, ln))
+    return fail(r, "%s init launch: %s", a.mode.name, ln.err);
   g_err[0] = 0;
   return 0;
 }
@@ -431,204 +614,39 @@ static int queue_run(const QueueArgs& a, const void* packed_weights, int first_s
   Geometry g{}; QueueLayout ql{}; DeviceInfo di{};
   const char* fn = a.mode.name;
   if (int r = check_queue_sizes(a.mode, a.cfg, a.items, a.frames, a.slots, a.max_iters)) return r;
-  if (!packed_weights || reinterpret_cast<uintptr_t>(packed_weights) % 1024)
+  if (!packed_weights || misaligned(packed_weights, 1024))
     return fail(GLOM_B200_ERR_INVALID, "%s: packed weights NULL or not 1024-byte aligned", fn);
   if (first_step < 0 || num_steps < 0)
     return fail(GLOM_B200_ERR_INVALID, "%s: first_step and num_steps must be >= 0 (got %d, %d)", fn, first_step, num_steps);
-  if (reinterpret_cast<uintptr_t>(remaining_out) % 4)
-    return fail(GLOM_B200_ERR_INVALID, "%s: remaining_out must be 4-byte aligned", fn);
+  if (misaligned(remaining_out, 4)) return fail(GLOM_B200_ERR_INVALID, "%s: remaining_out must be 4-byte aligned", fn);
   if (int r = check_queue(a, &g, &ql, &di)) return r;
-  const WorkspaceLayout& wl = ql.settle.fwd;
-  const PackedLayout pl = packed_layout(g.d, g.L, GLOM_B200_BF16);
-  const char* pw = static_cast<const char*>(packed_weights);
   char* ws = static_cast<char*>(a.workspace);
-  cudaStream_t st = static_cast<cudaStream_t>(a.stream);
   const QueueSlots q = queue_slots(a, ql);
   float* slab[2] = {reinterpret_cast<float*>(ws + ql.slab_off[0]), reinterpret_cast<float*>(ws + ql.slab_off[1])};
-  __nv_bfloat16* sb[2] = {reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off[0]), reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off[1])};
-  __nv_bfloat16* sp[2] = {reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off[0]), reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off[1])};
-  float* nsq[2] = {reinterpret_cast<float*>(ws + wl.nsq_off[0]), reinterpret_cast<float*>(ws + wl.nsq_off[1])};
-  __nv_bfloat16* xb = reinterpret_cast<__nv_bfloat16*>(ws + wl.xb_off);
-  int* frozen = reinterpret_cast<int*>(ws + ql.settle.frozen_off);
-  int* block_frozen = reinterpret_cast<int*>(ws + ql.settle.block_frozen_off);
-  float* dsq = reinterpret_cast<float*>(ws + ql.settle.dsq_off);
-  g_launches = 0;
+  StepBuffers sbuf = bind_step_buffers(ql.settle.fwd, packed_layout(g.d, g.L, GLOM_B200_BF16), a.workspace, packed_weights, a.pos);
+  const SettleFlags fl = bind_settle_flags(ql.settle, a.workspace);
+  Bf16Buffers& b = sbuf.step;
+  b.frozen = fl.frozen; b.block_frozen = fl.block_frozen; b.dsq_out = fl.dsq; b.block_fresh = q.block_fresh;
+  Launch& ln = begin_launch(di.sms, a.stream);
   const int last = first_step + (num_steps > 0 ? num_steps : 1);
   for (int t = first_step; t < last; ++t) {
     const int p = t & 1;
-    cudaError_t e = launch_queue_schedule(g, q, num_steps > 0, frozen, block_frozen, st, &g_launches, &g_prof);
-    if (e == cudaSuccess)
-      e = launch_queue_fill(g, q, a.tokens, a.pos, a.state_in, a.init_levels, a.state_out, slab[p], sb[p], sp[p], nsq[p], xb, st,
-                            &g_launches, &g_prof);
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "%s slot launch before step %d: %s", fn, t, cudaGetErrorString(e));
+    int r = launch_queue_schedule(g, q, num_steps > 0, fl.frozen, fl.block_frozen, ln);
+    if (r == 0)
+      r = launch_queue_fill(g, q, a.tokens, a.pos, a.state_in, a.init_levels, a.state_out, slab[p], sbuf.sb[p], sbuf.sp[p],
+                            sbuf.nsq[p], sbuf.xb, ln);
+    if (r) return fail(r, "%s slot launch before step %d: %s", fn, t, ln.err);
     if (num_steps == 0) break;
-    Bf16Buffers b{};
     b.s32_in = slab[p]; b.s32_out = slab[p ^ 1]; b.s32_in_bcast = 0;
-    b.sb_in = sb[p]; b.sb_out = sb[p ^ 1];
-    b.sp_in = sp[p]; b.sp_out = sp[p ^ 1];
-    b.xb = xb;
-    b.h = reinterpret_cast<__nv_bfloat16*>(ws + wl.h_off);
-    b.attn_acc = wl.attn_acc_bytes ? reinterpret_cast<float*>(ws + wl.attn_acc_off) : nullptr;
-    b.c = reinterpret_cast<__nv_bfloat16*>(ws + wl.c_off);
-    b.nsq_in = nsq[p]; b.nsq_out = nsq[p ^ 1];
-    b.pos = a.pos;
-    b.w1 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w1_off);
-    b.w2 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w2_off);
-    b.b1 = reinterpret_cast<const float*>(pw + pl.b1_off);
-    b.b2 = reinterpret_cast<const float*>(pw + pl.b2_off);
-    b.frozen = frozen; b.block_frozen = block_frozen; b.dsq_out = dsq; b.block_fresh = q.block_fresh;
-    char msg[400] = "";
-    const int r = step_bf16(g, b, t, g_encode, di.sms, st, &g_launches, msg, sizeof(msg), &g_prof);
-    if (r) return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "%s step %d: %s", fn, t, msg);
-    e = launch_settle_converge(g, t + 1, a.tol, dsq, b.nsq_out, frozen, block_frozen,
-                               reinterpret_cast<unsigned int*>(ws + ql.settle.done_off),
-                               reinterpret_cast<float*>(ws + ql.settle.level_q_off), a.steps_out, st, &g_launches, &q);
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "%s convergence launch after step %d: %s", fn, t, cudaGetErrorString(e));
+    set_parity(sbuf, p);
+    if (int r = step_bf16(g, b, t, ln)) return fail(r, "%s step %d: %s", fn, t, ln.err);
+    if (int r = launch_settle_converge(g, t + 1, a.tol, fl.dsq, b.nsq_out, fl.frozen, fl.block_frozen, fl.done, fl.level_q,
+                                       a.steps_out, ln, &q))
+      return fail(r, "%s convergence launch after step %d: %s", fn, t, ln.err);
   }
   if (remaining_out) {
-    const cudaError_t e = cudaMemcpyAsync(remaining_out, q.unfinished, sizeof(int32_t), cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "%s count copy: %s", fn, cudaGetErrorString(e));
-    ++g_launches;
-  }
-  g_err[0] = 0;
-  return 0;
-}
-
-static int forward_impl(const glom_b200_cfg* cfg, const void* packed_weights, const float* tokens, const float* pos,
-                        const float* state_in, const float* init_levels, float* state_out, int batch, int iters,
-                        int return_all, void* workspace, size_t workspace_bytes, void* stream, int resume_parity,
-                        const SettleRun* settle, const int32_t* steps) {
-  if (int r = check_cfg(cfg)) return r;
-  if (batch < 1 || iters < 0) return fail(GLOM_B200_ERR_INVALID, "batch must be >= 1 and iters >= 0");
-  if (cfg->precision == GLOM_B200_FP32 && cfg->dim + cfg->n > kAttnF32MaxDimPlusN)
-    return fail(GLOM_B200_ERR_INVALID,
-                "fp32 consensus keeps %d (dim + n) floats per block in shared memory: dim + n must be <= %d (got %d)",
-                kAttnF32Queries, kAttnF32MaxDimPlusN, cfg->dim + cfg->n);
-  if (!packed_weights || !tokens || !pos || !state_out) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
-  if (!state_in && !init_levels) return fail(GLOM_B200_ERR_INVALID, "need state_in or init_levels");
-  if (state_in == state_out) return fail(GLOM_B200_ERR_INVALID, "state_out must not alias state_in");
-  if (reinterpret_cast<uintptr_t>(packed_weights) % 1024 || reinterpret_cast<uintptr_t>(workspace) % 1024)
-    return fail(GLOM_B200_ERR_INVALID, "packed weights and workspace must be 1024-byte aligned");
-  if (reinterpret_cast<uintptr_t>(tokens) % 16 || reinterpret_cast<uintptr_t>(pos) % 16 ||
-      reinterpret_cast<uintptr_t>(state_out) % 16 || reinterpret_cast<uintptr_t>(state_in) % 16 ||
-      reinterpret_cast<uintptr_t>(init_levels) % 16)
-    return fail(GLOM_B200_ERR_INVALID, "tensor pointers must be 16-byte aligned");
-  DeviceInfo di{};
-  if (int r = device_info(&di)) return r;
-  const Geometry g = make_geometry(cfg, batch);
-  // settle and forward_steps freeze images: the SETTLE instantiations of the step kernels, driven by per-image flags
-  const bool freeze = settle || steps;
-  const SettleLayout sl = freeze ? settle_layout(g, iters, return_all) : SettleLayout{};
-  const WorkspaceLayout wl = freeze ? sl.fwd : workspace_layout(g, cfg->precision, iters, return_all);
-  const size_t ws_need = freeze ? sl.total : wl.total;
-  if (!workspace || workspace_bytes < ws_need)
-    return fail(GLOM_B200_ERR_WORKSPACE, "workspace: need %zu bytes, got %zu", ws_need, workspace_bytes);
-  const PackedLayout pl = packed_layout(g.d, g.L, cfg->precision);
-  const char* pw = static_cast<const char*>(packed_weights);
-  char* ws = static_cast<char*>(workspace);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t slab = (size_t)g.rows * g.L * g.d;
-  g_launches = 0;
-
-  // where the fp32 master of step t lives
-  float* wslab = reinterpret_cast<float*>(ws + wl.s32_off);
-  auto loc = [&](int t) -> float* {
-    if (return_all) return state_out + (size_t)t * slab;
-    return ((iters - t) % 2 == 0) ? state_out : wslab;
-  };
-
-  if (cfg->precision == GLOM_B200_BF16) {
-    __nv_bfloat16* sb[2] = {reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off[0]), reinterpret_cast<__nv_bfloat16*>(ws + wl.sb_off[1])};
-    __nv_bfloat16* sp[2] = {reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off[0]), reinterpret_cast<__nv_bfloat16*>(ws + wl.sp_off[1])};
-    float* nsq[2] = {reinterpret_cast<float*>(ws + wl.nsq_off[0]), reinterpret_cast<float*>(ws + wl.nsq_off[1])};
-    __nv_bfloat16* xb = reinterpret_cast<__nv_bfloat16*>(ws + wl.xb_off);
-    // resumed call (glom_b200_forward_resume): the shadows / norm partials of state_in are the ones the previous call left
-    // in buffer `p0`; the state prologue is skipped and step 0 reads the fp32 master straight from state_in
-    const bool resume = resume_parity >= 0;
-    const int p0 = resume ? resume_parity : 0;
-    const bool s0_direct = resume || (!return_all && iters >= 1);
-    cudaError_t e;
-    if (resume) {
-      e = launch_prep(g, nullptr, nullptr, pos, tokens, nullptr, nullptr, nullptr, xb, nullptr, st, &g_launches, &g_prof);
-      if (e == cudaSuccess && return_all) {       // slab 0 of the return_all form is S_0 (:126)
-        e = cudaMemcpyAsync(state_out, state_in, slab * sizeof(float), cudaMemcpyDeviceToDevice, st);
-        ++g_launches;
-      }
-    } else {
-      // S_0 as an fp32 slab is only materialised when it is part of the result (return_all slab 0, iters == 0): otherwise
-      // step 0 reads the carried state from the caller's tensor, or init_levels broadcast over the rows
-      e = launch_prep(g, state_in, init_levels, pos, tokens, s0_direct ? nullptr : loc(0), sb[0], sp[0], xb, nsq[0], st,
-                      &g_launches, &g_prof);
-    }
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "prep launch: %s", cudaGetErrorString(e));
-    // settle: no image has stopped yet.  forward_steps: the schedule kernel writes every flag before each step
-    int* frozen = freeze ? reinterpret_cast<int*>(ws + sl.frozen_off) : nullptr;
-    int* block_frozen = freeze ? reinterpret_cast<int*>(ws + sl.block_frozen_off) : nullptr;
-    float* dsq = settle ? reinterpret_cast<float*>(ws + sl.dsq_off) : nullptr;     // NULL: K2 sums no squared change
-    if (settle) {
-      e = cudaMemsetAsync(ws + sl.flags_off, 0, sl.flags_bytes, st);
-      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle flags memset: %s", cudaGetErrorString(e));
-    }
-    for (int t = 0; t < iters; ++t) {
-      if (steps) {         // images with steps[b] <= t are frozen from step t on (from the start when steps[b] == 0)
-        e = launch_steps_schedule(g, t, iters, steps, frozen, block_frozen, st, &g_launches);
-        if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "step schedule launch before step %d: %s", t, cudaGetErrorString(e));
-      }
-      Bf16Buffers b{};
-      b.s32_in = (s0_direct && t == 0) ? (state_in ? state_in : init_levels) : loc(t); b.s32_out = loc(t + 1);
-      b.s32_in_bcast = (s0_direct && t == 0 && !state_in) ? 1 : 0;
-      b.sb_in = sb[(t + p0) & 1]; b.sb_out = sb[(t + p0 + 1) & 1];
-      b.sp_in = sp[(t + p0) & 1]; b.sp_out = sp[(t + p0 + 1) & 1];
-      b.xb = xb;
-      b.h = reinterpret_cast<__nv_bfloat16*>(ws + wl.h_off);
-      b.attn_acc = wl.attn_acc_bytes ? reinterpret_cast<float*>(ws + wl.attn_acc_off) : nullptr;
-      b.c = reinterpret_cast<__nv_bfloat16*>(ws + wl.c_off);
-      b.nsq_in = nsq[(t + p0) & 1]; b.nsq_out = nsq[(t + p0 + 1) & 1];
-      b.pos = pos;
-      b.w1 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w1_off);
-      b.w2 = reinterpret_cast<const __nv_bfloat16*>(pw + pl.w2_off);
-      b.b1 = reinterpret_cast<const float*>(pw + pl.b1_off);
-      b.b2 = reinterpret_cast<const float*>(pw + pl.b2_off);
-      b.frozen = frozen; b.block_frozen = block_frozen; b.dsq_out = dsq;
-      char msg[400] = "";
-      const int r = step_bf16(g, b, t, g_encode, di.sms, st, &g_launches, msg, sizeof(msg), &g_prof);
-      if (r) return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "step %d: %s", t, msg);
-      if (settle) {
-        e = launch_settle_converge(g, t + 1, settle->tol, dsq, b.nsq_out, frozen, block_frozen,
-                                   reinterpret_cast<unsigned int*>(ws + sl.done_off), reinterpret_cast<float*>(ws + sl.level_q_off),
-                                   settle->steps, st, &g_launches);
-        if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "settle convergence launch after step %d: %s", t, cudaGetErrorString(e));
-      }
-    }
-    // settle and forward_steps: return_all slab t of image b must be S_min(t, steps[b]).  Otherwise S_steps[b] is in
-    // loc(steps[b]) and the ones in the workspace slab move to state_out; steps[b] == 0 (forward_steps only) takes S_0,
-    // which step 0 read straight from state_in / init_levels
-    const int32_t* image_steps = settle ? settle->steps : steps;
-    if (image_steps && return_all) {
-      e = launch_steps_fill(g, iters, image_steps, state_out, st, &g_launches);
-      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "return_all fill launch: %s", cudaGetErrorString(e));
-    } else if (image_steps && iters > 0) {
-      e = launch_settle_gather(g, iters, image_steps, wslab, state_out, state_in ? state_in : init_levels, state_in ? 0 : 1,
-                               st, &g_launches);
-      if (e != cudaSuccess)
-        return fail(GLOM_B200_ERR_CUDA, "%s gather launch: %s", settle ? "settle" : "step", cudaGetErrorString(e));
-    }
-  } else {
-    cudaError_t e = launch_broadcast_init(g, state_in, init_levels, loc(0), st, &g_launches, &g_prof);
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "init launch: %s", cudaGetErrorString(e));
-    for (int t = 0; t < iters; ++t) {
-      F32Buffers b{};
-      b.s_in = loc(t); b.s_out = loc(t + 1);
-      b.x = tokens; b.pos = pos;
-      b.h = reinterpret_cast<float*>(ws + wl.h_off);
-      b.c = reinterpret_cast<float*>(ws + wl.c_off);
-      b.w1 = reinterpret_cast<const float*>(pw + pl.w1_off);
-      b.w2 = reinterpret_cast<const float*>(pw + pl.w2_off);
-      b.b1 = reinterpret_cast<const float*>(pw + pl.b1_off);
-      b.b2 = reinterpret_cast<const float*>(pw + pl.b2_off);
-      e = step_f32(g, b, st, &g_launches, &g_prof);
-      if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "fp32 step %d launch: %s", t, cudaGetErrorString(e));
-    }
+    if (int r = ln.launched(cudaMemcpyAsync(remaining_out, q.unfinished, sizeof(int32_t), cudaMemcpyDeviceToDevice, ln.st)))
+      return fail(r, "%s count copy: %s", fn, ln.err);
   }
   g_err[0] = 0;
   return 0;
@@ -687,9 +705,14 @@ GLOM_B200_API int glom_b200_settle_video_run(const glom_b200_cfg* cfg, const voi
 
 static int tok_kp(int patch) { return (3 * patch * patch + 63) / 64 * 64; }
 
+// true unless the image is a batch of whole patches
+static bool bad_patch_grid(int batch, int height, int width, int patch) {
+  return batch < 1 || patch < 1 || height < patch || width < patch || height % patch || width % patch;
+}
+
 GLOM_B200_API int glom_b200_tokenize_workspace_bytes(int batch, int height, int width, int patch, int dim, int precision,
                                                      size_t* out_bytes) {
-  if (!out_bytes || batch < 1 || patch < 1 || dim < 1 || height < patch || width < patch || height % patch || width % patch)
+  if (!out_bytes || dim < 1 || bad_patch_grid(batch, height, width, patch))
     return fail(GLOM_B200_ERR_INVALID, "bad tokeniser geometry");
   if (precision == GLOM_B200_BF16) {
     const size_t rows = (size_t)batch * (height / patch) * (width / patch);
@@ -703,39 +726,36 @@ GLOM_B200_API int glom_b200_tokenize_workspace_bytes(int batch, int height, int 
 GLOM_B200_API int glom_b200_tokenize(const float* img, const float* weight, const float* bias, float* tokens, int batch, int height,
                        int width, int patch, int dim, int precision, void* workspace, size_t workspace_bytes, void* stream) {
   if (!img || !weight || !bias || !tokens) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
-  if (batch < 1 || patch < 1 || dim < 1 || height < patch || width < patch || height % patch || width % patch)
+  if (dim < 1 || bad_patch_grid(batch, height, width, patch))
     return fail(GLOM_B200_ERR_INVALID, "image %dx%d is not a positive multiple of patch %d", height, width, patch);
   if (precision != GLOM_B200_FP32 && precision != GLOM_B200_BF16) return fail(GLOM_B200_ERR_INVALID, "unknown precision %d", precision);
   DeviceInfo di{};
   if (int r = device_info(&di)) return r;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  g_launches = 0;
+  Launch& ln = begin_launch(di.sms, stream);
   if (precision == GLOM_B200_FP32) {
-    cudaError_t e = launch_tokenize(img, weight, bias, tokens, batch, height, width, patch, dim, st, &g_launches, &g_prof);
-    if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "tokenize launch: %s", cudaGetErrorString(e));
+    if (int r = launch_tokenize(img, weight, bias, tokens, batch, height, width, patch, dim, ln))
+      return fail(r, "tokenize launch: %s", ln.err);
     return 0;
   }
   if (dim % 64) return fail(GLOM_B200_ERR_INVALID, "bf16 tokeniser needs dim %% 64 == 0 (got %d)", dim);
   size_t need = 0;
   glom_b200_tokenize_workspace_bytes(batch, height, width, patch, dim, precision, &need);
-  if (!workspace || workspace_bytes < need || reinterpret_cast<uintptr_t>(workspace) % 1024)
+  if (!workspace || workspace_bytes < need || misaligned(workspace, 1024))
     return fail(GLOM_B200_ERR_WORKSPACE, "tokeniser workspace: need %zu bytes 1024-aligned, got %zu", need, workspace_bytes);
   const int kp = tok_kp(patch);
   const int rows = batch * (height / patch) * (width / patch);
   __nv_bfloat16* patches = static_cast<__nv_bfloat16*>(workspace);
   __nv_bfloat16* wtok = reinterpret_cast<__nv_bfloat16*>(static_cast<char*>(workspace) + align_up((size_t)rows * kp * 2, 1024));
-  ProfScope scope(&g_prof, PROF_TOKENIZE, st);
-  cudaError_t e = launch_patchify_bf16(img, weight, patches, wtok, batch, height, width, patch, dim, kp, st, &g_launches);
-  if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "patchify launch: %s", cudaGetErrorString(e));
-  char msg[300] = "";
-  if (int r = tokenize_tc(patches, wtok, bias, tokens, rows, dim, kp, g_encode, di.sms, st, &g_launches, msg, sizeof(msg)))
-    return fail(GLOM_B200_ERR_CUDA, "%s", msg);
+  ProfScope scope(ln.prof, PROF_TOKENIZE, ln.st);
+  if (int r = launch_patchify_bf16(img, weight, patches, wtok, batch, height, width, patch, dim, kp, ln))
+    return fail(r, "patchify launch: %s", ln.err);
+  if (int r = tokenize_tc(patches, wtok, bias, tokens, rows, dim, kp, ln)) return fail(r, "%s", ln.err);
   return 0;
 }
 
 GLOM_B200_API int glom_b200_tokenize_backward_workspace_bytes(int batch, int height, int width, int patch, int need_d_img,
                                                               size_t* out_bytes) {
-  if (!out_bytes || batch < 1 || patch < 1 || height < patch || width < patch || height % patch || width % patch)
+  if (!out_bytes || bad_patch_grid(batch, height, width, patch))
     return fail(GLOM_B200_ERR_INVALID, "tokeniser backward: bad arguments");
   *out_bytes = tokenize_backward_workspace_bytes(batch, height, width, patch, need_d_img);
   return 0;
@@ -745,17 +765,17 @@ static int tokenize_backward_impl(const float* img, const float* weight, const f
                                   float* d_bias, float* d_img, int batch, int height, int width, int patch, int dim,
                                   int deterministic, void* workspace, size_t workspace_bytes, void* stream) {
   if (!img || !weight || !d_tokens) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
-  if (batch < 1 || patch < 1 || dim < 1 || height < patch || width < patch || height % patch || width % patch)
+  if (dim < 1 || bad_patch_grid(batch, height, width, patch))
     return fail(GLOM_B200_ERR_INVALID, "image %dx%d is not a positive multiple of patch %d", height, width, patch);
   DeviceInfo di{};
   if (int r = device_info(&di)) return r;
   const size_t need = tokenize_backward_workspace_bytes(batch, height, width, patch, d_img != nullptr);
   if ((d_weight || d_img) && (!workspace || workspace_bytes < need))
     return fail(GLOM_B200_ERR_WORKSPACE, "tokeniser backward workspace: need %zu bytes, got %zu", need, workspace_bytes);
-  g_launches = 0;
-  const cudaError_t e = tokenize_backward(img, weight, d_tokens, d_weight, d_bias, d_img, batch, height, width, patch, dim,
-                                          workspace, static_cast<cudaStream_t>(stream), &g_launches, deterministic);
-  if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "tokeniser backward: %s", cudaGetErrorString(e));
+  Launch& ln = begin_launch(di.sms, stream);
+  if (int r = tokenize_backward(img, weight, d_tokens, d_weight, d_bias, d_img, batch, height, width, patch, dim, workspace, ln,
+                                deterministic))
+    return fail(r, "tokeniser backward: %s", ln.err);
   return 0;
 }
 
@@ -783,6 +803,33 @@ GLOM_B200_API int glom_b200_backward_workspace_bytes(const glom_b200_cfg* cfg, i
   return 0;
 }
 
+// The weight / gradient structs and tensor pointers of a backward, validated and gathered into `a`.  The explicit backward
+// takes exactly one of d_state0 / d_init; the implicit one (`implicit`) neither
+static int bind_backward(const glom_b200_weights_ref* w, const float* tokens, const float* pos, const float* states,
+                         const float* grad_out, const glom_b200_grads* gr, bool implicit, int deterministic, BackwardArgs* a) {
+  if (!w || w->struct_size != sizeof(glom_b200_weights_ref) || !gr || gr->struct_size != sizeof(glom_b200_grads))
+    return fail(GLOM_B200_ERR_INVALID, "weights / grads struct missing or wrong size");
+  if (!tokens || !pos || !states || !grad_out) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
+  if (!w->bu_w1 || !w->bu_b1 || !w->bu_w2 || !w->td_w1 || !w->td_b1 || !w->td_w2)
+    return fail(GLOM_B200_ERR_INVALID, "a weight pointer is NULL");
+  const bool outputs = gr->d_tokens && gr->d_pos && gr->d_bu_w1 && gr->d_bu_b1 && gr->d_bu_w2 && gr->d_bu_b2 && gr->d_td_w1 &&
+                       gr->d_td_b1 && gr->d_td_w2 && gr->d_td_b2;
+  if (!implicit && (!outputs || (!gr->d_state0 == !gr->d_init)))
+    return fail(GLOM_B200_ERR_INVALID, "gradient pointers: all MLP/token/pos outputs and exactly one of d_state0 / d_init");
+  if (implicit && !outputs) return fail(GLOM_B200_ERR_INVALID, "gradient pointers: all MLP/token/pos outputs are needed");
+  if (implicit && (gr->d_state0 || gr->d_init))
+    return fail(GLOM_B200_ERR_INVALID, "backward_implicit: d_state0 and d_init must be NULL (the fixed point does not "
+                                       "depend on the start state)");
+  *a = BackwardArgs{};
+  a->tokens = tokens; a->pos = pos; a->states = states; a->grad_out = grad_out;
+  a->bu_w1 = w->bu_w1; a->bu_b1 = w->bu_b1; a->bu_w2 = w->bu_w2; a->td_w1 = w->td_w1; a->td_b1 = w->td_b1; a->td_w2 = w->td_w2;
+  a->d_tokens = gr->d_tokens; a->d_pos = gr->d_pos; a->d_state0 = gr->d_state0; a->d_init = gr->d_init;
+  a->d_bu_w1 = gr->d_bu_w1; a->d_bu_b1 = gr->d_bu_b1; a->d_bu_w2 = gr->d_bu_w2; a->d_bu_b2 = gr->d_bu_b2;
+  a->d_td_w1 = gr->d_td_w1; a->d_td_b1 = gr->d_td_b1; a->d_td_w2 = gr->d_td_w2; a->d_td_b2 = gr->d_td_b2;
+  a->deterministic = deterministic;
+  return 0;
+}
+
 // glom_b200_backward (steps == NULL) and glom_b200_backward_steps (per-image step counts, iters = max_steps)
 static int backward_impl(const glom_b200_cfg* cfg, const glom_b200_weights_ref* w, const float* tokens, const float* pos,
                          const float* states, const float* grad_out, const glom_b200_grads* gr, int batch, int iters,
@@ -790,32 +837,16 @@ static int backward_impl(const glom_b200_cfg* cfg, const glom_b200_weights_ref* 
                          int deterministic = 0) {
   if (int r = check_cfg(cfg)) return r;
   if (batch < 1 || iters < 0) return fail(GLOM_B200_ERR_INVALID, "batch must be >= 1 and iters >= 0");
-  if (!w || w->struct_size != sizeof(glom_b200_weights_ref) || !gr || gr->struct_size != sizeof(glom_b200_grads))
-    return fail(GLOM_B200_ERR_INVALID, "weights / grads struct missing or wrong size");
-  if (!tokens || !pos || !states || !grad_out) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
-  if (!w->bu_w1 || !w->bu_b1 || !w->bu_w2 || !w->td_w1 || !w->td_b1 || !w->td_w2)
-    return fail(GLOM_B200_ERR_INVALID, "a weight pointer is NULL");
-  if (!gr->d_tokens || !gr->d_pos || !gr->d_bu_w1 || !gr->d_bu_b1 || !gr->d_bu_w2 || !gr->d_bu_b2 || !gr->d_td_w1 ||
-      !gr->d_td_b1 || !gr->d_td_w2 || !gr->d_td_b2 || (!gr->d_state0 == !gr->d_init))
-    return fail(GLOM_B200_ERR_INVALID, "gradient pointers: all MLP/token/pos outputs and exactly one of d_state0 / d_init");
+  BackwardArgs a{};
+  if (int r = bind_backward(w, tokens, pos, states, grad_out, gr, false, deterministic, &a)) return r;
   DeviceInfo di{};
   if (int r = device_info(&di)) return r;
   const Geometry g = make_geometry(cfg, batch);
   const BackwardLayout wl = backward_layout(g, cfg->precision);
-  if (!workspace || workspace_bytes < wl.total || reinterpret_cast<uintptr_t>(workspace) % 1024)
+  if (!workspace || workspace_bytes < wl.total || misaligned(workspace, 1024))
     return fail(GLOM_B200_ERR_WORKSPACE, "backward workspace: need %zu bytes 1024-aligned, got %zu", wl.total, workspace_bytes);
-  BackwardArgs a{};
-  a.tokens = tokens; a.pos = pos; a.states = states; a.grad_out = grad_out;
-  a.bu_w1 = w->bu_w1; a.bu_b1 = w->bu_b1; a.bu_w2 = w->bu_w2; a.td_w1 = w->td_w1; a.td_b1 = w->td_b1; a.td_w2 = w->td_w2;
-  a.d_tokens = gr->d_tokens; a.d_pos = gr->d_pos; a.d_state0 = gr->d_state0; a.d_init = gr->d_init;
-  a.d_bu_w1 = gr->d_bu_w1; a.d_bu_b1 = gr->d_bu_b1; a.d_bu_w2 = gr->d_bu_w2; a.d_bu_b2 = gr->d_bu_b2;
-  a.d_td_w1 = gr->d_td_w1; a.d_td_b1 = gr->d_td_b1; a.d_td_w2 = gr->d_td_w2; a.d_td_b2 = gr->d_td_b2;
-  a.deterministic = deterministic;
-  g_launches = 0;
-  char msg[400] = "";
-  if (int r = backward_run(g, a, cfg->precision, iters, grad_all, steps, workspace, g_encode, di.sms,
-                           static_cast<cudaStream_t>(stream), &g_launches, msg, sizeof(msg)))
-    return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "%s", msg);
+  Launch& ln = begin_launch(di.sms, stream);
+  if (int r = backward_run(g, a, cfg->precision, iters, grad_all, steps, workspace, ln)) return fail(r, "%s", ln.err);
   g_err[0] = 0;
   return 0;
 }
@@ -845,7 +876,7 @@ GLOM_B200_API int glom_b200_backward_ex(const glom_b200_cfg* cfg, const glom_b20
                                         void* stream) {
   if (deterministic != 0 && deterministic != 1)
     return fail(GLOM_B200_ERR_INVALID, "backward_ex: deterministic must be 0 or 1 (got %d)", deterministic);
-  if (steps && reinterpret_cast<uintptr_t>(steps) % 4) return fail(GLOM_B200_ERR_INVALID, "backward_ex: steps must be 4-byte aligned");
+  if (steps && misaligned(steps, 4)) return fail(GLOM_B200_ERR_INVALID, "backward_ex: steps must be 4-byte aligned");
   if (steps && max_steps < 0) return fail(GLOM_B200_ERR_INVALID, "backward_ex: max_steps must be >= 0 (got %d)", max_steps);
   return backward_impl(cfg, w, tokens, pos, states, grad_out, gr, batch, max_steps, steps, grad_all, workspace,
                        workspace_bytes, stream, deterministic);
@@ -873,38 +904,20 @@ GLOM_B200_API int glom_b200_backward_implicit(const glom_b200_cfg* cfg, const gl
   if (deterministic != 0 && deterministic != 1)
     return fail(GLOM_B200_ERR_INVALID, "backward_implicit: deterministic must be 0 or 1 (got %d)", deterministic);
   if (int r = check_steps_ptr("backward_implicit", "adjoint_steps_out", adjoint_steps_out)) return r;
-  if (reinterpret_cast<uintptr_t>(adjoint_q_out) % 4)
+  if (misaligned(adjoint_q_out, 4))
     return fail(GLOM_B200_ERR_INVALID, "backward_implicit: adjoint_q_out must be 4-byte aligned");
-  if (!w || w->struct_size != sizeof(glom_b200_weights_ref) || !gr || gr->struct_size != sizeof(glom_b200_grads))
-    return fail(GLOM_B200_ERR_INVALID, "weights / grads struct missing or wrong size");
-  if (!tokens || !pos || !state || !grad_out) return fail(GLOM_B200_ERR_INVALID, "a required pointer is NULL");
-  if (!w->bu_w1 || !w->bu_b1 || !w->bu_w2 || !w->td_w1 || !w->td_b1 || !w->td_w2)
-    return fail(GLOM_B200_ERR_INVALID, "a weight pointer is NULL");
-  if (!gr->d_tokens || !gr->d_pos || !gr->d_bu_w1 || !gr->d_bu_b1 || !gr->d_bu_w2 || !gr->d_bu_b2 || !gr->d_td_w1 ||
-      !gr->d_td_b1 || !gr->d_td_w2 || !gr->d_td_b2)
-    return fail(GLOM_B200_ERR_INVALID, "gradient pointers: all MLP/token/pos outputs are needed");
-  if (gr->d_state0 || gr->d_init)
-    return fail(GLOM_B200_ERR_INVALID, "backward_implicit: d_state0 and d_init must be NULL (the fixed point does not "
-                                       "depend on the start state)");
+  BackwardArgs a{};
+  if (int r = bind_backward(w, tokens, pos, state, grad_out, gr, true, deterministic, &a)) return r;
   DeviceInfo di{};
   if (int r = device_info(&di)) return r;
   const Geometry g = make_geometry(cfg, batch);
   const ImplicitLayout il = implicit_layout(g);
-  if (!workspace || workspace_bytes < il.total || reinterpret_cast<uintptr_t>(workspace) % 1024)
+  if (!workspace || workspace_bytes < il.total || misaligned(workspace, 1024))
     return fail(GLOM_B200_ERR_WORKSPACE, "backward_implicit workspace: need %zu bytes 1024-aligned, got %zu", il.total,
                 workspace_bytes);
-  BackwardArgs a{};
-  a.tokens = tokens; a.pos = pos; a.states = state; a.grad_out = grad_out;
-  a.bu_w1 = w->bu_w1; a.bu_b1 = w->bu_b1; a.bu_w2 = w->bu_w2; a.td_w1 = w->td_w1; a.td_b1 = w->td_b1; a.td_w2 = w->td_w2;
-  a.d_tokens = gr->d_tokens; a.d_pos = gr->d_pos;
-  a.d_bu_w1 = gr->d_bu_w1; a.d_bu_b1 = gr->d_bu_b1; a.d_bu_w2 = gr->d_bu_w2; a.d_bu_b2 = gr->d_bu_b2;
-  a.d_td_w1 = gr->d_td_w1; a.d_td_b1 = gr->d_td_b1; a.d_td_w2 = gr->d_td_w2; a.d_td_b2 = gr->d_td_b2;
-  a.deterministic = deterministic;
-  g_launches = 0;
-  char msg[400] = "";
-  if (int r = backward_implicit_run(g, a, adjoint_iters, adjoint_tol, adjoint_steps_out, adjoint_q_out, workspace, g_encode,
-                                    di.sms, static_cast<cudaStream_t>(stream), &g_launches, msg, sizeof(msg)))
-    return fail(r == -1 ? GLOM_B200_ERR_INVALID : GLOM_B200_ERR_CUDA, "%s", msg);
+  Launch& ln = begin_launch(di.sms, stream);
+  if (int r = backward_implicit_run(g, a, adjoint_iters, adjoint_tol, adjoint_steps_out, adjoint_q_out, workspace, ln))
+    return fail(r, "%s", ln.err);
   g_err[0] = 0;
   return 0;
 }
@@ -917,13 +930,13 @@ GLOM_B200_API int glom_b200_islands(const float* states, int slabs, int side_h, 
   if (slabs < 1 || slabs > 65535 || side_h < 1 || side_w < 1 || (long long)side_h * side_w > 8192 || levels < 1 ||
       levels > 65535 || dim < 4 || dim % 4)
     return fail(GLOM_B200_ERR_INVALID, "islands: need 1 <= slabs, levels <= 65535, side_h * side_w <= 8192, dim %% 4 == 0");
-  if (reinterpret_cast<uintptr_t>(states) % 16) return fail(GLOM_B200_ERR_INVALID, "states must be 16-byte aligned");
+  if (misaligned(states, 16)) return fail(GLOM_B200_ERR_INVALID, "states must be 16-byte aligned");
   DeviceInfo di{};
   if (int r = device_info(&di)) return r;
-  g_launches = 0;
-  cudaError_t e = launch_islands(states, slabs, side_h, side_w, levels, dim, threshold, cos_right, cos_down, agreement, labels,
-                                 num_islands, static_cast<cudaStream_t>(stream), &g_launches);
-  if (e != cudaSuccess) return fail(GLOM_B200_ERR_CUDA, "islands launch: %s", cudaGetErrorString(e));
+  Launch& ln = begin_launch(di.sms, stream);
+  if (int r = launch_islands(states, slabs, side_h, side_w, levels, dim, threshold, cos_right, cos_down, agreement, labels,
+                             num_islands, ln))
+    return fail(r, "islands launch: %s", ln.err);
   return 0;
 }
 

@@ -115,26 +115,20 @@ island_label_kernel(const float* __restrict__ cos_right, const float* __restrict
   if (threadIdx.x == 0) num_islands[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = total;
 }
 
-cudaError_t launch_islands(const float* states, int slabs, int side_h, int side_w, int L, int d, float threshold,
-                           float* cos_right, float* cos_down, float* agreement, int* labels, int* num_islands,
-                           cudaStream_t st, int* launches) {
+int launch_islands(const float* states, int slabs, int side_h, int side_w, int L, int d, float threshold, float* cos_right,
+                   float* cos_down, float* agreement, int* labels, int* num_islands, Launch& ln) {
+  cudaStream_t st = ln.st;
   const int n = side_h * side_w;
   island_edges_kernel<<<dim3(side_h, L, slabs), 256, 0, st>>>(states, side_h, side_w, L, d, cos_right, cos_down);
-  if (launches) ++*launches;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
+  GLOM_TRY(ln.launched());
   const size_t smem = (size_t)n * 4 + 2 * (size_t)n;
   // 6n bytes plus the kernel's static shared memory exceed the default 48 KB per block from n = 8190 on (the API allows
   // n <= 8192): opt in above 46 KB
   static SmemOptIn optin;
-  if (smem > 46 * 1024) {
-    e = optin.ensure(island_label_kernel, smem);
-    if (e != cudaSuccess) return e;
-  }
+  if (smem > 46 * 1024) GLOM_TRY(ln.check(optin.ensure(island_label_kernel, smem)));
   island_label_kernel<<<dim3(L, slabs), 256, smem, st>>>(cos_right, cos_down, side_h, side_w, threshold, agreement,
                                                           labels, num_islands);
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  return ln.launched();
 }
 
 }  // namespace glom

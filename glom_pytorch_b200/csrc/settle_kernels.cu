@@ -87,20 +87,25 @@ settle_converge_kernel(int n, int L, int nparts, int B, int rows, int step, floa
   if (tid == 0) *done = 0u;                         // ready for the next step's launch
 }
 
-cudaError_t launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
-                                   int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, cudaStream_t st,
-                                   int* launches, const QueueSlots* q) {
+// a block of SETTLE_THREADS threads per grid point, launched with programmatic stream serialisation
+template <typename... Params, typename... Args>
+static cudaError_t launch_pdl(void (*kernel)(Params...), dim3 grid, cudaStream_t st, Args... args) {
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(g.L, g.B);
+  cfg.gridDim = grid;
   cfg.blockDim = dim3(SETTLE_THREADS);
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernel
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernels
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  if (launches) ++*launches;
-  return cudaLaunchKernelEx(&cfg, settle_converge_kernel, g.n, g.L, g.nparts, g.B, g.rows, step, tol, dsq, nsq, frozen,
-                            block_frozen, done, level_q, steps, q ? *q : QueueSlots{});
+  return cudaLaunchKernelEx(&cfg, kernel, args...);
+}
+
+int launch_settle_converge(const Geometry& g, int step, float tol, const float* dsq, const float* nsq, int* frozen,
+                           int* block_frozen, unsigned int* done, float* level_q, int32_t* steps, Launch& ln,
+                           const QueueSlots* q) {
+  return ln.launched(launch_pdl(settle_converge_kernel, dim3(g.L, g.B), ln.st, g.n, g.L, g.nparts, g.B, g.rows, step, tol, dsq,
+                                nsq, frozen, block_frozen, done, level_q, steps, q ? *q : QueueSlots{}));
 }
 
 __device__ __forceinline__ int clamp_steps(int s, int max_steps) { return min(max(s, 0), max_steps); }
@@ -130,14 +135,13 @@ static unsigned copy_chunks(const Geometry& g, size_t per_img4) {
   return (unsigned)(want < cap ? want : cap);
 }
 
-cudaError_t launch_settle_gather(const Geometry& g, int max_iters, const int32_t* steps, const float* slab, float* state_out,
-                                 const float* s0, int s0_bcast, cudaStream_t st, int* launches) {
+int launch_settle_gather(const Geometry& g, int max_iters, const int32_t* steps, const float* slab, float* state_out,
+                         const float* s0, int s0_bcast, Launch& ln) {
   const size_t per_img4 = (size_t)g.n * g.L * g.d / 4;
-  settle_gather_kernel<<<dim3(copy_chunks(g, per_img4), g.B), 256, 0, st>>>(
+  settle_gather_kernel<<<dim3(copy_chunks(g, per_img4), g.B), 256, 0, ln.st>>>(
       max_iters, steps, per_img4, reinterpret_cast<const float4*>(slab), reinterpret_cast<float4*>(state_out),
       reinterpret_cast<const float4*>(s0), s0_bcast, (unsigned)(g.L * g.d / 4));
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  return ln.launched();
 }
 
 // glom_b200_forward_steps, before step t: frozen[b] = steps[b] <= t (steps clamped to [0, max_steps]) and
@@ -161,19 +165,11 @@ steps_schedule_kernel(int n, int B, int rows, int t, int max_steps, const int32_
   }
 }
 
-cudaError_t launch_steps_schedule(const Geometry& g, int t, int max_steps, const int32_t* steps, int* frozen, int* block_frozen,
-                                  cudaStream_t st, int* launches) {
+int launch_steps_schedule(const Geometry& g, int t, int max_steps, const int32_t* steps, int* frozen, int* block_frozen,
+                          Launch& ln) {
   const int items = g.B + (g.rows + 255) / 256;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((items + SETTLE_THREADS - 1) / SETTLE_THREADS);
-  cfg.blockDim = dim3(SETTLE_THREADS);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernel
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  if (launches) ++*launches;
-  return cudaLaunchKernelEx(&cfg, steps_schedule_kernel, g.n, g.B, g.rows, t, max_steps, steps, frozen, block_frozen);
+  return ln.launched(launch_pdl(steps_schedule_kernel, dim3((items + SETTLE_THREADS - 1) / SETTLE_THREADS), ln.st, g.n, g.B,
+                                g.rows, t, max_steps, steps, frozen, block_frozen));
 }
 
 // Grid (chunks, B), return_all: the step kernels store nothing for the rows of a frozen image, so slabs
@@ -190,13 +186,11 @@ __global__ void steps_fill_kernel(int max_steps, const int32_t* __restrict__ ste
   }
 }
 
-cudaError_t launch_steps_fill(const Geometry& g, int max_steps, const int32_t* steps, float* states, cudaStream_t st,
-                              int* launches) {
+int launch_steps_fill(const Geometry& g, int max_steps, const int32_t* steps, float* states, Launch& ln) {
   const size_t per_img4 = (size_t)g.n * g.L * g.d / 4;
-  steps_fill_kernel<<<dim3(copy_chunks(g, per_img4), g.B), 256, 0, st>>>(max_steps, steps, per_img4, per_img4 * g.B,
-                                                                         reinterpret_cast<float4*>(states));
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  steps_fill_kernel<<<dim3(copy_chunks(g, per_img4), g.B), 256, 0, ln.st>>>(max_steps, steps, per_img4, per_img4 * g.B,
+                                                                            reinterpret_cast<float4*>(states));
+  return ln.launched();
 }
 
 // ---- Glom.settle_queue: N images through B slots.  Slot s holds image slot_img[s]; its rows are rows s*n .. s*n+n-1
@@ -207,19 +201,6 @@ cudaError_t launch_steps_fill(const Geometry& g, int max_steps, const int32_t* s
 // Glom.settle_video runs the same kernels with q.frames = F > 1: the images are the frames i = stream * F + f, a slot
 // whose frame f < F - 1 stops takes frame f + 1 of its own stream, and that frame's S_0 is the slot's own S_k (the
 // settle_queue call is the case F = 1, where no slot continues).
-
-template <typename... Params, typename... Args>
-static cudaError_t launch_pdl(void (*kernel)(Params...), dim3 grid, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = dim3(SETTLE_THREADS);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;      // PDL: see pdl_wait() in the kernels
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, args...);
-}
 
 // One block: every slot empty (frozen, no image), every image queued.
 __global__ void __launch_bounds__(SETTLE_THREADS)
@@ -234,11 +215,9 @@ queue_init_kernel(int B, int nblk, QueueSlots q, int* frozen, int* block_frozen,
   if (threadIdx.x == 0) { *q.head = 0; *q.unfinished = q.images; *done = 0u; }
 }
 
-cudaError_t launch_queue_init(const Geometry& g, const QueueSlots& q, int* frozen, int* block_frozen, unsigned int* done,
-                              cudaStream_t st, int* launches, Profiler* prof) {
-  ProfScope scope(prof, PROF_PREP, st);
-  if (launches) ++*launches;
-  return launch_pdl(queue_init_kernel, dim3(1), st, g.B, (g.rows + 255) / 256, q, frozen, block_frozen, done);
+int launch_queue_init(const Geometry& g, const QueueSlots& q, int* frozen, int* block_frozen, unsigned int* done, Launch& ln) {
+  ProfScope scope(ln.prof, PROF_PREP, ln.st);
+  return ln.launched(launch_pdl(queue_init_kernel, dim3(1), ln.st, g.B, (g.rows + 255) / 256, q, frozen, block_frozen, done));
 }
 
 // One block, before a step.  The open slots (frozen: their image stopped, or empty) hand a pending image over to the fill
@@ -290,11 +269,9 @@ queue_schedule_kernel(int n, int B, int rows, int admit, QueueSlots q, int* froz
   }
 }
 
-cudaError_t launch_queue_schedule(const Geometry& g, const QueueSlots& q, int admit, int* frozen, int* block_frozen,
-                                  cudaStream_t st, int* launches, Profiler* prof) {
-  ProfScope scope(prof, PROF_PREP, st);
-  if (launches) ++*launches;
-  return launch_pdl(queue_schedule_kernel, dim3(1), st, g.n, g.B, g.rows, admit, q, frozen, block_frozen);
+int launch_queue_schedule(const Geometry& g, const QueueSlots& q, int admit, int* frozen, int* block_frozen, Launch& ln) {
+  ProfScope scope(ln.prof, PROF_PREP, ln.st);
+  return ln.launched(launch_pdl(queue_schedule_kernel, dim3(1), ln.st, g.n, g.B, g.rows, admit, q, frozen, block_frozen));
 }
 
 constexpr int FILL_ROWS = 8;                        // rows of one slot per block of the fill
@@ -337,14 +314,12 @@ queue_fill_kernel(int n, int L, int d, int nparts, int part_w, QueueSlots q, con
   for (int k = threadIdx.x; k < ni * d / 4; k += SETTLE_THREADS) xo[k] = cast4_bf16(tk[k]);
 }
 
-cudaError_t launch_queue_fill(const Geometry& g, const QueueSlots& q, const float* tokens, const float* pos,
-                              const float* state_in, const float* init_levels, float* state_out, float* slab,
-                              __nv_bfloat16* sb, __nv_bfloat16* sp, float* nsq, __nv_bfloat16* xb, cudaStream_t st,
-                              int* launches, Profiler* prof) {
-  ProfScope scope(prof, PROF_PREP, st);
-  if (launches) ++*launches;
-  return launch_pdl(queue_fill_kernel, dim3((g.n + FILL_ROWS - 1) / FILL_ROWS, g.B), st, g.n, g.L, g.d, g.nparts, g.part_w,
-                    q, tokens, pos, state_in, init_levels, state_out, slab, sb, sp, nsq, xb);
+int launch_queue_fill(const Geometry& g, const QueueSlots& q, const float* tokens, const float* pos, const float* state_in,
+                      const float* init_levels, float* state_out, float* slab, __nv_bfloat16* sb, __nv_bfloat16* sp,
+                      float* nsq, __nv_bfloat16* xb, Launch& ln) {
+  ProfScope scope(ln.prof, PROF_PREP, ln.st);
+  return ln.launched(launch_pdl(queue_fill_kernel, dim3((g.n + FILL_ROWS - 1) / FILL_ROWS, g.B), ln.st, g.n, g.L, g.d, g.nparts,
+                                g.part_w, q, tokens, pos, state_in, init_levels, state_out, slab, sb, sp, nsq, xb));
 }
 
 }  // namespace glom

@@ -56,9 +56,9 @@ __global__ void pack_weights_kernel(int d, int L, const float* __restrict__ bu_w
   }
 }
 
-cudaError_t launch_pack(int d, int L, int precision, const float* bu_w1, const float* bu_b1, const float* bu_w2,
-                        const float* bu_b2, const float* td_w1, const float* td_b1, const float* td_w2,
-                        const float* td_b2, void* packed, cudaStream_t st, int* launches) {
+int launch_pack(int d, int L, int precision, const float* bu_w1, const float* bu_b1, const float* bu_w2, const float* bu_b2,
+                const float* td_w1, const float* td_b1, const float* td_w2, const float* td_b2, void* packed, Launch& ln) {
+  cudaStream_t st = ln.st;
   const PackedLayout pl = packed_layout(d, L, precision);
   char* base = static_cast<char*>(packed);
   float* b1p = reinterpret_cast<float*>(base + pl.b1_off);
@@ -74,8 +74,7 @@ cudaError_t launch_pack(int d, int L, int precision, const float* bu_w1, const f
                                                         reinterpret_cast<float*>(base + pl.w1_off),
                                                         reinterpret_cast<float*>(base + pl.w2_off), b1p, b2p);
   }
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  return ln.launched();
 }
 
 // =====================================================================================
@@ -101,24 +100,20 @@ __global__ void cast_bf16_kernel(size_t n4, const float* __restrict__ src, __nv_
     reinterpret_cast<uint2*>(dst)[i] = cast4_bf16(reinterpret_cast<const float4*>(src)[i]);
 }
 
-cudaError_t launch_prep(const Geometry& g, const float* state_in, const float* init_levels, const float* pos,
-                        const float* tokens, float* s32_dst, __nv_bfloat16* sb, __nv_bfloat16* sp,
-                        __nv_bfloat16* xb, float* nsq, cudaStream_t st, int* launches, Profiler* prof) {
-  ProfScope scope(prof, PROF_PREP, st);
-  cudaError_t e = cudaSuccess;
+int launch_prep(const Geometry& g, const float* state_in, const float* init_levels, const float* pos, const float* tokens,
+                float* s32_dst, __nv_bfloat16* sb, __nv_bfloat16* sp, __nv_bfloat16* xb, float* nsq, Launch& ln) {
+  cudaStream_t st = ln.st;
+  ProfScope scope(ln.prof, PROF_PREP, st);
   if (sb) {              // sb == NULL: the state's shadows and norm partials are already in place (resumed call): tokens only
     const int warps = g.rows * g.L;
     const int block = 256, grid = (warps * 32 + block - 1) / block;
     prep_state_kernel<<<grid, block, 0, st>>>(g.rows, g.n, g.L, g.d, g.nparts, g.part_w, state_in, init_levels, pos, s32_dst, sb,
                                               sp, nsq);
-    if (launches) ++*launches;
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
+    GLOM_TRY(ln.launched());
   }
   const size_t n4 = (size_t)g.rows * g.d / 4;
   cast_bf16_kernel<<<(int)((n4 + 255) / 256 < sm_count() * 16 ? (n4 + 255) / 256 : sm_count() * 16), 256, 0, st>>>(n4, tokens, xb);
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  return ln.launched();
 }
 
 // S_0 materialisation for the fp32 path / return_all slab 0 (broadcast of init_levels or copy).
@@ -130,15 +125,14 @@ __global__ void init_state_kernel(size_t total4, int L, int d, const float* __re
                                                  : reinterpret_cast<const float4*>(init_levels)[i % ld4];
   }
 }
-cudaError_t launch_broadcast_init(const Geometry& g, const float* state_in, const float* init_levels, float* dst,
-                                  cudaStream_t st, int* launches, Profiler* prof) {
-  ProfScope scope(prof, PROF_PREP, st);
+int launch_broadcast_init(const Geometry& g, const float* state_in, const float* init_levels, float* dst, Launch& ln) {
+  cudaStream_t st = ln.st;
+  ProfScope scope(ln.prof, PROF_PREP, st);
   const size_t total4 = (size_t)g.rows * g.L * g.d / 4;
   const size_t want = (total4 + 255) / 256;
   init_state_kernel<<<(int)(want < sm_count() * 16 ? want : sm_count() * 16), 256, 0, st>>>(total4, g.L, g.d, state_in, init_levels,
                                                                                 dst);
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  return ln.launched();
 }
 
 // =====================================================================================
@@ -345,26 +339,23 @@ __global__ void __launch_bounds__(256) attn_f32_kernel(int n, int L, int d, int 
 }
 
 template <typename OutT>
-static cudaError_t launch_attn_simt(const Geometry& g, const float* s, OutT* c, cudaStream_t st, int* launches) {
+static int launch_attn_simt(const Geometry& g, const float* s, OutT* c, Launch& ln) {
   const size_t smem = (size_t)(AQ * g.d + AQ * g.n) * sizeof(float);
-  if (g.d + g.n > kAttnF32MaxDimPlusN) return cudaErrorInvalidValue;     // forward_impl rejects this shape up front
+  if (g.d + g.n > kAttnF32MaxDimPlusN) return ln.check(cudaErrorInvalidValue);     // forward_impl rejects this shape up front
   static SmemOptIn optin;
-  if (smem > 48 * 1024) {
-    cudaError_t e = optin.ensure(attn_f32_kernel<OutT>, smem);
-    if (e != cudaSuccess) return e;
-  }
+  if (smem > 48 * 1024) GLOM_TRY(ln.check(optin.ensure(attn_f32_kernel<OutT>, smem)));
   dim3 grid((g.n + AQ - 1) / AQ, g.L, g.B);
-  attn_f32_kernel<OutT><<<grid, 256, smem, st>>>(g.n, g.L, g.d, g.attend_self, g.mask_side, g.mask_d2_max, s, c);
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  attn_f32_kernel<OutT><<<grid, 256, smem, ln.st>>>(g.n, g.L, g.d, g.attend_self, g.mask_side, g.mask_d2_max, s, c);
+  return ln.launched();
 }
 
-cudaError_t step_f32(const Geometry& g, const F32Buffers& b, cudaStream_t st, int* launches, Profiler* prof) {
+int step_f32(const Geometry& g, const F32Buffers& b, Launch& ln) {
+  cudaStream_t st = ln.st;
+  Profiler* prof = ln.prof;
   // consensus
   {
     ProfScope scope(prof, PROF_ATTN, st);
-    cudaError_t e = launch_attn_simt<float>(g, b.s_in, b.c, st, launches);
-    if (e != cudaSuccess) return e;
+    GLOM_TRY(launch_attn_simt<float>(g, b.s_in, b.c, ln));
   }
   SgemmParams q{};
   q.d = g.d; q.L = g.L; q.n = g.n; q.G = g.G;
@@ -375,9 +366,7 @@ cudaError_t step_f32(const Geometry& g, const F32Buffers& b, cudaStream_t st, in
     ProfScope scope(prof, PROF_GEMM1, st);
     dim3 grid((q.M + 63) / 64, (q.N + 63) / 64, g.G);
     sgemm_kernel<MODE_FF1><<<grid, 256, 0, st>>>(q);
-    if (launches) ++*launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
+    GLOM_TRY(ln.launched());
   }
   // GEMM2 + combine -> state t+1
   q.N = g.d; q.K = 8 * g.d; q.w = b.w2; q.bias = b.b2; q.out = b.s_out; q.h = b.h; q.c = b.c;
@@ -385,21 +374,20 @@ cudaError_t step_f32(const Geometry& g, const F32Buffers& b, cudaStream_t st, in
     ProfScope scope(prof, PROF_GEMM2, st);
     dim3 grid((q.M + 63) / 64, (q.N + 63) / 64, g.L);
     sgemm_kernel<MODE_FF2><<<grid, 256, 0, st>>>(q);
-    if (launches) ++*launches;
-    return cudaGetLastError();
+    return ln.launched();
   }
 }
 
-cudaError_t launch_tokenize(const float* img, const float* w, const float* bias, float* tokens, int B, int H, int W,
-                            int p, int d, cudaStream_t st, int* launches, Profiler* prof) {
-  ProfScope scope(prof, PROF_TOKENIZE, st);
+int launch_tokenize(const float* img, const float* w, const float* bias, float* tokens, int B, int H, int W, int p, int d,
+                    Launch& ln) {
+  cudaStream_t st = ln.st;
+  ProfScope scope(ln.prof, PROF_TOKENIZE, st);
   SgemmParams q{};
   q.M = B * (H / p) * (W / p); q.N = d; q.K = 3 * p * p;
   q.w = w; q.bias = bias; q.out = tokens; q.img = img; q.Himg = H; q.Wimg = W; q.p = p;
   dim3 grid((q.M + 63) / 64, (q.N + 63) / 64, 1);
   sgemm_kernel<MODE_TOK><<<grid, 256, 0, st>>>(q);
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  return ln.launched();
 }
 
 
@@ -441,13 +429,13 @@ __global__ void patchify_bf16_kernel(const float* __restrict__ img, const float*
   }
 }
 
-cudaError_t launch_patchify_bf16(const float* img, const float* w, __nv_bfloat16* patches, __nv_bfloat16* wtok, int B,
-                                 int H, int W, int p, int d, int kp, cudaStream_t st, int* launches) {
+int launch_patchify_bf16(const float* img, const float* w, __nv_bfloat16* patches, __nv_bfloat16* wtok, int B, int H, int W,
+                         int p, int d, int kp, Launch& ln) {
+  cudaStream_t st = ln.st;
   const size_t total = ((size_t)B * (H / p) * (W / p) + d) * (kp / 2);
   const size_t want = (total + 255) / 256;
   patchify_bf16_kernel<<<(int)(want < sm_count() * 32 ? want : sm_count() * 32), 256, 0, st>>>(img, w, patches, wtok, B, H, W, p, d, kp);
-  if (launches) ++*launches;
-  return cudaGetLastError();
+  return ln.launched();
 }
 
 // ---------------------------------------------------------------- SM clock probe (bench.py's regime record)

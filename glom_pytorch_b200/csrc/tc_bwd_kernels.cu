@@ -446,17 +446,17 @@ bwd_gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // PRE: Xb        
   __syncthreads();
 }
 
-bool map2d_box(EncodeTiledFn enc, CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
-               char* err, size_t errlen, const char* what) {
+// -> 0 or GLOM_B200_ERR_CUDA
+int map2d_box(Launch& ln, CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, const char* what) {
   cuuint64_t gd[2] = {cols, rows};
   cuuint64_t gs[1] = {cols * 2};
   cuuint32_t bx[2] = {(cuuint32_t)BK, box_rows};
   cuuint32_t es[2] = {1, 1};
-  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gd, gs, bx, es,
+  const CUresult r = ln.enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gd, gs, bx, es,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { snprintf(err, errlen, "cuTensorMapEncodeTiled(%s) failed with CUresult %d", what, (int)r); return false; }
-  return true;
+  if (r != CUDA_SUCCESS) return ln.fail(GLOM_B200_ERR_CUDA, "cuTensorMapEncodeTiled(%s) failed with CUresult %d", what, (int)r);
+  return 0;
 }
 
 template <int MODE, bool DET = false>
@@ -478,78 +478,76 @@ cudaError_t launch(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorM
   return cudaLaunchKernelEx(&cfg, bwd_gemm_kernel<MODE, DET>, a0, a1, a2, b0, b1, b2, p);
 }
 
-bool map3d_box(EncodeTiledFn enc, CUtensorMap* m, const void* base, uint64_t inner, uint64_t rows, uint64_t batches,
-               uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows, char* err, size_t errlen,
-               const char* what) {
+int map3d_box(Launch& ln, CUtensorMap* m, const void* base, uint64_t inner, uint64_t rows, uint64_t batches,
+              uint64_t row_stride_elems, uint64_t batch_stride_elems, uint32_t box_rows, const char* what) {
   cuuint64_t gd[3] = {inner, rows, batches};
   cuuint64_t gs[2] = {row_stride_elems * 2, batch_stride_elems * 2};
   cuuint32_t bx[3] = {(cuuint32_t)BK, box_rows, 1};
   cuuint32_t es[3] = {1, 1, 1};
-  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gd, gs, bx, es,
+  const CUresult r = ln.enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gd, gs, bx, es,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { snprintf(err, errlen, "cuTensorMapEncodeTiled(%s) failed with CUresult %d", what, (int)r); return false; }
-  return true;
+  if (r != CUDA_SUCCESS) return ln.fail(GLOM_B200_ERR_CUDA, "cuTensorMapEncodeTiled(%s) failed with CUresult %d", what, (int)r);
+  return 0;
 }
 
 }  // namespace
 
 // Batched C[z] (n x N) (+)= A[z] B[z] on tensor cores for the attention backward (z = image * L + level).
-//   state-like operands: bf16 (B*n, L*d) tensors; attention-like: bf16 (Z, n, n).  a_mn / b_mn: see BwdParams.
-//   a2_src != nullptr: a second product A2[z] B2[z] of the same shape is accumulated into the same tile (its k blocks
+//   state-like operands: bf16 (B*n, L*d) tensors; attention-like: bf16 (Z, n, n).  a.mn / b.mn: see BwdParams.
+//   a2.src != nullptr: a second product A2[z] B2[z] of the same shape is accumulated into the same tile (its k blocks
 //   follow the first product's), so both land in `out` with one read-modify-write.
-int attn_bwd_gemm_tc(const Geometry& g, const void* a_src, int a_state, int a_mn, const void* b_src, int b_state, int b_mn,
-                     int N, int K, int out_kind, float* out, const int32_t* steps, int t, EncodeTiledFn enc, int num_sms,
-                     cudaStream_t st, int* launches, char* err, size_t errlen, const void* a2_src, int a2_state, int a2_mn, const void* b2_src,
-                     int b2_state, int b2_mn) {
+int attn_bwd_gemm_tc(const Geometry& g, AttnBwdOperand a, AttnBwdOperand b, int N, int K, int out_kind, float* out,
+                     const int32_t* steps, int t, Launch& ln, AttnBwdOperand a2, AttnBwdOperand b2) {
   const int n = g.n, L = g.L, d = g.d, Z = g.B * L;
   CUtensorMap ma, mb, ma2, mb2;
-  auto mk = [&](CUtensorMap* m, const void* src, int state, int mn, const char* what) {
-    const uint32_t box_rows = mn ? 64u : (uint32_t)BM;
-    if (state) return map3d_box(enc, m, src, (uint64_t)L * d, n, g.B, (uint64_t)L * d, (uint64_t)n * L * d, box_rows, err, errlen, what);
-    return map3d_box(enc, m, src, n, n, Z, n, (uint64_t)n * n, box_rows, err, errlen, what);
+  auto mk = [&](CUtensorMap* m, const AttnBwdOperand& o, const char* what) {
+    const uint32_t box_rows = o.mn ? 64u : (uint32_t)BM;
+    if (o.state) return map3d_box(ln, m, o.src, (uint64_t)L * d, n, g.B, (uint64_t)L * d, (uint64_t)n * L * d, box_rows, what);
+    return map3d_box(ln, m, o.src, n, n, Z, n, (uint64_t)n * n, box_rows, what);
   };
-  if (!mk(&ma, a_src, a_state, a_mn, "attn-bwd A") || !mk(&mb, b_src, b_state, b_mn, "attn-bwd B")) return -3;
+  GLOM_TRY(mk(&ma, a, "attn-bwd A"));
+  GLOM_TRY(mk(&mb, b, "attn-bwd B"));
   ma2 = ma; mb2 = mb;
-  if (a2_src && (!mk(&ma2, a2_src, a2_state, a2_mn, "attn-bwd A2") || !mk(&mb2, b2_src, b2_state, b2_mn, "attn-bwd B2"))) return -3;
+  if (a2.src) {
+    GLOM_TRY(mk(&ma2, a2, "attn-bwd A2"));
+    GLOM_TRY(mk(&mb2, b2, "attn-bwd B2"));
+  }
   BwdParams p{};
   p.rows = g.rows; p.d = d; p.L = L; p.n = n; p.G = g.G;
-  p.bN = N; p.bK = K; p.a_mn = a_mn; p.b_mn = b_mn; p.a_state = a_state; p.b_state = b_state; p.out_kind = out_kind; p.out = out;
+  p.bN = N; p.bK = K; p.a_mn = a.mn; p.b_mn = b.mn; p.a_state = a.state; p.b_state = b.state; p.out_kind = out_kind; p.out = out;
   p.steps = steps; p.t = t;
-  if (a2_src) { p.k_split = (K + BK - 1) / BK; p.a_mn2 = a2_mn; p.b_mn2 = b2_mn; p.a_state2 = a2_state; p.b_state2 = b2_state; }
+  if (a2.src) { p.k_split = (K + BK - 1) / BK; p.a_mn2 = a2.mn; p.b_mn2 = b2.mn; p.a_state2 = a2.state; p.b_state2 = b2.state; }
   p.num_tiles = Z * ((n + 255) / 256) * ((N + BN - 1) / BN);
-  cudaError_t e = launch<BW_BATCH>(ma, ma2, ma, mb, mb2, mb, p, num_sms, st);
-  if (launches) ++*launches;
-  if (e != cudaSuccess) { snprintf(err, errlen, "attention-backward gemm launch: %s", cudaGetErrorString(e)); return -3; }
-  return 0;
+  return ln.launched(launch<BW_BATCH>(ma, ma2, ma, mb, mb2, mb, p, ln.num_sms, ln.st), "attention-backward gemm launch");
 }
 
 // One reverse step of the MLPs on tensor cores.  Inputs are bf16 shadows prepared by the caller:
 //   xb (R, d), sb (R, L*d), sp (R, (L-1)*d) of S_t ; gsb (R, L*d) = bf16(dL/dS_{t+1} / c)
 //   w1p (G*4d, d), w2t (G*4d, d), w1t (G*d, 4d) bf16 packs of the current weights.
-int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches,
-                    char* err, size_t errlen) {
-  const int d = g.d, L = g.L, rows = g.rows, G = g.G;
-  if (d % 256) { snprintf(err, errlen, "tensor-core backward needs dim %% 256 == 0 (got %d)", d); return -1; }
+int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, Launch& ln) {
+  const int d = g.d, L = g.L, rows = g.rows, G = g.G, num_sms = ln.num_sms;
+  cudaStream_t st = ln.st;
+  if (d % 256) return ln.fail(GLOM_B200_ERR_INVALID, "tensor-core backward needs dim %% 256 == 0 (got %d)", d);
   const int m128 = (rows + 127) / 128;
   const uint64_t blocked_rows = (uint64_t)G * m128 * (4 * d / BK) * BM;
   CUtensorMap mxb, msb, msp, mgs, mw1p, mw2t, mw1t, mdpre128, mdpre64, mh64, mxb64, msb64, msp64, mgs64;
-  bool ok = true;
-  ok &= map2d_box(enc, &mxb, a.xb, rows, d, BM, err, errlen, "Xb");
-  ok &= map2d_box(enc, &msb, a.sb, rows, (uint64_t)L * d, BM, err, errlen, "Sb");
-  ok &= map2d_box(enc, &msp, a.sp, rows, (uint64_t)(L - 1) * d, BM, err, errlen, "Sp");
-  ok &= map2d_box(enc, &mgs, a.gsb, rows, (uint64_t)L * d, BM, err, errlen, "gsb");
-  ok &= map2d_box(enc, &mw1p, a.w1p, (uint64_t)G * 4 * d, d, BN / 2, err, errlen, "W1p");
-  ok &= map2d_box(enc, &mw2t, a.w2t, (uint64_t)G * 4 * d, d, BN / 2, err, errlen, "W2T");
-  ok &= map2d_box(enc, &mw1t, a.w1t, (uint64_t)G * d, (uint64_t)4 * d, BN / 2, err, errlen, "W1T");
-  ok &= map2d_box(enc, &mdpre128, a.dpre, blocked_rows, BK, BM, err, errlen, "dpre");
-  ok &= map2d_box(enc, &mdpre64, a.dpre, blocked_rows, BK, 64, err, errlen, "dpre64");
-  ok &= map2d_box(enc, &mh64, a.h, blocked_rows, BK, 64, err, errlen, "h64");
-  ok &= map2d_box(enc, &mxb64, a.xb, rows, d, 64, err, errlen, "Xb64");
-  ok &= map2d_box(enc, &msb64, a.sb, rows, (uint64_t)L * d, 64, err, errlen, "Sb64");
-  ok &= map2d_box(enc, &msp64, a.sp, rows, (uint64_t)(L - 1) * d, 64, err, errlen, "Sp64");
-  ok &= map2d_box(enc, &mgs64, a.gsb, rows, (uint64_t)L * d, 64, err, errlen, "gsb64");
-  if (!ok) return -3;
+  int bad = 0;                  // every map is attempted; the message is the last failure's
+  bad |= map2d_box(ln, &mxb, a.xb, rows, d, BM, "Xb");
+  bad |= map2d_box(ln, &msb, a.sb, rows, (uint64_t)L * d, BM, "Sb");
+  bad |= map2d_box(ln, &msp, a.sp, rows, (uint64_t)(L - 1) * d, BM, "Sp");
+  bad |= map2d_box(ln, &mgs, a.gsb, rows, (uint64_t)L * d, BM, "gsb");
+  bad |= map2d_box(ln, &mw1p, a.w1p, (uint64_t)G * 4 * d, d, BN / 2, "W1p");
+  bad |= map2d_box(ln, &mw2t, a.w2t, (uint64_t)G * 4 * d, d, BN / 2, "W2T");
+  bad |= map2d_box(ln, &mw1t, a.w1t, (uint64_t)G * d, (uint64_t)4 * d, BN / 2, "W1T");
+  bad |= map2d_box(ln, &mdpre128, a.dpre, blocked_rows, BK, BM, "dpre");
+  bad |= map2d_box(ln, &mdpre64, a.dpre, blocked_rows, BK, 64, "dpre64");
+  bad |= map2d_box(ln, &mh64, a.h, blocked_rows, BK, 64, "h64");
+  bad |= map2d_box(ln, &mxb64, a.xb, rows, d, 64, "Xb64");
+  bad |= map2d_box(ln, &msb64, a.sb, rows, (uint64_t)L * d, 64, "Sb64");
+  bad |= map2d_box(ln, &msp64, a.sp, rows, (uint64_t)(L - 1) * d, 64, "Sp64");
+  bad |= map2d_box(ln, &mgs64, a.gsb, rows, (uint64_t)L * d, 64, "gsb64");
+  if (bad) return bad;
   BwdParams p{};
   p.rows = rows; p.d = d; p.L = L; p.n = g.n; p.G = G; p.m128 = m128;
   p.b1p = a.b1p; p.pre = a.pre; p.h = a.h; p.dpre = a.dpre; p.ds = a.ds; p.d_tokens = a.d_tokens; p.d_pos = a.d_pos;
@@ -561,25 +559,18 @@ int mlp_backward_tc(const Geometry& g, const MlpBwdTc& a, EncodeTiledFn enc, int
   cudaError_t e;
   p.num_tiles = G * nm * (4 * d / BN);
   if (!a.skip_pre) {
-    e = launch<BW_PRE>(mxb, msb, msp, mw1p, mw1p, mw1p, p, num_sms, st);
-    if (launches) ++*launches;
-    if (e != cudaSuccess) { snprintf(err, errlen, "bwd pre launch: %s", cudaGetErrorString(e)); return -3; }
+    GLOM_TRY(ln.launched(launch<BW_PRE>(mxb, msb, msp, mw1p, mw1p, mw1p, p, num_sms, st), "bwd pre launch"));
   }
   e = a.deterministic ? launch<BW_DH, true>(mgs, mgs, mgs, mw2t, mw2t, mw2t, p, num_sms, st)
                       : launch<BW_DH>(mgs, mgs, mgs, mw2t, mw2t, mw2t, p, num_sms, st);
-  if (launches) ++*launches;
-  if (e != cudaSuccess) { snprintf(err, errlen, "bwd dh launch: %s", cudaGetErrorString(e)); return -3; }
+  GLOM_TRY(ln.launched(e, "bwd dh launch"));
   p.num_tiles = G * nm * (d / BN);
   e = a.deterministic ? launch<BW_DX, true>(mdpre128, mdpre128, mdpre128, mw1t, mw1t, mw1t, p, num_sms, st)
                       : launch<BW_DX>(mdpre128, mdpre128, mdpre128, mw1t, mw1t, mw1t, p, num_sms, st);
-  if (launches) ++*launches;
-  if (e != cudaSuccess) { snprintf(err, errlen, "bwd dx launch: %s", cudaGetErrorString(e)); return -3; }
+  GLOM_TRY(ln.launched(e, "bwd dx launch"));
   if (a.skip_dw) return 0;
   p.num_tiles = G * 2 * (d / 256) * (4 * d / BN);
-  e = launch<BW_DW>(mgs64, mdpre64, mh64, mxb64, msb64, msp64, p, num_sms, st);
-  if (launches) ++*launches;
-  if (e != cudaSuccess) { snprintf(err, errlen, "bwd dw launch: %s", cudaGetErrorString(e)); return -3; }
-  return 0;
+  return ln.launched(launch<BW_DW>(mgs64, mdpre64, mh64, mxb64, msb64, msp64, p, num_sms, st), "bwd dw launch");
 }
 
 }  // namespace glom

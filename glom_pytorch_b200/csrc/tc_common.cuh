@@ -158,28 +158,25 @@ __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b
   __syncwarp();
 }
 
-static inline bool encode_map(EncodeTiledFn enc, CUtensorMap* m, const void* base, int rank, const uint64_t* dims,
-                       const uint64_t* strides_bytes /* rank-1 */, const uint32_t* box, char* err, size_t errlen,
-                       const char* what) {
+// -> 0 or GLOM_B200_ERR_CUDA
+static inline int encode_map(Launch& ln, CUtensorMap* m, const void* base, int rank, const uint64_t* dims,
+                             const uint64_t* strides_bytes /* rank-1 */, const uint32_t* box, const char* what) {
   cuuint64_t gd[3]; cuuint64_t gs[2]; cuuint32_t bx[3]; cuuint32_t es[3] = {1, 1, 1};
   for (int i = 0; i < rank; ++i) { gd[i] = dims[i]; bx[i] = box[i]; }
   for (int i = 0; i < rank - 1; ++i) gs[i] = strides_bytes[i];
-  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
+  const CUresult r = ln.enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    snprintf(err, errlen, "cuTensorMapEncodeTiled(%s) failed with CUresult %d", what, (int)r);
-    return false;
-  }
-  return true;
+  if (r != CUDA_SUCCESS) return ln.fail(GLOM_B200_ERR_CUDA, "cuTensorMapEncodeTiled(%s) failed with CUresult %d", what, (int)r);
+  return 0;
 }
 
-static inline bool map2d(EncodeTiledFn enc, CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
-                  char* err, size_t errlen, const char* what) {
+static inline int map2d(Launch& ln, CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
+                        const char* what) {
   const uint64_t dims[2] = {cols, rows};
   const uint64_t strides[1] = {cols * 2};
   const uint32_t box[2] = {(uint32_t)BK, box_rows};
-  return encode_map(enc, m, base, 2, dims, strides, box, err, errlen, what);
+  return encode_map(ln, m, base, 2, dims, strides, box, what);
 }
 
 }  // namespace glom

@@ -927,6 +927,12 @@ template <int MODE, int BN, bool CNT, bool SETTLE = false>
 static cudaError_t launch_gemm_impl(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& bm,
                                     const CUtensorMap& out, const GemmParams& p, int num_sms, cudaStream_t st);
 
+// GLOM_B200_WAIT_COUNTERS=1 (diagnostics): the kernel instantiations whose block 0 accumulates its roles' wait cycles
+static bool count_waits() {
+  static const bool on = [] { const char* ev = getenv("GLOM_B200_WAIT_COUNTERS"); return ev && ev[0] == '1'; }();
+  return on;
+}
+
 template <int MODE, int BN>
 static cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& a2, const CUtensorMap& bm,
                                const CUtensorMap& out, const GemmParams& p, int num_sms, cudaStream_t st) {
@@ -934,10 +940,7 @@ static cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, con
   if constexpr (MODE != 2) {
     if (p.block_frozen) return launch_gemm_impl<MODE, BN, false, true>(a0, a1, a2, bm, out, p, num_sms, st);
   }
-  // GLOM_B200_WAIT_COUNTERS=1 (diagnostics): the instantiation whose block 0 accumulates its roles' wait cycles
-  static int count_waits = -1;
-  if (count_waits < 0) { const char* ev = getenv("GLOM_B200_WAIT_COUNTERS"); count_waits = (ev && ev[0] == '1') ? 1 : 0; }
-  if (count_waits) return launch_gemm_impl<MODE, BN, true>(a0, a1, a2, bm, out, p, num_sms, st);
+  if (count_waits()) return launch_gemm_impl<MODE, BN, true>(a0, a1, a2, bm, out, p, num_sms, st);
   return launch_gemm_impl<MODE, BN, false>(a0, a1, a2, bm, out, p, num_sms, st);
 }
 
@@ -995,16 +998,13 @@ static cudaError_t launch_attn_impl(const CUtensorMap& mq, const CUtensorMap& mk
 }
 
 // K3: consensus attention -> C
-static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiledFn enc, int num_sms, cudaStream_t st,
-                            int* launches, char* err, size_t errlen, Profiler* prof) {
+static int launch_attention(const Geometry& g, const Bf16Buffers& b, Launch& ln) {
   const int d = g.d, L = g.L, n = g.n;
   // Up to 576 columns the probabilities of a 128-query tile against all keys fit in shared memory: one launch.  Beyond,
   // the keys are processed in passes of ATTN_PASS_KEYS (one launch each, see AttnParams): no shape falls to CUDA cores.
   const int npass = (n <= ATTN_SINGLE_PASS_MAX) ? 1 : (n + ATTN_PASS_KEYS - 1) / ATTN_PASS_KEYS;
-  if (npass > 1 && !b.attn_acc) {
-    snprintf(err, errlen, "consensus for n = %d columns needs the key-pass scratch buffer (workspace too old?)", n);
-    return -3;
-  }
+  if (npass > 1 && !b.attn_acc)
+    return ln.fail(GLOM_B200_ERR_CUDA, "consensus for n = %d columns needs the key-pass scratch buffer (workspace too old?)", n);
   // All keys of a single pass of more than 128 and at most 256 (padded) keys form one 256-key S block; every other
   // pass uses 128-key blocks
   const int keys = (npass == 1 && (n + 15) / 16 * 16 > 128 && (n + 15) / 16 * 16 <= 256) ? 256 : 128;
@@ -1013,11 +1013,11 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiled
   const uint64_t strides[2] = {(uint64_t)L * d * 2, (uint64_t)n * L * d * 2};
   const uint32_t boxq[3] = {(uint32_t)BK, (uint32_t)BM, 1}, boxk[3] = {(uint32_t)BK, (uint32_t)keys, 1};
   const uint32_t boxv[3] = {(uint32_t)BK, 64, 1};
-  if (!encode_map(enc, &mq, b.sb_in, 3, dims, strides, boxq, err, errlen, "attn.q")) return -3;
-  if (!encode_map(enc, &mk, b.sb_in, 3, dims, strides, boxk, err, errlen, "attn.k")) return -3;
-  if (!encode_map(enc, &mv, b.sb_in, 3, dims, strides, boxv, err, errlen, "attn.v")) return -3;
-  static int count_waits = -1;
-  if (count_waits < 0) { const char* ev = getenv("GLOM_B200_WAIT_COUNTERS"); count_waits = (ev && ev[0] == '1') ? 1 : 0; }
+  GLOM_TRY(encode_map(ln, &mq, b.sb_in, 3, dims, strides, boxq, "attn.q"));
+  GLOM_TRY(encode_map(ln, &mk, b.sb_in, 3, dims, strides, boxk, "attn.k"));
+  GLOM_TRY(encode_map(ln, &mv, b.sb_in, 3, dims, strides, boxv, "attn.v"));
+  const bool cnt = count_waits();
+  cudaStream_t st = ln.st;
   for (int pass = 0; pass < npass; ++pass) {
     AttnParams ap{};
     ap.n = n; ap.L = L; ap.d = d;
@@ -1045,44 +1045,41 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, EncodeTiled
     int stages = 4;
     while (stages > 0 && fixed + (size_t)stages * slot > max_smem) --stages;
     // the consumers release a slot only after the next one's MMAs are issued: the ring needs two slots
-    if (stages < 2 || ap.nkb > (keys == 256 ? AttnCfg<256>::MAX_KB : AttnCfg<128>::MAX_KB)) {
-      snprintf(err, errlen, "consensus pass of %d keys does not fit shared memory", ap.nk);
-      return -3;
-    }
+    if (stages < 2 || ap.nkb > (keys == 256 ? AttnCfg<256>::MAX_KB : AttnCfg<128>::MAX_KB))
+      return ln.fail(GLOM_B200_ERR_CUDA, "consensus pass of %d keys does not fit shared memory", ap.nk);
     ap.num_stages = stages;
     const size_t smem = fixed + (size_t)stages * slot;
-    const int ctas = ap.num_items < num_sms ? ap.num_items : num_sms;
-    ProfScope scope(prof, PROF_ATTN, st);
+    const int ctas = ap.num_items < ln.num_sms ? ap.num_items : ln.num_sms;
+    ProfScope scope(ln.prof, PROF_ATTN, st);
     cudaError_t e;
     if (b.frozen) e = keys == 256 ? launch_attn_impl<256, false, true>(mq, mk, mv, ap, smem, ctas, st)
                                   : launch_attn_impl<128, false, true>(mq, mk, mv, ap, smem, ctas, st);
-    else if (keys == 256) e = count_waits ? launch_attn_impl<256, true>(mq, mk, mv, ap, smem, ctas, st)
+    else if (keys == 256) e = cnt ? launch_attn_impl<256, true>(mq, mk, mv, ap, smem, ctas, st)
                                           : launch_attn_impl<256, false>(mq, mk, mv, ap, smem, ctas, st);
-    else e = count_waits ? launch_attn_impl<128, true>(mq, mk, mv, ap, smem, ctas, st)
+    else e = cnt ? launch_attn_impl<128, true>(mq, mk, mv, ap, smem, ctas, st)
                          : launch_attn_impl<128, false>(mq, mk, mv, ap, smem, ctas, st);
-    if (launches) ++*launches;
-    if (e != cudaSuccess) { snprintf(err, errlen, "attn_kernel launch: %s", cudaGetErrorString(e)); return -3; }
+    GLOM_TRY(ln.launched(e, "attn_kernel launch"));
   }
   return 0;
 }
 
-int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTiledFn enc, int num_sms, cudaStream_t st,
-              int* launches, char* err, size_t errlen, Profiler* prof) {
-  const int d = g.d, L = g.L, n = g.n, rows = g.rows;
+int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, Launch& ln) {
+  const int d = g.d, L = g.L, n = g.n, rows = g.rows, num_sms = ln.num_sms;
+  cudaStream_t st = ln.st;
   // One launch each of K1 (all groups), K3, K2 (all levels).
   // H: (group, 128-row block, 64-column k block) blocks of 128 x 64, read by K2 a block at a time (mh) and written by
   // K1 a warpgroup's 64 rows at a time (mh_out)
   CUtensorMap mh, mh_out;
   const int m128 = (rows + BM - 1) / BM;
   const uint64_t h_rows = (uint64_t)g.G * m128 * (4 * d / BK) * BM;
-  if (!map2d(enc, &mh, b.h, h_rows, BK, BM, err, errlen, "H")) return -3;
-  if (!map2d(enc, &mh_out, b.h, h_rows, BK, 64, err, errlen, "H out")) return -3;
+  GLOM_TRY(map2d(ln, &mh, b.h, h_rows, BK, BM, "H"));
+  GLOM_TRY(map2d(ln, &mh_out, b.h, h_rows, BK, 64, "H out"));
   CUtensorMap mx, msb, msp, mw1, mw2;
-  if (!map2d(enc, &mx, b.xb, rows, d, BM, err, errlen, "Xb")) return -3;
-  if (!map2d(enc, &msb, b.sb_in, rows, (uint64_t)L * d, BM, err, errlen, "Sb")) return -3;
-  if (!map2d(enc, &msp, b.sp_in, rows, (uint64_t)(L - 1) * d, BM, err, errlen, "Sp")) return -3;
-  if (!map2d(enc, &mw1, b.w1, (uint64_t)g.G * 4 * d, d, 128, err, errlen, "W1p")) return -3;
-  if (!map2d(enc, &mw2, b.w2, (uint64_t)L * d, (uint64_t)8 * d, (uint32_t)g.bn2 / 2, err, errlen, "W2p")) return -3;
+  GLOM_TRY(map2d(ln, &mx, b.xb, rows, d, BM, "Xb"));
+  GLOM_TRY(map2d(ln, &msb, b.sb_in, rows, (uint64_t)L * d, BM, "Sb"));
+  GLOM_TRY(map2d(ln, &msp, b.sp_in, rows, (uint64_t)(L - 1) * d, BM, "Sp"));
+  GLOM_TRY(map2d(ln, &mw1, b.w1, (uint64_t)g.G * 4 * d, d, 128, "W1p"));
+  GLOM_TRY(map2d(ln, &mw2, b.w2, (uint64_t)L * d, (uint64_t)8 * d, (uint32_t)g.bn2 / 2, "W2p"));
   // ---------------- K1: grouped GEMM1 + bias + GELU -> H   (all 2L-1 groups)
   {
     GemmParams p{};
@@ -1097,13 +1094,11 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTil
     p.num_m = (rows + 255) / 256; p.num_n = 4 * d / 256; p.num_tiles = (g.G - p.z0) * p.num_m * p.num_n;
     p.bias = b.b1; p.m128 = m128;
     p.frozen = b.frozen; p.block_frozen = b.block_frozen; p.block_fresh = b.block_fresh;
-    ProfScope scope(prof, PROF_GEMM1, st);
-    cudaError_t e = launch_gemm<0, 256>(mx, msb, msp, mw1, mh_out, p, num_sms, st);
-    if (launches) ++*launches;
-    if (e != cudaSuccess) { snprintf(err, errlen, "gemm1 launch: %s", cudaGetErrorString(e)); return -3; }
+    ProfScope scope(ln.prof, PROF_GEMM1, st);
+    GLOM_TRY(ln.launched(launch_gemm<0, 256>(mx, msb, msp, mw1, mh_out, p, num_sms, st), "gemm1 launch"));
   }
   // ---------------- K3 between K1 and K2 (C is then written shortly before K2's epilogue reads it)
-  if (int rc = launch_attention(g, b, enc, num_sms, st, launches, err, errlen, prof)) return rc;
+  GLOM_TRY(launch_attention(g, b, ln));
   // ---------------- K2: grouped GEMM2 + combine -> state t+1 (+ shadows, norms)   (all levels)
   {
     GemmParams p{};
@@ -1115,12 +1110,11 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTil
     p.s32_out = b.s32_out; p.sb_out = b.sb_out; p.sp_out = b.sp_out; p.nsq_out = b.nsq_out; p.nparts = g.nparts;
     p.frozen = b.frozen; p.block_frozen = b.block_frozen; p.dsq_out = b.dsq_out;
     cudaError_t e;
-    ProfScope scope(prof, PROF_GEMM2, st);
+    ProfScope scope(ln.prof, PROF_GEMM2, st);
     if (g.bn2 == 256) e = launch_gemm<1, 256>(mh, mh, mh, mw2, mh, p, num_sms, st);
     else if (g.bn2 == 128) e = launch_gemm<1, 128>(mh, mh, mh, mw2, mh, p, num_sms, st);
     else e = launch_gemm<1, 64>(mh, mh, mh, mw2, mh, p, num_sms, st);
-    if (launches) ++*launches;
-    if (e != cudaSuccess) { snprintf(err, errlen, "gemm2 launch: %s", cudaGetErrorString(e)); return -3; }
+    GLOM_TRY(ln.launched(e, "gemm2 launch"));
   }
   return 0;
 }
@@ -1128,11 +1122,13 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, EncodeTil
 
 // ---------------- tensor-core tokeniser: tokens = patches(bf16) . Wtok(bf16)^T + bias   (glom_pytorch.py:94-97)
 int tokenize_tc(const __nv_bfloat16* patches, const __nv_bfloat16* wtok, const float* bias, float* tokens, int rows,
-                int d, int kp, EncodeTiledFn enc, int num_sms, cudaStream_t st, int* launches, char* err, size_t errlen) {
+                int d, int kp, Launch& ln) {
+  const int num_sms = ln.num_sms;
+  cudaStream_t st = ln.st;
   const int bn = (d % 256 == 0) ? 256 : (d % 128 == 0) ? 128 : 64;
   CUtensorMap ma, mb;
-  if (!map2d(enc, &ma, patches, rows, kp, BM, err, errlen, "patches")) return -3;
-  if (!map2d(enc, &mb, wtok, d, kp, (uint32_t)bn / 2, err, errlen, "Wtok")) return -3;
+  GLOM_TRY(map2d(ln, &ma, patches, rows, kp, BM, "patches"));
+  GLOM_TRY(map2d(ln, &mb, wtok, d, kp, (uint32_t)bn / 2, "Wtok"));
   GemmParams p{};
   p.rows = rows; p.d = d; p.L = 1; p.n = 1; p.G = 1;
   p.num_m = (rows + 255) / 256; p.num_n = d / bn; p.num_tiles = p.num_m * p.num_n;
@@ -1141,9 +1137,7 @@ int tokenize_tc(const __nv_bfloat16* patches, const __nv_bfloat16* wtok, const f
   if (bn == 256) e = launch_gemm<2, 256>(ma, ma, ma, mb, ma, p, num_sms, st);
   else if (bn == 128) e = launch_gemm<2, 128>(ma, ma, ma, mb, ma, p, num_sms, st);
   else e = launch_gemm<2, 64>(ma, ma, ma, mb, ma, p, num_sms, st);
-  if (launches) ++*launches;
-  if (e != cudaSuccess) { snprintf(err, errlen, "tokeniser gemm launch: %s", cudaGetErrorString(e)); return -3; }
-  return 0;
+  return ln.launched(e, "tokeniser gemm launch");
 }
 
 }  // namespace glom
