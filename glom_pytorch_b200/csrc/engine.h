@@ -137,7 +137,19 @@ struct Bf16Buffers {
   // Glom.settle_queue only (NULL otherwise): [ceil(rows / 256)] 1 = the block holds a slot admitted at this step; K1 then
   // runs MLP group 0 at every step, for these blocks only
   const int* block_fresh;
+  // 1: a forward from init_levels at a step t < L (DESIGN.md, "Image-independent levels"): the work whose inputs are the
+  // same in every image runs for the representative rows only
+  int ii_reduce;
 };
+
+// The representative rows of image-independent work: the first lcm(n, 128) rows, whole images and whole 128-row H blocks,
+// so 128-row block k holds the patches of block k % rep_h_blocks(n).  rep_row_blocks: the 256-row GEMM blocks covering them
+static inline int rep_h_blocks(int n) {
+  int a = n, b = 128;
+  while (b) { const int r = a % b; a = b; b = r; }
+  return n / a;
+}
+static inline int rep_row_blocks(int n) { return (rep_h_blocks(n) * 128 + 255) / 256; }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -210,6 +222,9 @@ int launch_settle_gather(const Geometry& g, int max_iters, const int32_t* steps,
 int launch_steps_schedule(const Geometry& g, int t, int max_steps, const int32_t* steps, int* frozen, int* block_frozen,
                           Launch& ln);
 int launch_steps_fill(const Geometry& g, int max_steps, const int32_t* steps, float* states, Launch& ln);
+// return_all of a forward whose steps 0 .. L-2 ran image-independent levels for the representative rows only: level l >= s
+// of slab s (1 <= s <= L-1) is copied from row r mod n into every row r >= n
+int launch_level_fill(const Geometry& g, float* states, Launch& ln);
 
 // fp32 consensus (attn_f32_kernel): a block of 16 queries keeps their rows (16 x dim) and logits (16 x n) as fp32 in
 // shared memory, within the 227 KB a block may opt in to: dim + n <= 3632

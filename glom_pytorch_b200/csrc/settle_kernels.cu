@@ -193,6 +193,23 @@ int launch_steps_fill(const Geometry& g, int max_steps, const int32_t* steps, fl
   return ln.launched();
 }
 
+// Grid (chunks, B - 1): slab s of a return_all forward from init_levels holds levels l >= s for image 0 only (steps
+// 0 .. L-2 ran them for the representative rows, see step_bf16); image b >= 1 receives image 0's rows of those levels.
+__global__ void level_fill_kernel(int L, int d4, size_t per_img4, size_t slab4, float4* __restrict__ states) {
+  const size_t o = (size_t)(blockIdx.y + 1) * per_img4;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < per_img4; i += (size_t)gridDim.x * blockDim.x) {
+    const int l = (int)(i / d4 % L);
+    for (int s = 1; s <= l; ++s) states[(size_t)s * slab4 + o + i] = states[(size_t)s * slab4 + i];
+  }
+}
+
+int launch_level_fill(const Geometry& g, float* states, Launch& ln) {
+  const size_t per_img4 = (size_t)g.n * g.L * g.d / 4;
+  level_fill_kernel<<<dim3(copy_chunks(g, per_img4), g.B - 1), 256, 0, ln.st>>>(g.L, g.d / 4, per_img4, per_img4 * g.B,
+                                                                               reinterpret_cast<float4*>(states));
+  return ln.launched();
+}
+
 // ---- Glom.settle_queue: N images through B slots.  Slot s holds image slot_img[s]; its rows are rows s*n .. s*n+n-1
 // of every step buffer, exactly as image s's rows in a settle call of batch B.  S_t of the slots lives in the private
 // slab t & 1, the shadows and norm partials in buffer t & 1, as in settle.  A slot whose image stops after step t-1 hands

@@ -81,6 +81,7 @@ struct K2Chunk {
   int l, L, d, n, row0;
   int prow0;            // row0 % n: patch index of the band's first row (position table row), computed once per tile
   int s_bcast;          // 1: s32_in is init_levels (L, d), the same for every row (first step of a call without carried state)
+  bool remap;           // 1: row r of s32_in and c_in is read from row r mod n (only the representative rows hold them)
   const float* s32_in; const __nv_bfloat16* c_in; const float* pos;
   float* s32_out; __nv_bfloat16* sb_out; __nv_bfloat16* sp_out;
 };
@@ -114,9 +115,15 @@ __device__ __forceinline__ void k2_chunk(const uint32_t (&v)[32], const float4 b
       const int r = (h * 4 + j) * 4 + rsub;
       sv[j] = make_float4(0.f, 0.f, 0.f, 0.f); pp[j] = sv[j]; cw[j] = make_uint2(0u, 0u);
       if ((FULL || r < rows_left) && (!SETTLE || ((live >> r) & 1u))) {
+        size_t so = base + (unsigned)(r * ld);
+        if (!SETTLE && k.remap) {
+          int sr = k.prow0 + r;                       // (row0 + r) % n
+          if (k.n >= 32) { if (sr >= k.n) sr -= k.n; } else sr %= k.n;
+          so = (size_t)k.l * k.d + col + c * 4 + (unsigned)(sr * ld);
+        }
         sv[j] = k.s_bcast ? __ldg(reinterpret_cast<const float4*>(k.s32_in + (size_t)k.l * k.d + col + c * 4))
-                          : __ldcs(reinterpret_cast<const float4*>(k.s32_in + base + (unsigned)(r * ld)));
-        cw[j] = __ldcs(reinterpret_cast<const uint2*>(k.c_in + base + (unsigned)(r * ld)));
+                          : __ldcs(reinterpret_cast<const float4*>(k.s32_in + so));
+        cw[j] = __ldcs(reinterpret_cast<const uint2*>(k.c_in + so));
         if (has_td) {
           int pr = k.prow0 + r;                       // (row0 + r) % n without a division per row (r < 32)
           if (k.n >= 32) { if (pr >= k.n) pr -= k.n; } else pr %= k.n;

@@ -108,6 +108,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
             const GemmParams p) {
   using Cfg = GemmCfg<MODE, BN>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr bool RED = MODE != 2 && !SETTLE;     // honours GemmParams::num_m_rep (image-independent work)
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment (128-byte swizzle atoms) by pointer arithmetic on the __shared__ array (keeps the shared address
   // space visible to the compiler: LDS/STS instead of generic LD/ST for every staging / patch access)
@@ -160,7 +161,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
       const int kbg_n = 4 * p.d / BK;
       const int blk_skip = (p.m128 - 1) * kbg_n;
       for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
-        const TileInfo t = decode_tile<MODE>(p, tile);
+        const TileInfo t = decode_tile<MODE, RED>(p, tile);
         if constexpr (SETTLE) { if (settle_skip<MODE>(p, t)) continue; }
         const CUtensorMap* amap;
         int a_col, b_row;
@@ -181,6 +182,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
         // K2: block (group g, 128-row block, 64-wide k block); [H_bu,l | H_td,l] are groups 2l and 2l+1, so k block kb
         // of the concatenation is block blk0 + kb of group 2l and, from kb = kbg_n on, of the group behind it
         const int blk0 = (2 * t.z * p.m128 + (a_row >> 7)) * kbg_n;
+        int td_skip = blk_skip;
+        if constexpr (RED && MODE == 1) {
+          // the top-down group's H was computed for the representative blocks only: read block k mod h_period instead
+          if (p.num_m_rep > 0 && t.z + 1 >= p.remap_l) td_skip -= ((a_row >> 7) - (a_row >> 7) % p.h_period) * kbg_n;
+        }
         for (int kb = 0; kb < t.num_kb; ++kb) {
           GLOM_CNT_WAIT(w0, mbar_wait(&empty_bar[stage], phase ^ 1));
           if (elected) {
@@ -188,7 +194,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
             uint64_t* bar = &full_bar[stage];
             mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
             if (MODE == 1) {
-              const int blk = blk0 + kb + (kb >= kbg_n ? blk_skip : 0);
+              const int blk = blk0 + kb + (kb >= kbg_n ? td_skip : 0);
               // H streams through once per pair of column tiles: evict-first keeps it from displacing weights / state
               tma_load_2d_hint(sa, amap, bar, 0, blk * BM, pol_first);
             } else {
@@ -229,17 +235,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
     int stage = 0; uint32_t phase = 0;
     float acc[BN / 2];
     for (int it = 0, tile; (tile = sched_tile<MODE>(p, cluster_id, num_clusters, it)) >= 0; ++it) {
-      const TileInfo t = decode_tile<MODE>(p, tile);
+      const TileInfo t = decode_tile<MODE, RED>(p, tile);
       if constexpr (SETTLE) { if (settle_skip<MODE>(p, t)) continue; }
       const int row0 = t.m_blk * 256 + cta_rank * BM + pair * 32;     // first row of this warp pair's 32-row band
       const int rows_left = p.rows - row0;                              // >= 32: whole band valid (warp-uniform)
       uint32_t live = ~0u;                                              // SETTLE, K2: bit r = row row0 + r is stored
       if constexpr (SETTLE && MODE == 1)
         live = __ballot_sync(0xffffffffu, row0 + lane < p.rows && !p.frozen[(row0 + lane) / p.n]);
+      // RED, K2: this level's S_t and C hold the representative rows only; row r reads row r mod n (k2_chunk)
+      bool remap = false;
+      if constexpr (RED && MODE == 1) remap = p.num_m_rep > 0 && t.z >= p.remap_l;
       if (MODE == 1 && lane < rows_left) {
         // The combine reads this band's fp32 state and C lines: pull them into L2 before the main loop, so the epilogue's
         // dependent global loads hit L2 instead of paying the HBM latency
-        const size_t o = ((size_t)(row0 + lane) * p.L + t.z) * p.d + t.n_blk * BN + x * (BN / 2);
+        const int src_row = remap ? (row0 + lane) % p.n : row0 + lane;
+        const size_t o = ((size_t)src_row * p.L + t.z) * p.d + t.n_blk * BN + x * (BN / 2);
 #pragma unroll
         for (int c = 0; c < BN / 2; c += 32) {
           if (!p.s_bcast) prefetch_l2(p.s32_in + o + c);
@@ -324,6 +334,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0,   // K1: tokens Xb (rows
           } else {
             K2Chunk kc;
             kc.l = t.z; kc.L = p.L; kc.d = p.d; kc.n = p.n; kc.row0 = row0; kc.prow0 = row0 % p.n; kc.s_bcast = p.s_bcast;
+            kc.remap = remap;
             kc.s32_in = p.s32_in; kc.c_in = p.c_in; kc.pos = p.pos;
             kc.s32_out = p.s32_out; kc.sb_out = p.sb_out; kc.sp_out = p.sp_out;
             const int col = t.n_blk * BN + cc;
@@ -444,6 +455,10 @@ struct AttnParams {
   float* o_acc;                        // (rows, L, d) fp32
   float* ml_acc;                       // (rows, L, 2) fp32: stabiliser (log2 units), row sum
   const int* frozen;                   // SETTLE: [B] 1 = the image has stopped, its items are skipped
+  // Levels [0, l_full) are items of every image, image-major; levels [l_full, L) follow for image 0 only: their state is
+  // the same in every image (a forward from init_levels, DESIGN.md "Image-independent levels").  L: every item.  The
+  // SETTLE instantiations ignore it (l_full = L)
+  int l_full;
 };
 
 // shared-memory bytes of a pass: P (nchunk x [128 x 64] bf16), the ring, two scale buffers (rs, bnd) + key coordinates,
@@ -499,7 +514,13 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
   constexpr int W_TMA = 0;
   constexpr int W_CONSUMER0 = 4;
   const int nsub = (p.d + 255) / 256;                  // O slices per item
-  const int per_img = p.ntiles * p.L;
+  const int per_img = p.ntiles * (SETTLE ? p.L : p.l_full);
+  const int full_items = p.num_items - p.ntiles * (p.L - p.l_full);
+  // item -> (image, level): image 0's image-independent levels after the items of every image
+  auto item_bl = [&](int it, int& b, int& l) {
+    if (SETTLE) { b = it / per_img; l = (it % per_img) / p.ntiles; }
+    else attn_item(it, full_items, per_img, p.ntiles, p.l_full, b, l);
+  };
   const int nkb = (KEYS == 256) ? 1 : p.nkb;           // compile-time single key block on the 256-key path
   constexpr float LOG2E = 1.4426950408889634f;
 
@@ -531,7 +552,8 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
       int stage = 0; uint32_t phase = 0;
       const uint32_t stages0 = smem_u32(stages);
       for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
-        const int b = it / per_img, l = (it % per_img) / p.ntiles;
+        int b, l;
+        item_bl(it, b, l);
         if constexpr (SETTLE) { if (p.frozen[b]) continue; }
         const int q0 = (it % p.ntiles) * BM;
         for (int kb = 0; kb < nkb; ++kb) {
@@ -577,7 +599,8 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
                               : use_mask ? ((uint32_t)((p.key0 + j) / p.mask_side) << 16) | (uint32_t)((p.key0 + j) % p.mask_side) : 0u;
       int k = 0;
       for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
-        const int b = it / per_img, l = (it % per_img) / p.ntiles;
+        int b, l;
+        item_bl(it, b, l);
         if constexpr (SETTLE) { if (p.frozen[b]) continue; }
         const size_t img_row0 = (size_t)b * p.n;
         const int buf = k & 1;
@@ -634,7 +657,8 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q,    // (L*d, n, B) box (64
 
     int k = 0;
     for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
-      const int b = it / per_img, l = (it % per_img) / p.ntiles;
+      int b, l;
+      item_bl(it, b, l);
       if constexpr (SETTLE) { if (p.frozen[b]) continue; }
       const int q0 = (it % p.ntiles) * BM;
       const size_t img_row0 = (size_t)b * p.n;
@@ -997,8 +1021,8 @@ static cudaError_t launch_attn_impl(const CUtensorMap& mq, const CUtensorMap& mk
   return cudaLaunchKernelEx(&acfg, attn_kernel<KEYS, CNT, SETTLE>, mq, mk, mv, ap);
 }
 
-// K3: consensus attention -> C
-static int launch_attention(const Geometry& g, const Bf16Buffers& b, Launch& ln) {
+// K3: consensus attention -> C.  Levels [l_full, L) run for image 0 only (see AttnParams::l_full)
+static int launch_attention(const Geometry& g, const Bf16Buffers& b, int l_full, Launch& ln) {
   const int d = g.d, L = g.L, n = g.n;
   // Up to 576 columns the probabilities of a 128-query tile against all keys fit in shared memory: one launch.  Beyond,
   // the keys are processed in passes of ATTN_PASS_KEYS (one launch each, see AttnParams): no shape falls to CUDA cores.
@@ -1036,7 +1060,8 @@ static int launch_attention(const Geometry& g, const Bf16Buffers& b, Launch& ln)
     ap.c_out = b.c;
     ap.scale = 1.0f / sqrtf((float)d);
     ap.ntiles = (n + BM - 1) / BM;
-    ap.num_items = ap.ntiles * L * g.B;
+    ap.l_full = l_full;
+    ap.num_items = ap.ntiles * (l_full * g.B + L - l_full);
     ap.frozen = b.frozen;
     // 256 keys: 3 slots of 48 KB next to 64 KB of P (n = 256: 219,392 B); 128 keys: 2 slots of 32 KB at 576 keys
     const uint32_t slot = keys == 256 ? AttnCfg<256>::SLOT_BYTES : AttnCfg<128>::SLOT_BYTES;
@@ -1094,11 +1119,13 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, Launch& l
     p.num_m = (rows + 255) / 256; p.num_n = 4 * d / 256; p.num_tiles = (g.G - p.z0) * p.num_m * p.num_n;
     p.bias = b.b1; p.m128 = m128;
     p.frozen = b.frozen; p.block_frozen = b.block_frozen; p.block_fresh = b.block_fresh;
+    // a forward from init_levels: the groups whose input is the same in every image run the representative rows only
+    if (b.ii_reduce) set_reduced(p, g.G, rep_row_blocks(n), [&](int z) { return ii_k1_full(z, step_index); });
     ProfScope scope(ln.prof, PROF_GEMM1, st);
     GLOM_TRY(ln.launched(launch_gemm<0, 256>(mx, msb, msp, mw1, mh_out, p, num_sms, st), "gemm1 launch"));
   }
   // ---------------- K3 between K1 and K2 (C is then written shortly before K2's epilogue reads it)
-  GLOM_TRY(launch_attention(g, b, ln));
+  GLOM_TRY(launch_attention(g, b, b.ii_reduce ? ii_k3_full_levels(step_index) : L, ln));
   // ---------------- K2: grouped GEMM2 + combine -> state t+1 (+ shadows, norms)   (all levels)
   {
     GemmParams p{};
@@ -1109,6 +1136,11 @@ int step_bf16(const Geometry& g, const Bf16Buffers& b, int step_index, Launch& l
     p.bias = b.b2; p.s32_in = b.s32_in; p.s_bcast = b.s32_in_bcast; p.c_in = b.c; p.pos = b.pos;
     p.s32_out = b.s32_out; p.sb_out = b.sb_out; p.sp_out = b.sp_out; p.nsq_out = b.nsq_out; p.nparts = g.nparts;
     p.frozen = b.frozen; p.block_frozen = b.block_frozen; p.dsq_out = b.dsq_out;
+    if (b.ii_reduce) {     // S_{t+1}[l] differs between images only for l <= t; the top level stays last (half cost)
+      set_reduced(p, L, rep_row_blocks(n), [&](int l) { return ii_k2_full(l, step_index); });
+      p.n_half = (L - 1 <= step_index ? p.num_m : p.num_m_rep) * p.num_n;
+      p.remap_l = step_index; p.h_period = rep_h_blocks(n);
+    }
     cudaError_t e;
     ProfScope scope(ln.prof, PROF_GEMM2, st);
     if (g.bn2 == 256) e = launch_gemm<1, 256>(mh, mh, mh, mw2, mh, p, num_sms, st);
