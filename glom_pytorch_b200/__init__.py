@@ -2,5 +2,6 @@
 from ._native import GlomB200Error, LIB_PATH
 from .glom import Glom
 from .islands import Islands, islands
+from . import ops  # noqa: F401  (registers the glom_b200 custom ops, so a saved ExportedProgram loads)
 
 __all__ = ["Glom", "GlomB200Error", "LIB_PATH", "Islands", "islands"]

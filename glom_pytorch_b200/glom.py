@@ -27,7 +27,11 @@ the packed copy is cached and keyed on each parameter's ``(data_ptr, _version)``
 ``.to()`` / ``.cuda()`` / ``.half()``-style ``_apply`` calls and ``invalidate_packed()``.  In-place edits through
 ``param.data`` do not bump ``_version``: call ``invalidate_packed()`` after them in eval mode.  A call made under CUDA
 graph capture packs inside its graph into a buffer of its own and uses workspaces no other call touches, so its graph
-reads the parameters at replay and depends on no other call (DESIGN.md, "CUDA graphs and streams").
+reads the parameters at replay and depends on no other call (DESIGN.md, "CUDA graphs and streams").  While
+torch.compile / torch.export trace, forward, settle, tokens and islands call the same engine entry points as the
+``glom_b200`` custom ops of ops.py, with the semantics of a captured call; ``last_launches`` is then not updated, and a
+compiled step's backward runs in the deterministic mode in effect at its forward call (DESIGN.md, "torch.compile and
+torch.export").
 
 Engine-only knob (keyword-only, additive): ``precision`` = ``"bf16"`` (default; wgmma tensor cores,
 bf16 operands, fp32 accumulate and fp32 state -- the arithmetic of the reference under
@@ -62,8 +66,11 @@ def _contiguous16(t):
 
 def _capturing():
     """True inside a CUDA graph capture on the current stream.  Such a call may only enqueue: it reads nothing on the
-    host, and it uses buffers of its own that no other call touches (Glom._capture_owned)."""
-    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+    host, and it uses buffers of its own that no other call touches (Glom._capture_owned).  Never true while
+    torch.compile / torch.export trace: that path calls the custom ops (ops.py), which always work in buffers of their
+    own."""
+    return (not torch.compiler.is_compiling() and torch.cuda.is_available()
+            and torch.cuda.is_current_stream_capturing())
 
 
 def _no_capture(what, why):
@@ -75,6 +82,19 @@ def _require_cuda(img):
     if not img.is_cuda:
         raise RuntimeError("glom_pytorch_b200.Glom runs on CUDA sm_90a (H100) only (no CPU fallback); "
                            "move the module and inputs to an H100")
+
+
+def radius_mask_d2(mask, side):
+    """d2_max of a (1, n, n) radius mask on a side x side patch grid (True = masked: squared distance > d2_max), or None
+    if the mask is no such mask.  Reads the mask on the host."""
+    mask = mask[0].cpu()
+    ar = torch.arange(side)
+    hh, ww = torch.meshgrid(ar, ar, indexing="ij")
+    co = torch.stack((hh.reshape(-1), ww.reshape(-1)), -1)
+    d2 = ((co[:, None, :] - co[None, :, :]) ** 2).sum(-1)
+    kept = d2[~mask]
+    d2_max = int(kept.max().item()) if kept.numel() else -1
+    return d2_max if torch.equal(d2 > d2_max, mask) else None
 
 
 class _Patchify(nn.Module):
@@ -159,16 +179,23 @@ class ConsensusAttention(nn.Module):
         """Key the buffer with its d2_max (None if it is not a radius mask on the grid), read from a host copy."""
         if self.local_consensus_radius <= 0:
             return
-        side = self.num_patches_side
-        mask = self.non_local_mask[0].cpu()
-        ar = torch.arange(side)
-        hh, ww = torch.meshgrid(ar, ar, indexing="ij")
-        co = torch.stack((hh.reshape(-1), ww.reshape(-1)), -1)
-        d2 = ((co[:, None, :] - co[None, :, :]) ** 2).sum(-1)
-        kept = d2[~mask]
-        d2_max = int(kept.max().item()) if kept.numel() else -1
-        self._mask_key = (self.non_local_mask, d2_max if torch.equal(d2 > d2_max, mask) else None,
+        self._mask_key = (self.non_local_mask, radius_mask_d2(self.non_local_mask, self.num_patches_side),
                           self.non_local_mask._version)
+
+    def _op_mask_args(self, n):
+        """mask_params for the custom-op path (glom_pytorch_b200.ops), which torch.compile / torch.export trace:
+        -> (mask_side, mask_d2_max, mask buffer or None).  The radius is the one of the last host check, a constant of
+        the trace (dynamo guards on ``_mask_key``); the op check_radius_mask re-checks the buffer when it runs, so an
+        in-place edit made after tracing raises instead of running with the old radius."""
+        if self.local_consensus_radius <= 0:
+            return 0, 0, None
+        side = self.num_patches_side
+        if n != side * side:
+            raise RuntimeError(f"local_consensus_radius needs n == num_patches ({side * side}), got {n} "
+                               "(the reference's masked_fill_ fails the same way)")
+        if self._mask_key[1] is None:
+            raise RuntimeError("attention.non_local_mask is not a radius mask on the patch grid")
+        return side, self._mask_key[1], self.non_local_mask
 
     def _apply(self, fn, *args, **kwargs):                 # .to() / .cuda() replace the buffer: its d2_max carries over
         if self.local_consensus_radius > 0 and not self._mask_fresh():
@@ -487,6 +514,8 @@ class Glom(nn.Module):
         p = self.patch_size
         if not self.use_native_tokenizer:
             return lin(self.image_to_tokens[0](img.float())).contiguous()
+        if torch.compiler.is_compiling():        # torch.compile / torch.export: the custom op (ops.py)
+            return torch.ops.glom_b200.tokenize(img, lin.weight, lin.bias, p, self.precision)
         img = img.float().contiguous()
         with torch.cuda.device(img.device):      # the library launches on the CURRENT device
             out = torch.empty(b, n, self.dim, dtype=torch.float32, device=img.device)
@@ -500,6 +529,7 @@ class Glom(nn.Module):
         return out
 
     # ------------------------------------------------------------------ cross-call persistence
+    @torch.compiler.disable
     def stage_tokens(self, img):
         """Video / multi-frame use (README.md:94-112): compute image_to_tokens of the NEXT frame now, on a side stream, so
         that it overlaps the tail of the forward call already enqueued for the current frame.  The following
@@ -675,6 +705,10 @@ class Glom(nn.Module):
         """forward and settle after their own argument checks: check the image and `levels`, take the tokens, and run the
         engine (`_run`'s arguments), through the autograd Function _ColumnUpdate when gradients are needed, or
         _SettleImplicit with `adjoint` = (adjoint_tol, adjoint_iters) (settle(differentiable="implicit"))."""
+        if torch.compiler.is_compiling():
+            if adjoint is not None:
+                return self._settle_implicit_eager(img, levels, needs_grad, iters, return_all, tol=tol, adjoint=adjoint)
+            return self._column_update_ops(img, levels, needs_grad, iters, return_all, steps, tol)
         _, n = self._check_input(img, levels)
         if not needs_grad:
             tokens = None if _capturing() else self._take_staged(img)      # a graph tokenises for itself
@@ -697,6 +731,33 @@ class Glom(nn.Module):
                                          *self._mlp_params())
         return _ColumnUpdate.apply(self, iters, steps, tol, return_all, tokens, pos, state0, self.init_levels,
                                    *self._mlp_params())
+
+    @torch.compiler.disable
+    def _settle_implicit_eager(self, *args, **kwargs):
+        """settle(differentiable="implicit") under torch.compile: the eager autograd Function behind a graph break (its
+        backward sets ``last_adjoint``)."""
+        return self._column_update(*args, **kwargs)
+
+    def _column_update_ops(self, img, levels, needs_grad, iters, return_all, steps, tol):
+        """_column_update while torch.compile / torch.export trace: the same engine calls as custom ops (ops.py), with
+        the semantics of a call under CUDA graph capture (no resume, no staged tokens, no packed-weight cache, the
+        parameters read when the op runs; ``last_launches`` is not updated).  With gradients the op keeps every state
+        for its backward and the last one is sliced here, as _ColumnUpdate does."""
+        _, n = self._check_input(img, levels)
+        mask_side, mask_d2_max, mask = self.attention._op_mask_args(n)
+        checked = None if mask is None else torch.ops.glom_b200.check_radius_mask(mask, mask_side, mask_d2_max)
+        tokens = self.tokens(img)                                            # (:114)
+        pos = self.pos_emb.weight[:n]                                        # (:117)
+        state0 = None if levels is None else levels.to(device=img.device, dtype=torch.float32)
+        args = (tokens, pos, state0, self.init_levels, *self._mlp_params())
+        cfg = (self.attention.attend_self, mask_side, mask_d2_max, checked)
+        if tol is None:
+            out = torch.ops.glom_b200.column_update(*args, steps, *cfg, self.precision, iters, return_all, needs_grad)
+        else:
+            out, steps = torch.ops.glom_b200.settle(*args, *cfg, tol, iters, return_all, needs_grad)
+        if needs_grad and not return_all:
+            out = out[iters]
+        return out if tol is None else (out, steps)
 
     # ------------------------------------------------------------------ inference until the columns settle
     def settle(self, img, tol, max_iters=None, levels=None, *, return_all=False, differentiable=False, adjoint_tol=None,
@@ -767,6 +828,7 @@ class Glom(nn.Module):
         return self._column_update(img, levels, needs_grad, max_iters, return_all, tol=tol, adjoint=adjoint)
 
     # ------------------------------------------------------------------ settling a stream of images
+    @torch.compiler.disable
     def settle_queue(self, img, tol, max_iters=None, levels=None, *, slots=32):
         """Settle N images through ``slots`` batch slots -> ``(levels, steps)``, as ``settle`` returns them for the whole
         batch.
@@ -791,6 +853,7 @@ class Glom(nn.Module):
         tokens = self.tokens(img)                                           # (:114) all N images, one engine call
         return self._settle_slots("settle_queue", tokens, levels, (num,), n, tol, max_iters, min(slots, num))
 
+    @torch.compiler.disable
     def settle_video(self, frames, tol, max_iters=None, levels=None, *, slots=32):
         """Settle S video streams frame by frame -> ``(levels, steps)``, each frame starting from the levels its stream's
         previous frame settled at.  ``frames`` is (S, F, 3, H, W); ``levels`` (S, n, L, d) or None (``init_levels``) is

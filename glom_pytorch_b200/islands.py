@@ -34,6 +34,8 @@ def islands(states, *, grid=None, threshold=0.9):
     side_h, side_w = grid
     if side_h * side_w != n:
         raise RuntimeError(f"grid {grid} does not tile n = {n}")
+    if torch.compiler.is_compiling():      # torch.compile / torch.export: the custom op (ops.py), no gradient
+        return Islands(*torch.ops.glom_b200.islands(states.detach(), side_h, side_w, float(threshold)))
     x = states.detach().to(torch.float32).contiguous()
     if x.data_ptr() % 16:                 # a contiguous view starting mid-row: the kernels load float4
         x = x.clone()
