@@ -1,4 +1,4 @@
-"""ctypes binding of libglom_b200.so (include/glom_b200.h).  No torch types cross the ABI:
+"""ctypes binding of libglom_b200.so (include/glom_b200.h and include/glom_b200_tree.h).  No torch types cross the ABI:
 only raw device pointers, sizes and the stream handle.  There is no fallback: if the library
 is missing or fails to load, importing the engine raises."""
 import ctypes
@@ -82,6 +82,11 @@ SIGNATURES = {
     "glom_b200_set_sm_count_target": (_i32, [_i32]),
 }
 EXPORTS = tuple(SIGNATURES)
+# every symbol of include/glom_b200_tree.h
+TREE_SIGNATURES = {
+    "glom_b200_island_tree": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+}
+TREE_EXPORTS = tuple(TREE_SIGNATURES)
 
 
 class GlomB200Error(RuntimeError):
@@ -101,7 +106,7 @@ def load():
             f"{LIB_PATH} not found: build it with `python -m glom_pytorch_b200.build` "
             "(nvcc, sm_90a). There is no CPU or PyTorch fallback for the GLOM column update.")
     lib = ctypes.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in SIGNATURES.items():
+    for name, (restype, argtypes) in (*SIGNATURES.items(), *TREE_SIGNATURES.items()):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.glom_b200_abi_version() != ABI_VERSION:
@@ -354,3 +359,10 @@ def islands(states_ptr, slabs, side_h, side_w, levels, dim, threshold, cos_right
             labels_ptr, num_islands_ptr, stream):
     check(load().glom_b200_islands(states_ptr, slabs, side_h, side_w, levels, dim, threshold, cos_right_ptr, cos_down_ptr,
                                    agreement_ptr, labels_ptr, num_islands_ptr, stream))
+
+
+def island_tree(labels_ptr, states_ptr, slabs, n, levels, dim, size_ptr, parent_ptr, containment_ptr, nested_ptr,
+                embedding_ptr, member_cos_ptr, coherence_ptr, stream):
+    """glom_b200_island_tree (include/glom_b200_tree.h); states_ptr None: no embedding outputs (their pointers None)."""
+    check(load().glom_b200_island_tree(labels_ptr, states_ptr, slabs, n, levels, dim, size_ptr, parent_ptr,
+                                       containment_ptr, nested_ptr, embedding_ptr, member_cos_ptr, coherence_ptr, stream))

@@ -9,9 +9,10 @@ import sys
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libglom_b200.so")
-SOURCES = ["glom_api.cu", "simt_kernels.cu", "tc_kernels.cu", "islands.cu", "bwd_kernels.cu", "tc_bwd_kernels.cu",
-           "settle_kernels.cu"]
-HEADERS = ["engine.h", "ptx.cuh", "tc_common.cuh", "gemm_sched.cuh", "prep_state.cuh", os.path.join("..", "..", "include", "glom_b200.h")]
+SOURCES = ["glom_api.cu", "simt_kernels.cu", "tc_kernels.cu", "islands.cu", "island_tree.cu", "bwd_kernels.cu",
+           "tc_bwd_kernels.cu", "settle_kernels.cu"]
+HEADERS = ["engine.h", "ptx.cuh", "tc_common.cuh", "gemm_sched.cuh", "prep_state.cuh", os.path.join("..", "..", "include", "glom_b200.h"),
+           os.path.join("..", "..", "include", "glom_b200_tree.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-cudart", "static",

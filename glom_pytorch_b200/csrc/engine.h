@@ -249,6 +249,10 @@ int launch_tokenize(const float* img, const float* w, const float* bias, float* 
 // island analytics on state slabs (islands.cu)
 int launch_islands(const float* states, int slabs, int side_h, int side_w, int L, int d, float threshold, float* cos_right,
                    float* cos_down, float* agreement, int* labels, int* num_islands, Launch& ln);
+// part-whole trees over island labels (island_tree.cu); states == NULL: no embedding kernel
+int launch_island_tree(const int* labels, const float* states, int slabs, int n, int L, int d, int* size, int* parent,
+                       float* containment, float* nested, float* embedding, float* member_cos, float* coherence,
+                       Launch& ln);
 
 cudaError_t launch_clock_probe(unsigned long long* out, unsigned long long spin_ns, cudaStream_t st);
 // (cycles, ns) sampled INSIDE the tensor-core kernels since the last reset, by ProfKind (tc_kernels.cu)

@@ -1,6 +1,7 @@
 // C ABI of libglom_b200.so (see include/glom_b200.h).  Host logic only: argument checking,
 // buffer layout, the per-step launch sequence.  No device allocation, no stream sync.
 #include "../../include/glom_b200.h"
+#include "../../include/glom_b200_tree.h"
 #include "engine.h"
 
 #include <mutex>
@@ -947,6 +948,29 @@ GLOM_B200_API int glom_b200_islands(const float* states, int slabs, int side_h, 
   if (int r = launch_islands(states, slabs, side_h, side_w, levels, dim, threshold, cos_right, cos_down, agreement, labels,
                              num_islands, ln))
     return fail(r, "islands launch: %s", ln.err);
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_island_tree(const int32_t* labels, const float* states, int slabs, int n, int levels, int dim,
+                                        int32_t* size, int32_t* parent, float* containment, float* nested,
+                                        float* embedding, float* member_cos, float* coherence, void* stream) {
+  if (!labels || !size || !parent || !containment || (!nested && levels != 1))
+    return fail(GLOM_B200_ERR_INVALID, "island_tree: a required pointer is NULL");
+  if (!states != !embedding || !states != !member_cos || !states != !coherence)
+    return fail(GLOM_B200_ERR_INVALID, "island_tree: states, embedding, member_cos and coherence are all NULL or all set");
+  if (slabs < 1 || slabs > 65535 || n < 1 || n > 8192 || levels < 1 || levels > 65535 || dim < 4 || dim % 4)
+    return fail(GLOM_B200_ERR_INVALID, "island_tree: need 1 <= slabs, levels <= 65535, 1 <= n <= 8192, dim %% 4 == 0");
+  if (misaligned(states, 16) || misaligned(embedding, 16))
+    return fail(GLOM_B200_ERR_INVALID, "island_tree: states and embedding must be 16-byte aligned");
+  if (misaligned(labels, 4) || misaligned(size, 4) || misaligned(parent, 4) || misaligned(containment, 4) ||
+      misaligned(nested, 4) || misaligned(member_cos, 4) || misaligned(coherence, 4))
+    return fail(GLOM_B200_ERR_INVALID, "island_tree: labels and outputs must be 4-byte aligned");
+  DeviceInfo di{};
+  if (int r = device_info(&di)) return r;
+  Launch& ln = begin_launch(di.sms, stream);
+  if (int r = launch_island_tree(labels, states, slabs, n, levels, dim, size, parent, containment, nested, embedding,
+                                 member_cos, coherence, ln))
+    return fail(r, "island_tree launch: %s", ln.err);
   return 0;
 }
 

@@ -5,7 +5,7 @@ Each op wraps the same C entry points as the eager path (include/glom_b200.h, th
 it allocates its outputs, its packed weights and its workspace with the torch allocator when it runs, and mutates no
 input.  Fake implementations give the output shapes from the (possibly symbolic) input shapes, and the differentiable
 ops carry their autograd formulas, whose backwards are ops of their own.  ``Glom`` routes ``forward``, ``settle``,
-``tokens`` and ``islands`` through these ops while ``torch.compiler.is_compiling()`` (DESIGN.md, "torch.compile and
+``tokens``, ``islands`` and ``parse_tree`` through these ops while ``torch.compiler.is_compiling()`` (DESIGN.md, "torch.compile and
 torch.export"); eager calls never reach them.
 
   tokenize(img, weight, bias, patch, precision) -> tokens                      glom_b200_tokenize
@@ -20,6 +20,8 @@ torch.export"); eager calls never reach them.
   column_update_backward(tokens, pos, states, grad_out, 8 MLP weights, steps?, attend_self, mask_side, mask_d2_max,
       precision, iters, grad_all, has_state0, deterministic) -> 12 gradients    glom_b200_backward[_steps|_ex]
   islands(states, side_h, side_w, threshold) -> 5 tensors                       glom_b200_islands
+  parse_tree(states, side_h, side_w, threshold, embeddings) -> 9 tensors        glom_b200_islands +
+                                                                                glom_b200_island_tree
 
 ``column_update`` / ``settle`` return every state, (T+1, B, n, L, d), when ``return_all`` or ``keep_states``, else the
 last one.  ``keep_states`` is what the autograd formula needs: the backward recomputes each step from the states, so a
@@ -427,3 +429,26 @@ def _(states, side_h, side_w, threshold):
     return (states.new_empty(shape, dtype=torch.float32), states.new_empty(shape, dtype=torch.float32),
             states.new_empty(shape, dtype=torch.float32), states.new_empty(shape, dtype=torch.int32),
             states.new_empty((*lead, levels), dtype=torch.int32))
+
+
+@torch.library.custom_op("glom_b200::parse_tree", mutates_args=())
+def parse_tree(states: Tensor, side_h: int, side_w: int, threshold: float, embeddings: bool) -> tuple[
+        Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """glom_pytorch_b200.parse_tree on (..., n, L, d) states -> the 9 ParseTree fields; without embeddings the last three
+    are zero-size."""
+    from .islands import parse_tree as eager_parse_tree
+    out = eager_parse_tree(states, grid=(side_h, side_w), threshold=threshold, embeddings=embeddings)
+    return tuple(states.new_empty(0, dtype=torch.float32) if t is None else t for t in out)
+
+
+@parse_tree.register_fake
+def _(states, side_h, side_w, threshold, embeddings):
+    *lead, n, levels, dim = states.shape
+    shape = (*lead, levels, n)
+
+    def opt(shp):
+        return states.new_empty(shp if embeddings else (0,), dtype=torch.float32)
+    return (states.new_empty(shape, dtype=torch.int32), states.new_empty((*lead, levels), dtype=torch.int32),
+            states.new_empty(shape, dtype=torch.int32), states.new_empty(shape, dtype=torch.int32),
+            states.new_empty(shape, dtype=torch.float32), states.new_empty((*lead, levels - 1), dtype=torch.float32),
+            opt((*lead, levels, n, dim)), opt(shape), opt(shape))
