@@ -208,6 +208,9 @@ struct FrozenRows {
 };
 
 // khat = S / max(|S|, 1e-12) per (row, level) ; rnorm = 1 / max(|S|, 1e-12)      (F.normalize, :58)
+// rnorm carries one more bit in its sign: negative where the clamp was active (|S| < 1e-12), for normalize_bwd_kernel.
+// The reciprocal is always positive and finite, so the sign is free and -r has the magnitude of r to the last bit;
+// comparing r with 1 / 1e-12f instead would not be exact, as norms just above 1e-12 round to the same reciprocal.
 __global__ void normalize_rows_kernel(int nrows, int d, const float* __restrict__ s, float* __restrict__ khat,
                                       float* __restrict__ rnorm, __nv_bfloat16* __restrict__ khat_b, FrozenRows frozen) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -217,13 +220,14 @@ __global__ void normalize_rows_kernel(int nrows, int d, const float* __restrict_
   for (int c = lane; c < d; c += 32) ss = fmaf(p[c], p[c], ss);
 #pragma unroll
   for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  const float r = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+  const float nrm = sqrtf(ss);
+  const float r = 1.0f / fmaxf(nrm, 1e-12f);
   for (int c = lane; c < d; c += 32) {
     const float v = p[c] * r;
     khat[(size_t)row * d + c] = v;
     if (khat_b) khat_b[(size_t)row * d + c] = __float2bfloat16_rn(v);
   }
-  if (lane == 0) rnorm[row] = r;
+  if (lane == 0) rnorm[row] = nrm < 1e-12f ? -r : r;
 }
 // in-place masked softmax over the last dim of sim (Z, n, n)     (:62-71); one warp per row
 __global__ void attn_softmax_kernel(int Z, int n, int attend_self, int mask_side, int mask_d2_max, float scale,
@@ -281,17 +285,22 @@ __global__ void attn_softmax_bwd_kernel(int Z, int n, int attend_self, int mask_
   }
 }
 // ds[row] += (dkhat - khat (khat . dkhat)) * rnorm        (backward of F.normalize); one warp per (row, level)
+// A row whose norm was clamped (rnorm < 0) is S / 1e-12, linear in S: ds[row] += dkhat * |rnorm|, no projection.
 __global__ void normalize_bwd_kernel(int nrows, int d, const float* __restrict__ khat, const float* __restrict__ dkhat,
                                      const float* __restrict__ rnorm, float* __restrict__ ds, FrozenRows frozen) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (row >= nrows || frozen(row)) return;
   const float* k = khat + (size_t)row * d;
   const float* g = dkhat + (size_t)row * d;
+  const float r = rnorm[row];
+  if (r < 0.f) {
+    for (int c = lane; c < d; c += 32) ds[(size_t)row * d + c] += g[c] * -r;
+    return;
+  }
   float dot = 0.f;
   for (int c = lane; c < d; c += 32) dot = fmaf(k[c], g[c], dot);
 #pragma unroll
   for (int o = 16; o; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
-  const float r = rnorm[row];
   for (int c = lane; c < d; c += 32) ds[(size_t)row * d + c] += (g[c] - k[c] * dot) * r;
 }
 // dinit[l, c] = sum over rows of g[(row, l, c)]           (broadcast of init_levels, :124); grid (L*d/256, row chunks)

@@ -126,6 +126,8 @@ __device__ __forceinline__ Tile decode(const BwdParams& p, int tile) {
 }
 
 // Phi(x) and phi(x) of the standard normal: gelu(x) = x Phi(x), gelu'(x) = Phi(x) + x phi(x)   (exact-erf form, :30)
+// Over every float32 x: |gelu error| <= 3.8e-7 and |gelu' error| <= 4.5e-6 (both inside [-6, 6]); past |x| = 6 at most
+// 6e-9 and 3.7e-8 (tests/test_backward_oracle.py, test_backward_gelu_fit_within_documented_bound)
 __device__ __forceinline__ void normal_cdf_pdf(float x, float& cdf, float& pdf) {
   const float a = fabsf(x), t = fminf(a, 6.0f);
   float q = 3.290448512416333e-05f;
@@ -135,7 +137,9 @@ __device__ __forceinline__ void normal_cdf_pdf(float x, float& cdf, float& pdf) 
   q = fmaf(q, t, -0.45887142419815063f);
   q = fmaf(q, t, -1.1511567831039429f);
   q = fmaf(q, t, -0.9999995827674866f);
-  const float tail = ex2_approx(q);                  // Phi(-|x|)
+  // Phi(-|x|); zero past 6, where it is below 1e-9: cdf becomes 0 or 1 and pdf 0, so that gelu' = cdf + x pdf does not
+  // grow with |x| as the fit's x * phi(6) would
+  const float tail = a > 6.0f ? 0.0f : ex2_approx(q);
   cdf = x >= 0.f ? 1.0f - tail : tail;
   // phi(t) = Phi(-t) * hazard(t): the hazard function is smooth, a degree-6 fit on [0, 6] is good to 2.4e-5 relative,
   // and the epilogue (XU-bound: ex2 + bf16 packing) saves its second ex2 per element

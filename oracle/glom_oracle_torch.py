@@ -179,7 +179,7 @@ def step_backward_bf16(P, tokens, pos, s, g, *, attend_self=False, mask=None, at
     With attn_tc (n % 8 == 0) the consensus backward runs on tensor cores too:
       khat_b = bf16(khat) (normalize_rows_kernel); logits = sb khat_b^T; a_b = bf16(A) (attn_softmax_kernel);
       dA = gsb sb^T; dsim_b = bf16(scale * dsim) (attn_softmax_bwd_kernel); ds += a_b^T gsb + dsim_b khat_b;
-      dkhat = dsim_b^T sb; the normalisation backward is fp32 on khat, rnorm.
+      dkhat = dsim_b^T sb; the normalisation backward is fp32 on khat, rnorm (dkhat * rnorm on rows clamped at 1e-12).
     Without attn_tc (the mixed path) the consensus backward is fp32 on S_t and g / c: exact here."""
     P = {k: _f64(P[k]) for k in MLP_KEYS}
     tokens, pos, s, g = _f64(tokens), _f64(pos), _f64(s), _f64(g)
@@ -230,7 +230,8 @@ def step_backward_bf16(P, tokens, pos, s, g, *, attend_self=False, mask=None, at
     # consensus (:56-73), per (image, level): q = v = S_t, k = normalize(S_t)
     q = s.permute(0, 2, 1, 3)                                                 # b l i d
     dc = gs.permute(0, 2, 1, 3)
-    rn = 1.0 / q.norm(dim=-1, keepdim=True).clamp_min(1e-12)
+    nrm = q.norm(dim=-1, keepdim=True)
+    rn = 1.0 / nrm.clamp_min(1e-12)
     khat = q * rn
     scale = d ** -0.5
     fixed = torch.zeros(n, n, dtype=torch.bool)
@@ -256,7 +257,8 @@ def step_backward_bf16(P, tokens, pos, s, g, *, attend_self=False, mask=None, at
         ab, dsb = A, scale * dsim
     dq = ab.transpose(-1, -2) @ dcs + dsb @ kk
     dk = dsb.transpose(-1, -2) @ qs
-    dq = dq + (dk - khat * (khat * dk).sum(-1, keepdim=True)) * rn
+    # a row clamped at eps (|S| < 1e-12) is S / 1e-12, linear in S: its gradient has no tangent projection
+    dq = dq + torch.where(nrm < 1e-12, dk, dk - khat * (khat * dk).sum(-1, keepdim=True)) * rn
     ds += dq.permute(0, 2, 1, 3)
     out["d_state"] = ds
     return out

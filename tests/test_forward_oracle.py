@@ -31,6 +31,8 @@ Bounds (rel, abs), set at about 3x the worst value observed over all the GPU tes
         (5e-7, 3.5e-7)   [rel 1.7e-7, abs 1.1e-7]
   tok   the tensor-core tokeniser vs the bf16-operand tokeniser
         (1.5e-6, 3e-6)   [rel 5.1e-7, abs 9.7e-7]
+The key rows at norms 0 .. 2e-12 ("subeps") and the self-only rows of a radius below 1, with both stabilisers (H100
+80GB HBM3, 700 W): emu <= 3.5e-4 / 3.9e-3 (H), tc <= 3.1e-3 / 2.6e-3, simt <= 2.6e-7 / 3.5e-7.
 No kernel missed the reference by more than rounding explains.  The faults of test_bounds_catch_faults miss these
 bounds by 17x (rel) and 4.8x (abs) at least.
 """
@@ -309,6 +311,19 @@ SHAPES = {
     # logit bounds at 0.9x and 1.1x of the stabiliser switch in the same warps, a zero level (the 1e-12 eps)
     "d256_bound_edge": (256, 3, 32, 4, None, 2, {}, "edge"),
     "d256_bound_edge_self": (256, 3, 32, 4, None, 2, dict(consensus_self=True), "edge"),
+    # key rows at norms on both sides of the 1e-12 eps, facing aligned queries (see _subeps_state)
+    "d256_n144_subeps": (256, 3, 48, 4, None, 5, {}, "subeps"),
+    "d256_n576_r2.5_self_subeps": (256, 2, 96, 4, None, 1, dict(local_consensus_radius=2.5, consensus_self=True),
+                                   "subeps"),
+    "d192_n144_r3_self_subeps": (192, 3, 48, 4, None, 2, dict(local_consensus_radius=3, consensus_self=True), "subeps"),
+    # a radius below 1: every row's only key is itself (the diagonal's constant logit without attend_self), every other
+    # key block and pass of the row is empty; n = 784 in passes of 512 + 272; with both stabilisers at the edge states
+    "d256_n256_self_only": (256, 2, 64, 4, None, 2, dict(local_consensus_radius=0.5), 1.0),
+    "d256_n784_self_only_self": (256, 2, 56, 2, None, 1, dict(local_consensus_radius=0.5, consensus_self=True), 1.0),
+    "d256_n256_self_only_self_edge": (256, 3, 64, 4, None, 2, dict(local_consensus_radius=0.5, consensus_self=True),
+                                      "edge"),
+    "d256_n784_self_only_edge": (256, 3, 56, 2, None, 2, dict(local_consensus_radius=0.5), "edge"),
+    "d192_n144_self_only": (192, 3, 48, 4, None, 2, dict(local_consensus_radius=0.5), 1.0),
     # configs[1] dims
     "config2_dims": (512, 6, 224, 14, None, 2, {}, 1.0),
     # the consensus kernel's own cases: one query tile; a 256-key block of real keys (the unmasked straight-line path);
@@ -334,6 +349,33 @@ def _edge_state(B, n, L, d, g):
     return S
 
 
+SUBEPS_NORMS = (0.0, 1e-30, 0.3e-12, 0.9e-12, 0.999e-12, 1.001e-12, 2e-12)
+SUBEPS_LEVEL = 1
+
+
+def _subeps_state(B, n, L, d, g, dtype=torch.float32):
+    """Rows of rms 1, except level SUBEPS_LEVEL of image 0: there every row is c_i v for one unit vector v, so that its
+    queries are aligned with its keys, with |c_i| of rms 1 per element and both signs, and rows 0..6 have the norms
+    SUBEPS_NORMS: zero, one whose squares underflow in fp32, and rows just below and above F.normalize's eps 1e-12."""
+    S = torch.randn(B, n, L, d, generator=g, dtype=dtype)
+    v = torch.randn(d, generator=g, dtype=dtype)
+    v = v / v.norm()
+    c = (0.5 + torch.rand(n, generator=g, dtype=dtype)) * math.sqrt(d)
+    c = torch.where(torch.rand(n, generator=g, dtype=dtype) < 0.5, -c, c)
+    c[:len(SUBEPS_NORMS)] = torch.tensor(SUBEPS_NORMS, dtype=dtype)
+    S[0, :, SUBEPS_LEVEL] = c[:, None] * v
+    return S
+
+
+def _state(kind, B, n, L, d, g):
+    """A random state of rms `kind`, or one of the named kinds "edge" (_edge_state) and "subeps" (_subeps_state)."""
+    if kind == "edge":
+        return _edge_state(B, n, L, d, g)
+    if kind == "subeps":
+        return _subeps_state(B, n, L, d, g)
+    return torch.randn(B, n, L, d, generator=g) * kind
+
+
 def _model(name, precision, seed=0, batch=None):
     dim, L, isz, p, hw, B, kw, rms = SHAPES[name]
     B = batch or B
@@ -346,8 +388,7 @@ def _model(name, precision, seed=0, batch=None):
     n = (hw[0] // p) * (hw[1] // p)
     g = torch.Generator().manual_seed(seed + 29)
     img = torch.randn((B, 3) + hw, generator=g)
-    S = _edge_state(B, n, L, dim, g) if rms == "edge" else torch.randn(B, n, L, dim, generator=g) * rms
-    return m, img, S, n
+    return m, img, _state(rms, B, n, L, dim, g), n
 
 
 def _mask(m, n):
@@ -525,7 +566,7 @@ def test_tensor_core_tokeniser(dim, p, hw, B):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", ["d192_n36", "d128_n256_r2_self"])
+@pytest.mark.parametrize("name", ["d192_n36", "d128_n256_r2_self", "d192_n144_r3_self_subeps", "d192_n144_self_only"])
 def test_fp32_engine_steps(name):
     """The fp32 CUDA-core engine: one step from a carried state and a chain of 3 steps from init_levels, each slab
     against column_step at the engine's previous slab."""
