@@ -28,10 +28,10 @@ the packed copy is cached and keyed on each parameter's ``(data_ptr, _version)``
 ``param.data`` do not bump ``_version``: call ``invalidate_packed()`` after them in eval mode.  A call made under CUDA
 graph capture packs inside its graph into a buffer of its own and uses workspaces no other call touches, so its graph
 reads the parameters at replay and depends on no other call (DESIGN.md, "CUDA graphs and streams").  While
-torch.compile / torch.export trace, forward, settle, tokens and islands call the same engine entry points as the
-``glom_b200`` custom ops of ops.py, with the semantics of a captured call; ``last_launches`` is then not updated, and a
-compiled step's backward runs in the deterministic mode in effect at its forward call (DESIGN.md, "torch.compile and
-torch.export").
+torch.compile / torch.export trace, forward, settle, tokens and islands call the ``glom_b200`` custom ops of ops.py,
+which run the same host bodies as eager calls (``_engine_forward`` and its siblings below) in buffers of their own, with
+the semantics of a captured call; ``last_launches`` is then not updated, and a compiled step's backward runs in the
+deterministic mode in effect at its forward call (DESIGN.md, "torch.compile and torch.export").
 
 Engine-only knob (keyword-only, additive): ``precision`` = ``"bf16"`` (default; wgmma tensor cores,
 bf16 operands, fp32 accumulate and fp32 state -- the arithmetic of the reference under
@@ -62,6 +62,137 @@ def _contiguous16(t):
     that starts mid-row of a larger buffer (e.g. ``big.view(-1)[1:1 + k].view(shape)``) is copied."""
     t = t.contiguous()
     return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+def _f32(t, device=None):
+    """t detached, as fp32 (on `device` if given), contiguous and 16-byte aligned: an fp32 tensor argument of the engine."""
+    return _contiguous16(t.detach().to(device=device, dtype=torch.float32))
+
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _stream(device):
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+_GRADS = tuple(k for k, _ in _native.Grads._fields_[1:])     # d_tokens, d_pos, d_state0, d_init, then the 8 MLP weights'
+
+
+# ---------------------------------------------------------------------- the host side of each engine call
+# One body per C operation, shared by eager Glom and the glom_b200 custom ops (ops.py).  They differ only in where the
+# buffers come from: `workspace` is a callable nbytes -> uint8 device tensor (eager: the module's cached workspace of a
+# slot, or a buffer of the capture's own; ops: a fresh _aligned_bytes), and eager passes its cached packed weights.
+def _pack_weights(cfg, params, packed):
+    """glom_b200_pack_weights: the 8 MLP parameters in the reference layout, packed for cfg into `packed` -> packed."""
+    srcs = [_f32(p) for p in params]
+    with torch.cuda.device(packed.device):
+        _native.pack_weights(cfg, [t.data_ptr() for t in srcs], packed.data_ptr(), packed.numel(),
+                             _stream(packed.device))
+    return packed
+
+
+def _engine_inputs(tokens, pos, state0, init_levels):
+    """The fp32 tensor arguments of a forward, settle or queue call -> (tokens, pos, state0 or None, init_levels)."""
+    return (_f32(tokens), _f32(pos), None if state0 is None else _f32(state0, tokens.device), _f32(init_levels))
+
+
+def _engine_forward(cfg, packed, tokens, pos, state0, init_levels, iters, keep_all, workspace, steps=None, tol=None):
+    """One forward engine call from state0 (None: init_levels) with the packed weights of cfg:
+    * glom_b200_forward: `iters` steps;
+    * `steps`, a (B,) integer tensor with maximum `iters` (glom_b200_forward_steps): steps[b] steps for image b;
+    * `tol` (glom_b200_settle / _settle_all): up to `iters` steps, each image stopped on the GPU.
+    -> (iters+1, B, n, L, d) fp32 if keep_all, else (B, n, L, d); with `tol` (states, steps (B,) int32)."""
+    device = tokens.device
+    b, n = tokens.shape[0], tokens.shape[1]
+    with torch.cuda.device(device):
+        stream = _stream(device)
+        tokens, pos, state0, init = _engine_inputs(tokens, pos, state0, init_levels)
+        shape = (b, n) + tuple(init.shape)
+        out = torch.empty(((iters + 1,) + shape) if keep_all else shape, dtype=torch.float32, device=device)
+        args = (cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), _ptr(state0), init.data_ptr(), out.data_ptr(), b)
+        if tol is not None:
+            steps = torch.empty(b, dtype=torch.int32, device=device)
+            ws = workspace((_native.settle_all_workspace_bytes if keep_all else _native.settle_workspace_bytes)(cfg, b, iters))
+            _native.settle(*args, iters, keep_all, tol, steps.data_ptr(), ws.data_ptr(), ws.numel(), stream)
+            return out, steps
+        if steps is None:
+            ws = workspace(_native.workspace_bytes(cfg, b, iters, keep_all))
+            _native.forward(*args, iters, keep_all, ws.data_ptr(), ws.numel(), stream)
+        else:
+            steps = steps.to(device=device, dtype=torch.int32).contiguous()
+            ws = workspace(_native.forward_steps_workspace_bytes(cfg, b, iters, keep_all))
+            _native.forward_steps(*args, steps.data_ptr(), iters, keep_all, ws.data_ptr(), ws.numel(), stream)
+    return out
+
+
+def _zero_grads(tokens, pos, weights, d_state0=None, d_init=None):
+    """The gradient buffers of a backward, by _native.Grads field name: zeroed fp32 tensors shaped like tokens, pos and
+    the weights, and d_state0 / d_init of the shapes given (None: absent)."""
+    shapes = (tokens.shape, pos.shape, d_state0, d_init, *(w.shape for w in weights))
+    return {k: None if s is None else torch.zeros(s, dtype=torch.float32, device=tokens.device)
+            for k, s in zip(_GRADS, shapes)}
+
+
+def _engine_backward(cfg, tokens, pos, states, grad_out, weights, iters, grad_all, steps, has_state0, deterministic,
+                     workspace):
+    """glom_b200_backward from the kept states (iters+1, B, n, L, d) and the cotangent of every slab (grad_all) or of
+    slab `iters`; with `steps` (the forward's per-image step counts) glom_b200_backward_steps, with `deterministic` the
+    fixed-order reductions of glom_b200_backward_ex.  -> the 12 gradients by Grads field name: d_state0 is None
+    without a start state, d_init with one."""
+    device = states.device
+    b = states.shape[1]
+    with torch.cuda.device(device):
+        grad_out = _f32(grad_out)
+        wts = [_f32(w) for w in weights]
+        tokens, pos = _f32(tokens), _f32(pos)
+        g = _zero_grads(tokens, pos, wts, states.shape[1:] if has_state0 else None,
+                        None if has_state0 else states.shape[-2:])
+        ws = workspace(_native.backward_workspace_bytes(cfg, b))
+        if steps is not None:
+            steps = steps.to(device=device, dtype=torch.int32).contiguous()
+        _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
+                         grad_out.data_ptr(), {k: _ptr(v) for k, v in g.items()}, b, iters, grad_all, ws.data_ptr(),
+                         ws.numel(), _stream(device), _ptr(steps), deterministic=deterministic)
+    return g
+
+
+def _engine_tokenize(img, weight, bias, patch, precision, workspace):
+    """glom_b200_tokenize: image_to_tokens of a (B, 3, H, W) image -> (B, n, dim) fp32."""
+    img = img.detach().float().contiguous()
+    b, _, h, w = img.shape
+    dim = weight.shape[0]
+    device = img.device
+    with torch.cuda.device(device):
+        out = torch.empty(b, (h // patch) * (w // patch), dim, dtype=torch.float32, device=device)
+        wt, bs = _f32(weight), _f32(bias)
+        nbytes = _native.tokenize_workspace_bytes(b, h, w, patch, dim, precision)
+        ws = workspace(nbytes) if nbytes else None
+        _native.tokenize(img.data_ptr(), wt.data_ptr(), bs.data_ptr(), out.data_ptr(), b, h, w, patch, dim, precision,
+                         _ptr(ws), nbytes, _stream(device))
+    return out
+
+
+def _engine_tokenize_backward(img, weight, d_tokens, patch, need_img, need_weight, need_bias, deterministic, workspace):
+    """glom_b200_tokenize_backward (deterministic: _ex, d_bias by a fixed-order column sum) -> (d_img, d_weight,
+    d_bias), each None when not needed."""
+    img = img.detach().float().contiguous()
+    b, _, h, w = img.shape
+    dim = weight.shape[0]
+    device = img.device
+    d_tokens = d_tokens.to(torch.float32).contiguous()
+    wt = _f32(weight)
+
+    def zeros(shape, need):
+        return torch.zeros(shape, dtype=torch.float32, device=device) if need else None
+    d_w, d_b, d_i = zeros(wt.shape, need_weight), zeros(dim, need_bias), zeros(img.shape, need_img)
+    with torch.cuda.device(device):
+        ws = workspace(_native.tokenize_backward_workspace_bytes(b, h, w, patch, need_img))
+        _native.tokenize_backward(img.data_ptr(), wt.data_ptr(), d_tokens.data_ptr(), _ptr(d_w), _ptr(d_b), _ptr(d_i),
+                                  b, h, w, patch, dim, ws.data_ptr(), ws.numel(), _stream(device),
+                                  deterministic=deterministic)
+    return d_i, d_w, d_b
 
 
 def _capturing():
@@ -157,19 +288,24 @@ class ConsensusAttention(nn.Module):
         loaded state_dict is honoured; raises if the buffer is not a radial mask on the grid.  The buffer is checked on
         the host when it is created, moved, loaded or copied, so this call reads nothing from the device (and may run
         inside a CUDA graph capture) unless the buffer was edited in place since."""
+        return self._mask_args(n, recheck=True)[:2]
+
+    def _mask_args(self, n, recheck):
+        """-> (mask_side, mask_d2_max, mask buffer or None), checked; `recheck`: re-derive d2_max from the buffer first
+        if it was edited in place since its last host check."""
         if self.local_consensus_radius <= 0:
-            return 0, 0
+            return 0, 0, None
         side = self.num_patches_side
         if n != side * side:
             raise RuntimeError(f"local_consensus_radius needs n == num_patches ({side * side}), got {n} "
                                "(the reference's masked_fill_ fails the same way)")
-        if not self._mask_fresh():
+        if recheck and not self._mask_fresh():
             _no_capture("a call after an in-place edit of attention.non_local_mask",
                         "checking the edited mask reads it on the host; make one call outside the capture first")
             self._derive_mask()
         if self._mask_key[1] is None:
             raise RuntimeError("attention.non_local_mask is not a radius mask on the patch grid")
-        return side, self._mask_key[1]
+        return side, self._mask_key[1], self.non_local_mask
 
     def _mask_fresh(self):
         key = getattr(self, "_mask_key", None)
@@ -187,15 +323,7 @@ class ConsensusAttention(nn.Module):
         -> (mask_side, mask_d2_max, mask buffer or None).  The radius is the one of the last host check, a constant of
         the trace (dynamo guards on ``_mask_key``); the op check_radius_mask re-checks the buffer when it runs, so an
         in-place edit made after tracing raises instead of running with the old radius."""
-        if self.local_consensus_radius <= 0:
-            return 0, 0, None
-        side = self.num_patches_side
-        if n != side * side:
-            raise RuntimeError(f"local_consensus_radius needs n == num_patches ({side * side}), got {n} "
-                               "(the reference's masked_fill_ fails the same way)")
-        if self._mask_key[1] is None:
-            raise RuntimeError("attention.non_local_mask is not a radius mask on the patch grid")
-        return side, self._mask_key[1], self.non_local_mask
+        return self._mask_args(n, recheck=False)
 
     def _apply(self, fn, *args, **kwargs):                 # .to() / .cuda() replace the buffer: its d2_max carries over
         if self.local_consensus_radius > 0 and not self._mask_fresh():
@@ -259,31 +387,16 @@ class _ColumnUpdate(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out, *_grad_steps):
-        module, iters = ctx.module, ctx.iters
+        module = ctx.module
         tokens, pos, states, *weights = ctx.saved_tensors
         device = states.device
-        b, n = tokens.shape[0], tokens.shape[1]
-        grad_out = _contiguous16(grad_out.to(torch.float32))
-        wts = [_contiguous16(w.detach().to(torch.float32)) for w in weights]
-        zeros = torch.zeros
-        g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos),
-             "d_state0": zeros(states.shape[1:], dtype=torch.float32, device=device) if ctx.had_state0 else None,
-             "d_init": None if ctx.had_state0 else zeros(module.levels, module.dim, dtype=torch.float32, device=device)}
-        names = ("d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")
-        for k, w in zip(names, wts):
-            g[k] = zeros_like32(w)
         with torch.cuda.device(device):
-            cfg = module.engine_cfg(n)           # bf16 engine: MLP GEMMs of the backward on tensor cores
-            ws_bytes = _native.backward_workspace_bytes(cfg, b)
-            ws = module._get_workspace(ws_bytes, device, "_bwd_workspace")      # cached across steps
-            ptrs = {k: (None if v is None else v.data_ptr()) for k, v in g.items()}
-            _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
-                             grad_out.data_ptr(), ptrs, b, iters, ctx.return_all, ws.data_ptr(), ws.numel(),
-                             torch.cuda.current_stream(device).cuda_stream,
-                             None if ctx.steps is None else ctx.steps.data_ptr(),
-                             deterministic=torch.are_deterministic_algorithms_enabled())
+            cfg = module.engine_cfg(tokens.shape[1])           # bf16 engine: MLP GEMMs of the backward on tensor cores
+            g = _engine_backward(cfg, tokens, pos, states, grad_out, weights, ctx.iters, ctx.return_all, ctx.steps,
+                                 ctx.had_state0, torch.are_deterministic_algorithms_enabled(),
+                                 lambda nb: module._get_workspace(nb, device, "_bwd_workspace"))   # cached across steps
         return (None, None, None, None, None, g["d_tokens"], g["d_pos"], g["d_state0"] if ctx.want_state0 else None,
-                g["d_init"], *[g[k] for k in names])
+                g["d_init"], *[g[k] for k in _GRADS[4:]])
 
 
 class _SettleImplicit(torch.autograd.Function):
@@ -308,12 +421,9 @@ class _SettleImplicit(torch.autograd.Function):
         tokens, pos, state, *weights = ctx.saved_tensors
         device = state.device
         b, n = tokens.shape[0], tokens.shape[1]
-        grad_out = _contiguous16(grad_out.to(torch.float32))
-        wts = [_contiguous16(w.detach().to(torch.float32)) for w in weights]
-        names = ("d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1", "d_td_w2", "d_td_b2")
-        g = {"d_tokens": zeros_like32(tokens), "d_pos": zeros_like32(pos)}
-        for k, w in zip(names, wts):
-            g[k] = zeros_like32(w)
+        grad_out = _f32(grad_out)
+        wts = [_f32(w) for w in weights]
+        g = _zero_grads(tokens, pos, wts)
         adj_steps = torch.empty(b, dtype=torch.int32, device=device)
         adj_q = torch.empty(b, module.levels, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
@@ -321,16 +431,12 @@ class _SettleImplicit(torch.autograd.Function):
             ws_bytes = _native.backward_implicit_workspace_bytes(cfg, b)
             ws = module._get_workspace(ws_bytes, device, "_implicit_workspace")      # cached across steps
             _native.backward_implicit(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(),
-                                      state.data_ptr(), grad_out.data_ptr(), {k: v.data_ptr() for k, v in g.items()}, b,
+                                      state.data_ptr(), grad_out.data_ptr(), {k: _ptr(v) for k, v in g.items()}, b,
                                       ctx.adjoint_iters, ctx.adjoint_tol, adj_steps.data_ptr(), adj_q.data_ptr(),
-                                      ws.data_ptr(), ws.numel(), torch.cuda.current_stream(device).cuda_stream,
+                                      ws.data_ptr(), ws.numel(), _stream(device),
                                       deterministic=torch.are_deterministic_algorithms_enabled())
         module.last_adjoint = (adj_steps, adj_q)
-        return (None, None, None, None, None, g["d_tokens"], g["d_pos"], None, None, *[g[k] for k in names])
-
-
-def zeros_like32(t):
-    return torch.zeros(t.shape, dtype=torch.float32, device=t.device)
+        return (None, None, None, None, None, g["d_tokens"], g["d_pos"], None, None, *[g[k] for k in _GRADS[4:]])
 
 
 class _Tokenize(torch.autograd.Function):
@@ -351,23 +457,11 @@ class _Tokenize(torch.autograd.Function):
     def backward(ctx, d_tokens):
         module = ctx.module
         img, weight = ctx.saved_tensors
-        need_img, need_w, need_b = ctx.needs_input_grad[1], ctx.needs_input_grad[2], ctx.needs_input_grad[3]
         device = img.device
-        b, _, h, w = img.shape
-        p = module.patch_size
-        d_tokens = d_tokens.to(torch.float32).contiguous()
-        wt = weight.detach().to(torch.float32).contiguous()
-        d_w = zeros_like32(wt) if need_w else None
-        d_b = torch.zeros(module.dim, dtype=torch.float32, device=device) if need_b else None
-        d_i = zeros_like32(img) if need_img else None
         with torch.cuda.device(device):
-            ws_bytes = _native.tokenize_backward_workspace_bytes(b, h, w, p, need_img)
-            ws = module._get_workspace(ws_bytes, device, "_tok_bwd_ws")
-            _native.tokenize_backward(img.data_ptr(), wt.data_ptr(), d_tokens.data_ptr(),
-                                      None if d_w is None else d_w.data_ptr(), None if d_b is None else d_b.data_ptr(),
-                                      None if d_i is None else d_i.data_ptr(), b, h, w, p, module.dim,
-                                      ws.data_ptr(), ws.numel(), torch.cuda.current_stream(device).cuda_stream,
-                                      deterministic=torch.are_deterministic_algorithms_enabled())
+            d_i, d_w, d_b = _engine_tokenize_backward(img, weight, d_tokens, module.patch_size, *ctx.needs_input_grad[1:4],
+                                                      torch.are_deterministic_algorithms_enabled(),
+                                                      lambda nb: module._get_workspace(nb, device, "_tok_bwd_ws"))
         return None, d_i, d_w, d_b
 
 
@@ -468,12 +562,6 @@ class Glom(nn.Module):
         # are then, and depends on no other call or graph.
         if not self.training and not capturing and self._packed is not None and self._packed[0] == key:
             return self._packed[1]
-        srcs = []
-        for p in params:
-            t = p.detach()
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                t = t.float().contiguous()
-            srcs.append(t)
         nbytes = _native.packed_weight_bytes(cfg)
         if capturing:
             packed = self._capture_owned(nbytes, device)
@@ -482,7 +570,7 @@ class Glom(nn.Module):
             packed = self._packed[1]            # same stream order as the kernels that read it: safe to overwrite
         else:
             packed = _aligned_bytes(nbytes, device)
-        _native.pack_weights(cfg, [t.data_ptr() for t in srcs], packed.data_ptr(), nbytes, stream)
+        _pack_weights(cfg, params, packed)
         if not capturing:
             self._packed = (key, packed)
         return packed
@@ -509,22 +597,15 @@ class Glom(nn.Module):
     def tokens(self, img):
         """image_to_tokens (:114): fp32 CUDA-core kernel (precision fp32) or bf16 gather + wgmma GEMM (bf16)."""
         lin = self.image_to_tokens[1]
-        _, _, h, w = img.shape
-        b, n = self._check_input(img, loop=False)
-        p = self.patch_size
+        self._check_input(img, loop=False)
         if not self.use_native_tokenizer:
             return lin(self.image_to_tokens[0](img.float())).contiguous()
         if torch.compiler.is_compiling():        # torch.compile / torch.export: the custom op (ops.py)
-            return torch.ops.glom_b200.tokenize(img, lin.weight, lin.bias, p, self.precision)
-        img = img.float().contiguous()
-        with torch.cuda.device(img.device):      # the library launches on the CURRENT device
-            out = torch.empty(b, n, self.dim, dtype=torch.float32, device=img.device)
-            wt, bs = lin.weight.detach().float().contiguous(), lin.bias.detach().float().contiguous()
-            tws_bytes = _native.tokenize_workspace_bytes(b, h, w, p, self.dim, self.precision)
-            tws = self._get_workspace(tws_bytes, img.device, "_tok_ws") if tws_bytes else None
-            _native.tokenize(img.data_ptr(), wt.data_ptr(), bs.data_ptr(), out.data_ptr(), b, h, w, p, self.dim,
-                             self.precision, tws.data_ptr() if tws_bytes else None, tws_bytes,
-                             torch.cuda.current_stream(img.device).cuda_stream)
+            return torch.ops.glom_b200.tokenize(img, lin.weight, lin.bias, self.patch_size, self.precision)
+        device = img.device
+        with torch.cuda.device(device):          # the library launches on the CURRENT device
+            out = _engine_tokenize(img, lin.weight, lin.bias, self.patch_size, self.precision,
+                                   lambda nb: self._get_workspace(nb, device, "_tok_ws"))
         self._tok_launches = _native.last_launch_count()
         return out
 
@@ -569,7 +650,8 @@ class Glom(nn.Module):
 
     # ------------------------------------------------------------------ engine call
     def _run(self, tokens, pos, state_in, init, iters, return_all, *, steps=None, tol=None, allow_resume=False):
-        """One engine call.  tokens (B,n,d), pos (n,d), state_in (B,n,L,d) or None, init (L,d): CUDA tensors.
+        """One engine call (_engine_forward) with the module's packed weights and workspace.  tokens (B,n,d), pos (n,d),
+        state_in (B,n,L,d) or None, init (L,d): CUDA tensors.
         * Plain (glom_b200_forward): `iters` steps.  allow_resume (eval, no autograd): when `state_in` IS the tensor the
           previous call returned, unmodified, and the workspace is the same, the engine still holds that state's bf16
           shadows / norm partials: the state prologue is skipped (glom_b200_forward_resume).
@@ -587,53 +669,37 @@ class Glom(nn.Module):
             allow_resume = False
         else:
             resume, self._resume = self._resume, None
-        plain = steps is None and tol is None
+        allow_resume = allow_resume and steps is None and tol is None and iters >= 1 and self.precision == "bf16"
+        ws = None
+
+        def workspace(nbytes):
+            nonlocal ws
+            ws = self._get_workspace(nbytes, device)
+            return ws
         with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
+            stream = _stream(device)
             pos_key = (self.pos_emb.weight.data_ptr(), self.pos_emb.weight._version)
             call_key = (device.index, stream, b, n, self.precision, pos_key)
-            use_resume = (plain and allow_resume and resume is not None and state_in is not None and iters >= 1
-                          and self.precision == "bf16" and resume["ref"]() is state_in
+            use_resume = (allow_resume and resume is not None and state_in is not None and resume["ref"]() is state_in
                           and state_in._version == resume["version"] and resume["key"] == call_key)
-            tokens = _contiguous16(tokens.detach().to(torch.float32))
-            pos = _contiguous16(pos.detach().to(torch.float32))
-            init = _contiguous16(init.detach().to(torch.float32))
-            if state_in is not None:
-                state_in = _contiguous16(state_in.detach().to(device=device, dtype=torch.float32))
-            state_ptr = None if state_in is None else state_in.data_ptr()
             cfg = self.engine_cfg(n)
             packed = self._packed_weights(cfg, device, stream)
-            shape = (b, n, self.levels, self.dim)
-            out = torch.empty(((iters + 1,) + shape) if return_all else shape, dtype=torch.float32, device=device)
-            if tol is not None:
-                steps = torch.empty(b, dtype=torch.int32, device=device)
-            if plain:
-                ws_bytes = _native.workspace_bytes(cfg, b, iters, return_all)
-            elif tol is None:
-                ws_bytes = _native.forward_steps_workspace_bytes(cfg, b, iters, return_all)
-            else:
-                ws_bytes = (_native.settle_all_workspace_bytes if return_all else _native.settle_workspace_bytes)(cfg, b, iters)
-            ws = self._get_workspace(ws_bytes, device)
-            if tol is not None:
-                _native.settle(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
-                               out.data_ptr(), b, iters, return_all, tol, steps.data_ptr(), ws.data_ptr(), ws.numel(), stream)
-            elif steps is not None:
-                _native.forward_steps(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
-                                      out.data_ptr(), b, steps.data_ptr(), iters, return_all, ws.data_ptr(), ws.numel(),
-                                      stream)
-            elif use_resume and ws.data_ptr() == resume["ws"]:
-                parity = _native.forward_resume(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr,
-                                                out.data_ptr(), b, iters, return_all, ws.data_ptr(), ws.numel(), stream,
-                                                resume["parity"])
+            if use_resume and workspace(_native.workspace_bytes(cfg, b, iters, return_all)).data_ptr() == resume["ws"]:
+                tokens, pos, state_in, _ = _engine_inputs(tokens, pos, state_in, init)
+                shape = (b, n, self.levels, self.dim)
+                out = torch.empty(((iters + 1,) + shape) if return_all else shape, dtype=torch.float32, device=device)
+                parity = _native.forward_resume(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(),
+                                                state_in.data_ptr(), out.data_ptr(), b, iters, return_all, ws.data_ptr(),
+                                                ws.numel(), stream, resume["parity"])
             else:
                 parity = iters & 1
-                _native.forward(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
-                                out.data_ptr(), b, iters, return_all, ws.data_ptr(), ws.numel(), stream)
+                out = _engine_forward(cfg, packed, tokens, pos, state_in, init, iters, return_all, workspace, steps=steps,
+                                      tol=tol)
             self.last_launches = _native.last_launch_count() + getattr(self, "_tok_launches", 0)
-            if plain and allow_resume and not return_all and iters >= 1 and self.precision == "bf16":
+            if allow_resume and not return_all:
                 self._resume = {"ref": weakref.ref(out), "version": out._version, "key": call_key, "ws": ws.data_ptr(),
                                 "parity": parity}
-        return out if tol is None else (out, steps)
+        return out
 
     def _parse_iters(self, iters, b):
         """-> (iters, steps): a scalar step count and None, or, for a per-image vector whose entries differ, its maximum
@@ -816,12 +882,7 @@ class Glom(nn.Module):
         if needs_grad and not differentiable:
             raise RuntimeError("Glom.settle is inference only: call it under torch.no_grad() / torch.inference_mode() "
                                "or with parameters and inputs that do not require grad, or pass differentiable=True")
-        max_iters = self.levels * 2 if max_iters is None else int(max_iters)
-        if max_iters < 1:
-            raise ValueError(f"max_iters must be >= 1, got {max_iters}")
-        tol = float(tol)
-        if tol != tol:
-            raise ValueError("tol is NaN")
+        tol, max_iters = self._settle_limits(tol, max_iters)
         adjoint = None
         if implicit and needs_grad:
             adjoint = (tol if adjoint_tol is None else adjoint_tol, max_iters if adjoint_iters is None else adjoint_iters)
@@ -889,6 +950,16 @@ class Glom(nn.Module):
                                         min(slots, num))
         return out.view(num, num_frames, n, self.levels, self.dim), steps.view(num, num_frames)
 
+    def _settle_limits(self, tol, max_iters):
+        """settle's tol (not NaN) and max_iters (None = 2L, >= 1) -> (tol, max_iters)."""
+        max_iters = self.levels * 2 if max_iters is None else int(max_iters)
+        if max_iters < 1:
+            raise ValueError(f"max_iters must be >= 1, got {max_iters}")
+        tol = float(tol)
+        if tol != tol:
+            raise ValueError("tol is NaN")
+        return tol, max_iters
+
     def _slot_args(self, name, img, levels, tol, max_iters, slots):
         """The argument checks of settle_queue / settle_video -> (tol, max_iters, slots)."""
         _no_capture(f"Glom.{name}", "its host loop reads the number of unfinished images between engine calls; capture "
@@ -899,12 +970,7 @@ class Glom(nn.Module):
         if self._needs_grad(img, levels):
             raise RuntimeError(f"Glom.{name} is inference only: call it under torch.no_grad() / torch.inference_mode() "
                                "or with parameters and inputs that do not require grad")
-        max_iters = self.levels * 2 if max_iters is None else int(max_iters)
-        if max_iters < 1:
-            raise ValueError(f"max_iters must be >= 1, got {max_iters}")
-        tol = float(tol)
-        if tol != tol:
-            raise ValueError("tol is NaN")
+        tol, max_iters = self._settle_limits(tol, max_iters)
         slots = int(slots)
         if slots < 1:
             raise ValueError(f"slots must be >= 1, got {slots}")
@@ -917,18 +983,15 @@ class Glom(nn.Module):
         images = prod(counts)
         begin, run = getattr(_native, name + "_begin"), getattr(_native, name + "_run")
         with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            pos = _contiguous16(self.pos_emb.weight[:n].detach().to(torch.float32))
-            init = _contiguous16(self.init_levels.detach().to(torch.float32))
-            state_in = None if levels is None else _contiguous16(levels.detach().to(device=device, dtype=torch.float32))
-            state_ptr = None if state_in is None else state_in.data_ptr()
+            stream = _stream(device)
+            tokens, pos, state_in, init = _engine_inputs(tokens, self.pos_emb.weight[:n], levels, self.init_levels)
             cfg = self.engine_cfg(n)
             packed = self._packed_weights(cfg, device, stream)
             out = torch.empty(images, n, self.levels, self.dim, dtype=torch.float32, device=device)
             steps = torch.empty(images, dtype=torch.int32, device=device)
             remaining = torch.empty(1, dtype=torch.int32, device=device)
             ws = self._get_workspace(getattr(_native, name + "_workspace_bytes")(cfg, slots, max_iters), device)
-            args = (tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(), out.data_ptr(), steps.data_ptr(),
+            args = (tokens.data_ptr(), pos.data_ptr(), _ptr(state_in), init.data_ptr(), out.data_ptr(), steps.data_ptr(),
                     *counts, slots, max_iters, tol, ws.data_ptr(), ws.numel(), stream)
             begin(cfg, *args)
             launches, first = _native.last_launch_count(), 0

@@ -14,6 +14,7 @@ from math import isqrt
 import torch
 
 from . import _native
+from .glom import _f32
 
 Islands = namedtuple("Islands", "cos_right cos_down agreement labels num_islands")
 ParseTree = namedtuple("ParseTree", "labels num_islands size parent containment nested embedding member_cos coherence")
@@ -37,12 +38,6 @@ def _geometry(states, grid):
     return lead, n, L, d, side_h, side_w
 
 
-def _states16(states):
-    """fp32, contiguous and 16-byte aligned: the kernels load float4 (a contiguous view starting mid-row is copied)."""
-    x = states.detach().to(torch.float32).contiguous()
-    return x.clone() if x.data_ptr() % 16 else x
-
-
 def islands(states, *, grid=None, threshold=0.9):
     """states: (..., n, L, d) fp32 CUDA tensor (e.g. ``model(img, return_all=True)``: (T+1, B, n, L, d)).
     grid: (side_h, side_w) with side_h * side_w == n (default: square).  Returns ``Islands`` of tensors shaped
@@ -51,7 +46,7 @@ def islands(states, *, grid=None, threshold=0.9):
     lead, n, L, d, side_h, side_w = _geometry(states, grid)
     if torch.compiler.is_compiling():      # torch.compile / torch.export: the custom op (ops.py), no gradient
         return Islands(*torch.ops.glom_b200.islands(states.detach(), side_h, side_w, float(threshold)))
-    x = _states16(states)
+    x = _f32(states)                       # the kernels load float4
     slabs = 1
     for v in lead:
         slabs *= v
@@ -87,7 +82,7 @@ def parse_tree(states, *, grid=None, threshold=0.9, embeddings=False):
     if torch.compiler.is_compiling():
         out = torch.ops.glom_b200.parse_tree(states.detach(), side_h, side_w, float(threshold), bool(embeddings))
         return ParseTree(*out[:6], *(out[6:] if embeddings else (None,) * 3))
-    x = _states16(states)
+    x = _f32(states)                       # the kernels load float4
     isl = islands(x, grid=(side_h, side_w), threshold=threshold)
     slabs = 1
     for v in lead:

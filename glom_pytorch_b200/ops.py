@@ -1,12 +1,12 @@
 """The engine as ``torch.library`` custom ops in the namespace ``glom_b200``, so that ``torch.compile`` (also with
 ``fullgraph=True``) and ``torch.export`` trace ``Glom`` instead of stopping at its ctypes calls.
 
-Each op wraps the same C entry points as the eager path (include/glom_b200.h, through ``_native``) and is functional:
-it allocates its outputs, its packed weights and its workspace with the torch allocator when it runs, and mutates no
-input.  Fake implementations give the output shapes from the (possibly symbolic) input shapes, and the differentiable
-ops carry their autograd formulas, whose backwards are ops of their own.  ``Glom`` routes ``forward``, ``settle``,
-``tokens``, ``islands`` and ``parse_tree`` through these ops while ``torch.compiler.is_compiling()`` (DESIGN.md, "torch.compile and
-torch.export"); eager calls never reach them.
+Each op runs the same host body as the eager path (glom.py's ``_engine_*`` functions and ``_pack_weights``, one per C
+entry point of include/glom_b200.h) and is functional: its outputs, packed weights and workspace come from the torch
+allocator when it runs, and it mutates no input.  Fake implementations give the output shapes from the (possibly
+symbolic) input shapes, and the differentiable ops carry their autograd formulas, whose backwards are ops of their own.
+``Glom`` routes ``forward``, ``settle``, ``tokens``, ``islands`` and ``parse_tree`` through these ops while
+``torch.compiler.is_compiling()`` (DESIGN.md, "torch.compile and torch.export"); eager calls never reach them.
 
   tokenize(img, weight, bias, patch, precision) -> tokens                      glom_b200_tokenize
   tokenize_backward(img, weight, d_tokens, patch, need_img, need_weight, need_bias, deterministic)
@@ -43,18 +43,8 @@ import torch
 from torch import Tensor
 
 from . import _native
-from .glom import _aligned_bytes, _contiguous16, radius_mask_d2
-
-_GRADS = ("d_tokens", "d_pos", "d_state0", "d_init", "d_bu_w1", "d_bu_b1", "d_bu_w2", "d_bu_b2", "d_td_w1", "d_td_b1",
-          "d_td_w2", "d_td_b2")
-
-
-def _stream(device):
-    return torch.cuda.current_stream(device).cuda_stream
-
-
-def _f32(t):
-    return _contiguous16(t.detach().to(torch.float32))
+from .glom import (_aligned_bytes, _engine_backward, _engine_forward, _engine_tokenize, _engine_tokenize_backward,
+                   _pack_weights, radius_mask_d2)
 
 
 _checked_masks = {}      # id(mask) -> (weakref to mask, its _version, its d2_max or None)
@@ -131,12 +121,14 @@ def _check_image_args(img, weight, patch):
              f"weight must be (dim, {patch * patch * 3}), got {tuple(weight.shape)}")
 
 
-def _packed(cfg, weights, device):
-    srcs = [w.detach().float().contiguous() for w in weights]
-    nbytes = _native.packed_weight_bytes(cfg)
-    packed = _aligned_bytes(nbytes, device)
-    _native.pack_weights(cfg, [t.data_ptr() for t in srcs], packed.data_ptr(), nbytes, _stream(device))
-    return packed
+def _fresh(device):
+    """The workspace provider of an op: a buffer of its own from the torch allocator."""
+    return lambda nbytes: _aligned_bytes(nbytes, device)
+
+
+def _or_empty(t, device):
+    """A gradient the engine did not compute (None) as the zero-size tensor of the op's schema."""
+    return torch.zeros(0, dtype=torch.float32, device=device) if t is None else t
 
 
 def _state_shape(tokens, init_levels):
@@ -148,35 +140,11 @@ def _engine_call(tokens, pos, state0, init_levels, weights, steps, attend_self, 
     """The body of column_update and settle: one engine call in buffers of its own -> states (, steps)."""
     _check_column_args(tokens, pos, state0, init_levels, weights, steps, iters)
     device = tokens.device
-    b, n, dim = tokens.shape
-    levels = init_levels.shape[0]
-    with torch.cuda.device(device):
-        stream = _stream(device)
-        tokens, pos, init = _f32(tokens), _f32(pos), _f32(init_levels)
-        state0 = None if state0 is None else _f32(state0)
-        state_ptr = None if state0 is None else state0.data_ptr()
-        cfg = _native.make_cfg(dim, levels, n, attend_self, mask_side, mask_d2_max, precision)
-        packed = _packed(cfg, weights, device)
-        shape = (b, n, levels, dim)
-        out = torch.empty(((iters + 1,) + shape) if engine_all else shape, dtype=torch.float32, device=device)
-        if tol is not None:
-            steps = torch.empty(b, dtype=torch.int32, device=device)
-            nbytes = (_native.settle_all_workspace_bytes if engine_all else _native.settle_workspace_bytes)(cfg, b, iters)
-            ws = _aligned_bytes(nbytes, device)
-            _native.settle(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
-                           out.data_ptr(), b, iters, engine_all, tol, steps.data_ptr(), ws.data_ptr(), ws.numel(), stream)
-            return out, steps
-        if steps is not None:
-            steps = steps.to(device=device, dtype=torch.int32).contiguous()
-            ws = _aligned_bytes(_native.forward_steps_workspace_bytes(cfg, b, iters, engine_all), device)
-            _native.forward_steps(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
-                                  out.data_ptr(), b, steps.data_ptr(), iters, engine_all, ws.data_ptr(), ws.numel(),
-                                  stream)
-        else:
-            ws = _aligned_bytes(_native.workspace_bytes(cfg, b, iters, engine_all), device)
-            _native.forward(cfg, packed.data_ptr(), tokens.data_ptr(), pos.data_ptr(), state_ptr, init.data_ptr(),
-                            out.data_ptr(), b, iters, engine_all, ws.data_ptr(), ws.numel(), stream)
-    return out
+    cfg = _native.make_cfg(tokens.shape[2], init_levels.shape[0], tokens.shape[1], attend_self, mask_side, mask_d2_max,
+                           precision)
+    packed = _pack_weights(cfg, weights, _aligned_bytes(_native.packed_weight_bytes(cfg), device))
+    return _engine_forward(cfg, packed, tokens, pos, state0, init_levels, iters, engine_all, _fresh(device), steps=steps,
+                           tol=tol)
 
 
 # ----------------------------------------------------------------------------- radius mask
@@ -199,18 +167,7 @@ def tokenize(img: Tensor, weight: Tensor, bias: Tensor, patch: int, precision: s
     _check_image_args(img, weight, patch)
     _check_floats(img.device, img=img, weight=weight, bias=bias)
     _check_shape("bias", bias, weight.shape[:1])
-    img = img.detach().float().contiguous()
-    b, _, h, w = img.shape
-    dim = weight.shape[0]
-    device = img.device
-    with torch.cuda.device(device):
-        out = torch.empty(b, (h // patch) * (w // patch), dim, dtype=torch.float32, device=device)
-        wt, bs = weight.detach().float().contiguous(), bias.detach().float().contiguous()
-        nbytes = _native.tokenize_workspace_bytes(b, h, w, patch, dim, precision)
-        ws = _aligned_bytes(nbytes, device) if nbytes else None
-        _native.tokenize(img.data_ptr(), wt.data_ptr(), bs.data_ptr(), out.data_ptr(), b, h, w, patch, dim, precision,
-                         None if ws is None else ws.data_ptr(), nbytes, _stream(device))
-    return out
+    return _engine_tokenize(img, weight, bias, patch, precision, _fresh(img.device))
 
 
 @tokenize.register_fake
@@ -227,23 +184,9 @@ def tokenize_backward(img: Tensor, weight: Tensor, d_tokens: Tensor, patch: int,
     _check_floats(img.device, img=img, weight=weight, d_tokens=d_tokens)
     _check_shape("d_tokens", d_tokens, (img.shape[0], (img.shape[2] // patch) * (img.shape[3] // patch),
                                         weight.shape[0]))
-    img = img.detach().float().contiguous()
-    b, _, h, w = img.shape
-    dim = weight.shape[0]
-    device = img.device
-    d_tokens = d_tokens.to(torch.float32).contiguous()
-    wt = weight.detach().to(torch.float32).contiguous()
-    empty = img.new_empty(0, dtype=torch.float32)
-    d_w = torch.zeros(wt.shape, dtype=torch.float32, device=device) if need_weight else empty
-    d_b = torch.zeros(dim, dtype=torch.float32, device=device) if need_bias else empty.clone()
-    d_i = torch.zeros(img.shape, dtype=torch.float32, device=device) if need_img else empty.clone()
-    with torch.cuda.device(device):
-        ws = _aligned_bytes(_native.tokenize_backward_workspace_bytes(b, h, w, patch, need_img), device)
-        _native.tokenize_backward(img.data_ptr(), wt.data_ptr(), d_tokens.data_ptr(),
-                                  d_w.data_ptr() if need_weight else None, d_b.data_ptr() if need_bias else None,
-                                  d_i.data_ptr() if need_img else None, b, h, w, patch, dim, ws.data_ptr(), ws.numel(),
-                                  _stream(device), deterministic=deterministic)
-    return d_i, d_w, d_b
+    grads = _engine_tokenize_backward(img, weight, d_tokens, patch, need_img, need_weight, need_bias, deterministic,
+                                      _fresh(img.device))
+    return tuple(_or_empty(g, img.device) for g in grads)
 
 
 @tokenize_backward.register_fake
@@ -328,27 +271,11 @@ def column_update_backward(tokens: Tensor, pos: Tensor, states: Tensor, grad_out
     _check_floats(tokens.device, states=states, grad_out=grad_out)
     _check_shape("tokens", tokens, (states.shape[1], states.shape[2], states.shape[4]))
     _check_shape("grad_out", grad_out, states.shape if grad_all else states.shape[1:])
-    device = states.device
-    b, n, levels, dim = states.shape[1:]
-    grad_out = _f32(grad_out)
-    wts = [_f32(w) for w in weights]
-    tokens, pos = _f32(tokens), _f32(pos)
-
-    def zeros(shape):
-        return torch.zeros(shape, dtype=torch.float32, device=device)
-    g = [zeros(tokens.shape), zeros(pos.shape), zeros(states.shape[1:] if has_state0 else (0,)),
-         zeros((0,) if has_state0 else (levels, dim))] + [zeros(w.shape) for w in wts]
-    ptrs = {k: v.data_ptr() for k, v in zip(_GRADS, g)}
-    ptrs["d_state0" if not has_state0 else "d_init"] = None
-    with torch.cuda.device(device):
-        cfg = _native.make_cfg(dim, levels, n, attend_self, mask_side, mask_d2_max, precision)
-        ws = _aligned_bytes(_native.backward_workspace_bytes(cfg, b), device)
-        if steps is not None:
-            steps = steps.to(device=device, dtype=torch.int32).contiguous()
-        _native.backward(cfg, [w.data_ptr() for w in wts], tokens.data_ptr(), pos.data_ptr(), states.data_ptr(),
-                         grad_out.data_ptr(), ptrs, b, iters, grad_all, ws.data_ptr(), ws.numel(), _stream(device),
-                         None if steps is None else steps.data_ptr(), deterministic=deterministic)
-    return g
+    _, n, levels, dim = states.shape[1:]
+    cfg = _native.make_cfg(dim, levels, n, attend_self, mask_side, mask_d2_max, precision)
+    g = _engine_backward(cfg, tokens, pos, states, grad_out, weights, iters, grad_all, steps, has_state0, deterministic,
+                         _fresh(states.device))
+    return [_or_empty(t, states.device) for t in g.values()]
 
 
 @column_update_backward.register_fake
