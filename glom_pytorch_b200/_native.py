@@ -1,5 +1,5 @@
-"""ctypes binding of libglom_b200.so (include/glom_b200.h and include/glom_b200_tree.h).  No torch types cross the ABI:
-only raw device pointers, sizes and the stream handle.  There is no fallback: if the library
+"""ctypes binding of libglom_b200.so (include/glom_b200.h, include/glom_b200_tree.h and include/glom_b200_track.h).  No
+torch types cross the ABI: only raw device pointers, sizes and the stream handle.  There is no fallback: if the library
 is missing or fails to load, importing the engine raises."""
 import ctypes
 import os
@@ -87,6 +87,11 @@ TREE_SIGNATURES = {
     "glom_b200_island_tree": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 TREE_EXPORTS = tuple(TREE_SIGNATURES)
+# every symbol of include/glom_b200_track.h
+TRACK_SIGNATURES = {
+    "glom_b200_island_track": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+}
+TRACK_EXPORTS = tuple(TRACK_SIGNATURES)
 
 
 class GlomB200Error(RuntimeError):
@@ -106,7 +111,7 @@ def load():
             f"{LIB_PATH} not found: build it with `python -m glom_pytorch_b200.build` "
             "(nvcc, sm_90a). There is no CPU or PyTorch fallback for the GLOM column update.")
     lib = ctypes.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in (*SIGNATURES.items(), *TREE_SIGNATURES.items()):
+    for name, (restype, argtypes) in (*SIGNATURES.items(), *TREE_SIGNATURES.items(), *TRACK_SIGNATURES.items()):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = restype, argtypes
     if lib.glom_b200_abi_version() != ABI_VERSION:
@@ -366,3 +371,9 @@ def island_tree(labels_ptr, states_ptr, slabs, n, levels, dim, size_ptr, parent_
     """glom_b200_island_tree (include/glom_b200_tree.h); states_ptr None: no embedding outputs (their pointers None)."""
     check(load().glom_b200_island_tree(labels_ptr, states_ptr, slabs, n, levels, dim, size_ptr, parent_ptr,
                                        containment_ptr, nested_ptr, embedding_ptr, member_cos_ptr, coherence_ptr, stream))
+
+
+def island_track(labels_ptr, outer, times, inner, n, levels, prev_ptr, overlap_ptr, next_ptr, track_ptr, stream):
+    """glom_b200_island_track (include/glom_b200_track.h): labels (outer, times, inner, levels, n)."""
+    check(load().glom_b200_island_track(labels_ptr, outer, times, inner, n, levels, prev_ptr, overlap_ptr, next_ptr,
+                                        track_ptr, stream))

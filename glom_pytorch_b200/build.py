@@ -9,10 +9,11 @@ import sys
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libglom_b200.so")
-SOURCES = ["glom_api.cu", "simt_kernels.cu", "tc_kernels.cu", "islands.cu", "island_tree.cu", "bwd_kernels.cu",
-           "tc_bwd_kernels.cu", "settle_kernels.cu"]
-HEADERS = ["engine.h", "ptx.cuh", "tc_common.cuh", "gemm_sched.cuh", "prep_state.cuh", os.path.join("..", "..", "include", "glom_b200.h"),
-           os.path.join("..", "..", "include", "glom_b200_tree.h")]
+SOURCES = ["glom_api.cu", "simt_kernels.cu", "tc_kernels.cu", "islands.cu", "island_tree.cu", "island_track.cu",
+           "bwd_kernels.cu", "tc_bwd_kernels.cu", "settle_kernels.cu"]
+HEADERS = ["engine.h", "ptx.cuh", "tc_common.cuh", "gemm_sched.cuh", "prep_state.cuh", "island_pairs.cuh",
+           os.path.join("..", "..", "include", "glom_b200.h"), os.path.join("..", "..", "include", "glom_b200_tree.h"),
+           os.path.join("..", "..", "include", "glom_b200_track.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-cudart", "static",

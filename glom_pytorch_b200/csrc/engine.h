@@ -253,6 +253,9 @@ int launch_islands(const float* states, int slabs, int side_h, int side_w, int L
 int launch_island_tree(const int* labels, const float* states, int slabs, int n, int L, int d, int* size, int* parent,
                        float* containment, float* nested, float* embedding, float* member_cos, float* coherence,
                        Launch& ln);
+// island tracks through time over island labels (island_track.cu); labels (outer, times, inner, L, n)
+int launch_island_track(const int* labels, int outer, int times, int inner, int n, int L, int* prev, int* overlap,
+                        int* next, int* track, Launch& ln);
 
 cudaError_t launch_clock_probe(unsigned long long* out, unsigned long long spin_ns, cudaStream_t st);
 // (cycles, ns) sampled INSIDE the tensor-core kernels since the last reset, by ProfKind (tc_kernels.cu)

@@ -1,6 +1,7 @@
 // C ABI of libglom_b200.so (see include/glom_b200.h).  Host logic only: argument checking,
 // buffer layout, the per-step launch sequence.  No device allocation, no stream sync.
 #include "../../include/glom_b200.h"
+#include "../../include/glom_b200_track.h"
 #include "../../include/glom_b200_tree.h"
 #include "engine.h"
 
@@ -971,6 +972,25 @@ GLOM_B200_API int glom_b200_island_tree(const int32_t* labels, const float* stat
   if (int r = launch_island_tree(labels, states, slabs, n, levels, dim, size, parent, containment, nested, embedding,
                                  member_cos, coherence, ln))
     return fail(r, "island_tree launch: %s", ln.err);
+  return 0;
+}
+
+GLOM_B200_API int glom_b200_island_track(const int32_t* labels, int outer, int times, int inner, int n, int levels,
+                                         int32_t* prev, int32_t* overlap, int32_t* next, int32_t* track, void* stream) {
+  if (!labels || !prev || !overlap || !next || !track)
+    return fail(GLOM_B200_ERR_INVALID, "island_track: a required pointer is NULL");
+  if (outer < 1 || times < 1 || inner < 1 || outer > 65535 || times > 65535 || inner > 65535 ||
+      (long long)outer * times * inner > 65535 || n < 1 || n > 8192 || levels < 1 || levels > 65535)
+    return fail(GLOM_B200_ERR_INVALID,
+                "island_track: need 1 <= outer * times * inner <= 65535, 1 <= n <= 8192, 1 <= levels <= 65535");
+  if (misaligned(labels, 4) || misaligned(prev, 4) || misaligned(overlap, 4) || misaligned(next, 4) ||
+      misaligned(track, 4))
+    return fail(GLOM_B200_ERR_INVALID, "island_track: labels and outputs must be 4-byte aligned");
+  DeviceInfo di{};
+  if (int r = device_info(&di)) return r;
+  Launch& ln = begin_launch(di.sms, stream);
+  if (int r = launch_island_track(labels, outer, times, inner, n, levels, prev, overlap, next, track, ln))
+    return fail(r, "island_track launch: %s", ln.err);
   return 0;
 }
 

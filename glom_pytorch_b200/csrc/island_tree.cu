@@ -19,38 +19,18 @@
 // sequentially over the members in increasing patch order, the cosines' dot products in a fixed per-lane order and a
 // fixed butterfly.  The grid is (L, slabs) and depends on nothing else, so no result depends on the SM count.
 #include "engine.h"
+#include "island_pairs.cuh"
 
 namespace glom {
 
 namespace {
 
 constexpr int kTreeThreads = 256;
-constexpr int kKeyBits = 13;                      // k < n <= 8192 = 2^13
-constexpr unsigned kKeyMask = (1u << kKeyBits) - 1;
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
-}
-
-// murmur3's 32-bit finaliser: pair keys j * n + k share their low bits for power-of-two n
-__device__ __forceinline__ unsigned mix(unsigned h) {
-  h ^= h >> 16; h *= 0x85ebca6bu; h ^= h >> 13; h *= 0xc2b2ae35u; h ^= h >> 16;
-  return h;
-}
-
-// the island patch i belongs to under the member rule above, or -1
-__device__ __forceinline__ int member_of(const int* __restrict__ lab, int i) {
-  const int j = lab[i];
-  return (j >= 0 && j <= i && lab[j] == j) ? j : -1;
-}
-
-// hash-table slots of the tree kernel: a power of two >= 2n (load factor <= 1/2), at least 64
-inline int tree_slots(int n) {
-  int s = 64;
-  while (s < 2 * n) s <<= 1;
-  return s;
 }
 
 }  // namespace
@@ -83,32 +63,21 @@ island_tree_kernel(const int* __restrict__ labels, int n, int slots, int* __rest
     if (!has_up) continue;
     const int k = member_of(up, i);
     if (k < 0) continue;
-    const unsigned key = (unsigned)j * (unsigned)n + (unsigned)k;
-    const unsigned long long tag = (unsigned long long)(key + 1) << 32;
-    for (unsigned h = mix(key) & mask;; h = (h + 1) & mask) {             // linear probing; never full
-      const unsigned long long old = atomicCAS(&table[h], 0ull, tag | 1ull);
-      if (old == 0ull) break;
-      if ((old >> 32) == (unsigned long long)(key + 1)) { atomicAdd(&table[h], 1ull); break; }
-    }
+    pair_insert(table, mask, (unsigned)j * (unsigned)n + (unsigned)k);
   }
   __syncthreads();
   if (has_up) {
-    for (int s = threadIdx.x; s < slots; s += blockDim.x) {
-      const unsigned long long e = table[s];
-      if (!e) continue;
-      const unsigned key = (unsigned)(e >> 32) - 1, overlap = (unsigned)(e & 0xffffffffu);
-      const unsigned j = key / (unsigned)n, k = key - j * (unsigned)n;
-      atomicMax(&best[j], overlap << kKeyBits | (kKeyMask - k));
-    }
+    pair_sweep(table, slots, n,
+               [&](unsigned j, unsigned k, unsigned overlap) { atomicMax(&best[j], pack_best(overlap, k)); });
     __syncthreads();
   }
   int mine = 0;
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
     const int c = cnt[j];                                                // 0 unless j is a root with members
     const unsigned b = best[j];
-    const int overlap = (int)(b >> kKeyBits);
+    const int overlap = best_overlap(b);
     size[o + j] = c;
-    parent[o + j] = b ? (int)(kKeyMask - (b & kKeyMask)) : -1;
+    parent[o + j] = best_label(b);
     containment[o + j] = b ? (float)overlap / (float)c : 0.f;
     if (b && overlap == c) mine += c;
   }

@@ -6,7 +6,9 @@ across iterations for clustering, from which one can inspect for the theorized i
 the downstream consumer of the ``(T+1, B, n, L, d)`` slab, run on the GPU by ``glom_b200_islands``
 (include/glom_b200.h; kernels in csrc/islands.cu, HBM-bound: every state vector is read once).  ``parse_tree`` relates
 each level's islands to the level above -- the part-whole tree the paper is about -- by ``glom_b200_island_tree``
-(include/glom_b200_tree.h; kernels in csrc/island_tree.cu).
+(include/glom_b200_tree.h; kernels in csrc/island_tree.cu).  ``track_islands`` links each level's islands from one
+time step to the next -- the iterations of a ``return_all`` trajectory, or the frames of ``settle_video`` -- by
+``glom_b200_island_track`` (include/glom_b200_track.h; kernels in csrc/island_track.cu).
 """
 from collections import namedtuple
 from math import isqrt
@@ -18,6 +20,7 @@ from .glom import _f32
 
 Islands = namedtuple("Islands", "cos_right cos_down agreement labels num_islands")
 ParseTree = namedtuple("ParseTree", "labels num_islands size parent containment nested embedding member_cos coherence")
+IslandTracks = namedtuple("IslandTracks", "labels num_islands prev overlap next track")
 
 
 def _geometry(states, grid):
@@ -106,3 +109,45 @@ def parse_tree(states, *, grid=None, threshold=0.9, embeddings=False):
                             ptr(parent), ptr(containment), ptr(nested), ptr(emb), ptr(member_cos), ptr(coherence),
                             torch.cuda.current_stream(dev).cuda_stream)
     return ParseTree(isl.labels, isl.num_islands, size, parent, containment, nested, emb, member_cos, coherence)
+
+
+def track_islands(states, *, time_dim=0, grid=None, threshold=0.9):
+    """The islands of ``islands(states, grid=grid, threshold=threshold)`` followed through time: leading dimension
+    ``time_dim`` of ``states`` (..., n, L, d) is time (0 for a ``return_all`` trajectory (T+1, B, ...), 1 for
+    ``settle_video``'s (S, F, ...)), and the other leading dimensions index independent sequences
+    (include/glom_b200_track.h, kernels in csrc/island_track.cu).  Returns ``IslandTracks``:
+
+    - ``labels``, ``num_islands``: those of ``islands`` (same call, same bits);
+    - ``prev`` (..., L, n) int32: at a root j of time step t >= 1, the island at t - 1 sharing most of its patches (ties
+      to the smaller label); -1 at non-roots, at t = 0 and where no patch of j was in an island at t - 1;
+    - ``overlap`` (..., L, n) int32: that number of shared patches where ``prev >= 0``, else 0;
+    - ``next`` (..., L, n) int32: at a root of step t < T - 1, the island at t + 1 sharing most of its patches (ties to
+      the smaller label); -1 elsewhere;
+    - ``track`` (..., L, n) int32: per patch, the track id of its island.  An island continues the track of its
+      ``prev`` when each is the other's best match, else it starts track t * n + j (born at step ``id // n``, root
+      ``id % n``).  In a split the larger part keeps the track; in a merge the larger overlap carries its track on.
+
+    Every output is bit-reproducible.  Nothing is read back to the host, so the call can be captured in a CUDA graph;
+    under torch.compile it is the ``glom_b200::track_islands`` op.  No gradient flows through it."""
+    lead, n, L, d, side_h, side_w = _geometry(states, grid)
+    if not lead:
+        raise RuntimeError("track_islands: states must be (..., n, L, d) with at least one leading (time) dimension")
+    t_dim = time_dim + len(lead) + 3 if time_dim < 0 else time_dim
+    if not 0 <= t_dim < len(lead):
+        raise RuntimeError(f"track_islands: time_dim = {time_dim} is not a leading dimension of states "
+                           f"{tuple(states.shape)} (..., n, L, d)")
+    if torch.compiler.is_compiling():
+        return IslandTracks(*torch.ops.glom_b200.track_islands(states.detach(), side_h, side_w, float(threshold), t_dim))
+    x = _f32(states)                       # the kernels load float4
+    isl = islands(x, grid=(side_h, side_w), threshold=threshold)
+    outer = inner = 1
+    for v in lead[:t_dim]:
+        outer *= v
+    for v in lead[t_dim + 1:]:
+        inner *= v
+    dev = x.device
+    prev, overlap, nxt, track = (torch.empty((*lead, L, n), dtype=torch.int32, device=dev) for _ in range(4))
+    with torch.cuda.device(dev):
+        _native.island_track(isl.labels.data_ptr(), outer, lead[t_dim], inner, n, L, prev.data_ptr(), overlap.data_ptr(),
+                             nxt.data_ptr(), track.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    return IslandTracks(isl.labels, isl.num_islands, prev, overlap, nxt, track)

@@ -5,8 +5,8 @@ Each op runs the same host body as the eager path (glom.py's ``_engine_*`` funct
 entry point of include/glom_b200.h) and is functional: its outputs, packed weights and workspace come from the torch
 allocator when it runs, and it mutates no input.  Fake implementations give the output shapes from the (possibly
 symbolic) input shapes, and the differentiable ops carry their autograd formulas, whose backwards are ops of their own.
-``Glom`` routes ``forward``, ``settle``, ``tokens``, ``islands`` and ``parse_tree`` through these ops while
-``torch.compiler.is_compiling()`` (DESIGN.md, "torch.compile and torch.export"); eager calls never reach them.
+``Glom`` routes ``forward``, ``settle``, ``tokens``, ``islands``, ``parse_tree`` and ``track_islands`` through these ops
+while ``torch.compiler.is_compiling()`` (DESIGN.md, "torch.compile and torch.export"); eager calls never reach them.
 
   tokenize(img, weight, bias, patch, precision) -> tokens                      glom_b200_tokenize
   tokenize_backward(img, weight, d_tokens, patch, need_img, need_weight, need_bias, deterministic)
@@ -22,6 +22,8 @@ symbolic) input shapes, and the differentiable ops carry their autograd formulas
   islands(states, side_h, side_w, threshold) -> 5 tensors                       glom_b200_islands
   parse_tree(states, side_h, side_w, threshold, embeddings) -> 9 tensors        glom_b200_islands +
                                                                                 glom_b200_island_tree
+  track_islands(states, side_h, side_w, threshold, time_dim) -> 6 tensors       glom_b200_islands +
+                                                                                glom_b200_island_track
 
 ``column_update`` / ``settle`` return every state, (T+1, B, n, L, d), when ``return_all`` or ``keep_states``, else the
 last one.  ``keep_states`` is what the autograd formula needs: the backward recomputes each step from the states, so a
@@ -379,3 +381,20 @@ def _(states, side_h, side_w, threshold, embeddings):
             states.new_empty(shape, dtype=torch.int32), states.new_empty(shape, dtype=torch.int32),
             states.new_empty(shape, dtype=torch.float32), states.new_empty((*lead, levels - 1), dtype=torch.float32),
             opt((*lead, levels, n, dim)), opt(shape), opt(shape))
+
+
+@torch.library.custom_op("glom_b200::track_islands", mutates_args=())
+def track_islands(states: Tensor, side_h: int, side_w: int, threshold: float, time_dim: int) -> tuple[
+        Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """glom_pytorch_b200.track_islands on (..., n, L, d) states, time along leading dimension time_dim (>= 0) -> the 6
+    IslandTracks fields."""
+    from .islands import track_islands as eager_track_islands
+    return tuple(eager_track_islands(states, time_dim=time_dim, grid=(side_h, side_w), threshold=threshold))
+
+
+@track_islands.register_fake
+def _(states, side_h, side_w, threshold, time_dim):
+    *lead, n, levels, _ = states.shape
+    shape = (*lead, levels, n)
+    return (states.new_empty(shape, dtype=torch.int32), states.new_empty((*lead, levels), dtype=torch.int32),
+            *(states.new_empty(shape, dtype=torch.int32) for _ in range(4)))
