@@ -37,12 +37,17 @@ struct GemmF32 {
   MatOut C;     // (m, n)
   float alpha, beta;
   const float* bias;   // optional, per n
+  // optional: batches z of images z / zdiv with steps[z / zdiv] <= t are skipped (C untouched): the per-(image, level)
+  // attention problems of images frozen at reverse step t
+  const int32_t* steps;
+  int t;
 };
 
 __global__ void __launch_bounds__(256) gemm_f32_kernel(GemmF32 q) {
   __shared__ float As[16][64 + 4];
   __shared__ float Bs[16][64 + 4];
   const int z = blockIdx.z, z0 = z / q.zdiv, z1 = z % q.zdiv;
+  if (q.steps && __ldg(q.steps + z0) <= q.t) return;
   const float* A = q.A.p + z0 * q.A.s_b0 + z1 * q.A.s_b1;
   const float* B = q.B.p + z0 * q.B.s_b0 + z1 * q.B.s_b1;
   float* C = q.C.p + z0 * q.C.s_b0 + z1 * q.C.s_b1;
@@ -125,14 +130,19 @@ __global__ void scale_by_contrib_kernel(size_t total, int L, int d, const float*
     reinterpret_cast<float4*>(ds)[i] = v;
   }
 }
-// xp (R, d) = S[:, l, :] + pos[row % n]     (top-down input, :136)
-__global__ void add_pos_kernel(int rows, int n, int L, int d, int l, const float* __restrict__ s,
-                               const float* __restrict__ pos, float* __restrict__ xp) {
+// xp (R, d) = src[row] (+ pos[row % n])     (an MLP group's input: tokens, S[:, l-1, :], or S[:, l+1, :] + pos, :134-136)
+// steps (nullable): rows of images frozen at reverse step t (steps[row / n] <= t) get 0, so that the MLP backward of a
+// frozen row multiplies finite values by its zero cotangent whatever its state holds (NaN and inf included)
+__global__ void mlp_input_kernel(int rows, int n, int d, const float* __restrict__ src, long long src_row,
+                                 const float* __restrict__ pos, const int32_t* __restrict__ steps, int t,
+                                 float* __restrict__ xp) {
   const size_t total = (size_t)rows * d;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const size_t r = i / d;
     const int c = (int)(i % d);
-    xp[i] = s[(r * L + l) * d + c] + pos[(size_t)(r % n) * d + c];
+    if (steps && __ldg(steps + r / n) <= t) { xp[i] = 0.f; continue; }
+    const float v = src[r * src_row + c];
+    xp[i] = pos ? v + pos[(size_t)(r % n) * d + c] : v;
   }
 }
 // h = gelu(pre) ; dpre = dh * gelu'(pre)   (exact erf form, :30), dpre overwrites dh
@@ -498,9 +508,12 @@ int tokenize_backward(const float* img, const float* weight, const float* d_toke
   return 0;
 }
 
-__global__ void cast_bf16_rows(size_t n4, const float* __restrict__ src, __nv_bfloat16* __restrict__ dst) {
+// dst = bf16(src); stopped (nullable): the float4s of images b with stopped[b] <= 0 (per_image4 of them per image) get 0
+__global__ void cast_bf16_rows(size_t n4, const float* __restrict__ src, __nv_bfloat16* __restrict__ dst,
+                               const int32_t* __restrict__ stopped = nullptr, size_t per_image4 = 1) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    const float4 v = reinterpret_cast<const float4*>(src)[i];
+    float4 v = reinterpret_cast<const float4*>(src)[i];
+    if (stopped && __ldg(stopped + i / per_image4) <= 0) v = make_float4(0.f, 0.f, 0.f, 0.f);
     reinterpret_cast<uint2*>(dst)[i] = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
   }
 }
@@ -591,10 +604,12 @@ static int backward_step(const Geometry& g, const BackwardArgs& a, const float* 
     for (int l = 0; l < groups; ++l) {
       // input of the group: bottom-up l reads tokens (l == 0) or S[l-1]; top-down l reads S[l+1] + pos
       Mat X{};
-      if (net == 0 && l == 0) X = Mat{a.tokens, d, 1, 0, 0};
-      else if (net == 0) X = Mat{s_t + (size_t)(l - 1) * d, ld, 1, 0, 0};
+      if (net == 0 && l == 0 && !steps) X = Mat{a.tokens, d, 1, 0, 0};
+      else if (net == 0 && !steps) X = Mat{s_t + (size_t)(l - 1) * d, ld, 1, 0, 0};
       else {
-        add_pos_kernel<<<nblk((size_t)R * d), 256, 0, st>>>(R, n, L, d, l + 1, s_t, a.pos, xp);
+        const float* src = net == 1 ? s_t + (size_t)(l + 1) * d : l == 0 ? a.tokens : s_t + (size_t)(l - 1) * d;
+        mlp_input_kernel<<<nblk((size_t)R * d), 256, 0, st>>>(R, n, d, src, l == 0 && net == 0 ? d : ld,
+                                                              net == 1 ? a.pos : nullptr, steps, t, xp);
         GLOM_TRY(ln.launched());
         X = Mat{xp, d, 1, 0, 0};
       }
@@ -647,30 +662,30 @@ static int backward_step(const Geometry& g, const BackwardArgs& a, const float* 
     const long long sb = (long long)n * ld, sl = d, nn = (long long)n * n;
     const float scale = 1.0f / sqrtf((float)d);
     const int wblocks = (R * L * 32 + 255) / 256;
-    const FrozenRows all_rows{nullptr, 0, 1};           // masked by gs = 0 instead
-    normalize_rows_kernel<<<wblocks, 256, 0, st>>>(R * L, d, s_t, khat, rnorm, nullptr, all_rows);
+    const FrozenRows frozen{steps, t, n * L};          // frozen images' problems are skipped, as on the tensor cores
+    normalize_rows_kernel<<<wblocks, 256, 0, st>>>(R * L, d, s_t, khat, rnorm, nullptr, frozen);
     GLOM_TRY(ln.launched());
     GemmF32 q{};
     // sim = scale * Q Khat^T                              (n x n per (b, l))
-    q = GemmF32{n, n, d, L, Mat{s_t, ld, 1, sb, sl}, Mat{khat, 1, ld, sb, sl}, MatOut{A, n, 1, nn * L, nn}, 1.f, 0.f, nullptr};
+    q = GemmF32{n, n, d, L, Mat{s_t, ld, 1, sb, sl}, Mat{khat, 1, ld, sb, sl}, MatOut{A, n, 1, nn * L, nn}, 1.f, 0.f, nullptr, steps, t};
     GLOM_TRY(gemm_f32(q, Z, ln));
-    attn_softmax_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, nullptr, all_rows);
+    attn_softmax_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, scale, A, nullptr, frozen);
     GLOM_TRY(ln.launched());
     // dA = dC V^T
-    q = GemmF32{n, n, d, L, Mat{gs, ld, 1, sb, sl}, Mat{s_t, 1, ld, sb, sl}, MatOut{dA, n, 1, nn * L, nn}, 1.f, 0.f, nullptr};
+    q = GemmF32{n, n, d, L, Mat{gs, ld, 1, sb, sl}, Mat{s_t, 1, ld, sb, sl}, MatOut{dA, n, 1, nn * L, nn}, 1.f, 0.f, nullptr, steps, t};
     GLOM_TRY(gemm_f32(q, Z, ln));
     // dV: ds += A^T dC
-    q = GemmF32{n, d, n, L, Mat{A, 1, n, nn * L, nn}, Mat{gs, ld, 1, sb, sl}, MatOut{ds, ld, 1, sb, sl}, 1.f, 1.f, nullptr};
+    q = GemmF32{n, d, n, L, Mat{A, 1, n, nn * L, nn}, Mat{gs, ld, 1, sb, sl}, MatOut{ds, ld, 1, sb, sl}, 1.f, 1.f, nullptr, steps, t};
     GLOM_TRY(gemm_f32(q, Z, ln));
-    attn_softmax_bwd_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, 1.f, nullptr, all_rows);
+    attn_softmax_bwd_kernel<<<(Z * n * 32 + 255) / 256, 256, 0, st>>>(Z, n, g.attend_self, g.mask_side, g.mask_d2_max, A, dA, 1.f, nullptr, frozen);
     GLOM_TRY(ln.launched());
     // dQ: ds += scale * dsim Khat
-    q = GemmF32{n, d, n, L, Mat{dA, n, 1, nn * L, nn}, Mat{khat, ld, 1, sb, sl}, MatOut{ds, ld, 1, sb, sl}, scale, 1.f, nullptr};
+    q = GemmF32{n, d, n, L, Mat{dA, n, 1, nn * L, nn}, Mat{khat, ld, 1, sb, sl}, MatOut{ds, ld, 1, sb, sl}, scale, 1.f, nullptr, steps, t};
     GLOM_TRY(gemm_f32(q, Z, ln));
     // dKhat = scale * dsim^T Q
-    q = GemmF32{n, d, n, L, Mat{dA, 1, n, nn * L, nn}, Mat{s_t, ld, 1, sb, sl}, MatOut{dkhat, ld, 1, sb, sl}, scale, 0.f, nullptr};
+    q = GemmF32{n, d, n, L, Mat{dA, 1, n, nn * L, nn}, Mat{s_t, ld, 1, sb, sl}, MatOut{dkhat, ld, 1, sb, sl}, scale, 0.f, nullptr, steps, t};
     GLOM_TRY(gemm_f32(q, Z, ln));
-    normalize_bwd_kernel<<<wblocks, 256, 0, st>>>(R * L, d, khat, dkhat, rnorm, ds, all_rows);
+    normalize_bwd_kernel<<<wblocks, 256, 0, st>>>(R * L, d, khat, dkhat, rnorm, ds, frozen);
     GLOM_TRY(ln.launched());
   }
   return 0;
@@ -707,25 +722,28 @@ __global__ void pack_bwd_weights_kernel(int d, int L, const float* __restrict__ 
   }
 }
 // bf16 shadows of a step: sb = bf16(S_t), sp = bf16(S_t[:, 1:] + pos), gsb = bf16(gs)
-// kept (nullable): the rows of images with kept[b] <= t are not rewritten.  Such an image was frozen at step t + 1 too,
-// so its gsb rows already hold the exact zeros the MLP GEMMs of partially frozen blocks need, and its sb / sp rows hold
-// finite values those GEMMs only multiply by zero (with return_all states they are the same bits: S_t == S_{t+1})
+// steps (nullable): the rows of images frozen at step t (steps[b] <= t) get zeros in all three, so that the MLP GEMMs of
+// partially frozen blocks multiply finite operands by their zero cotangents whatever the state holds (NaN and inf
+// included; the attention skips those images' problems).  kept: those rows already hold the zeros (written at reverse
+// step t + 1, where the image was frozen too), so they are not rewritten
 __global__ void bwd_shadows_kernel(int rows, int n, int L, int d, const float* __restrict__ s, const float* __restrict__ gs,
                                    const float* __restrict__ pos, __nv_bfloat16* __restrict__ sb,
                                    __nv_bfloat16* __restrict__ sp, __nv_bfloat16* __restrict__ gsb,
-                                   const int32_t* __restrict__ kept, int t) {
+                                   const int32_t* __restrict__ steps, int t, int kept) {
   const size_t total4 = (size_t)rows * L * d / 4;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += (size_t)gridDim.x * blockDim.x) {
     const size_t e = i * 4;
     const int c = (int)(e % d), l = (int)((e / d) % L);
     const size_t r = e / ((size_t)L * d);
-    if (kept && __ldg(kept + r / n) <= t) continue;
-    const float4 v = *reinterpret_cast<const float4*>(s + e);
-    const float4 gv = *reinterpret_cast<const float4*>(gs + e);
+    const bool frozen = steps && __ldg(steps + r / n) <= t;
+    if (frozen && kept) continue;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 v = frozen ? zero : *reinterpret_cast<const float4*>(s + e);
+    const float4 gv = frozen ? zero : *reinterpret_cast<const float4*>(gs + e);
     *reinterpret_cast<uint2*>(sb + e) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
     *reinterpret_cast<uint2*>(gsb + e) = make_uint2(pack_bf16x2(gv.x, gv.y), pack_bf16x2(gv.z, gv.w));
     if (l >= 1) {
-      const float4 q = *reinterpret_cast<const float4*>(pos + (size_t)(r % n) * d + c);
+      const float4 q = frozen ? zero : *reinterpret_cast<const float4*>(pos + (size_t)(r % n) * d + c);
       *reinterpret_cast<uint2*>(sp + (r * (L - 1) + (l - 1)) * d + c) =
           make_uint2(pack_bf16x2(v.x + q.x, v.y + q.y), pack_bf16x2(v.z + q.z, v.w + q.w));
     }
@@ -763,7 +781,9 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
                                                      w.w1p, w.w2t, w.w1t, w.b1p);
     GLOM_TRY(ln.launched("backward"));
     const size_t n4 = (size_t)g.rows * g.d / 4;
-    cast_bf16_rows<<<nblk(n4), 256, 0, st>>>(n4, a.tokens, w.xb);
+    // the tokens of an image that runs no step (steps[b] = 0) are never used, and its MLP rows must multiply finite
+    // operands by their zero cotangents: its rows of xb are zeros, as bwd_shadows_kernel does for sb / sp
+    cast_bf16_rows<<<nblk(n4), 256, 0, st>>>(n4, a.tokens, w.xb, steps, (size_t)g.n * g.d / 4);
     GLOM_TRY(ln.launched("backward"));
     if (g.rows % 128) {     // rows of the last 128-row block beyond R are read as K entries of the dW GEMMs: keep them zero
       GLOM_TRY(ln.check(cudaMemsetAsync(m.h, 0, wl.blocked_bytes, st), "backward"));
@@ -777,7 +797,7 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
     const float* s_t = a.states + (size_t)t * state;
     float* ds = slab[k & 1];
     // an image frozen at step t (steps[b] <= t) below the first reverse step was frozen at step t + 1 as well: its rows
-    // of gs and of the bf16 shadows still hold what step t + 1 wrote (zeros in gs / gsb), so they are not rewritten.  A
+    // of gs and of the bf16 shadows still hold what step t + 1 wrote (zeros), so they are not rewritten.  A
     // reverse step at which every image is frozen (t >= max(steps), the tail of a settle_all backward) then only passes
     // ds = gin + gextra through; its other launches find no work.
     const int32_t* kept = (steps && t < iters - 1) ? steps : nullptr;
@@ -787,7 +807,8 @@ int backward_run(const Geometry& g, const BackwardArgs& a, int precision, int it
       if (a.relin) {      // sb / sp hold this state's shadows: only the cotangent changes (frozen rows: gs = 0 -> gsb = 0)
         cast_bf16_rows<<<nblk(state / 4), 256, 0, st>>>(state / 4, gs, w.gsb);
       } else {
-        bwd_shadows_kernel<<<nblk(state / 4), 256, 0, st>>>(g.rows, g.n, g.L, g.d, s_t, gs, a.pos, w.sb, w.sp, w.gsb, kept, t);
+        bwd_shadows_kernel<<<nblk(state / 4), 256, 0, st>>>(g.rows, g.n, g.L, g.d, s_t, gs, a.pos, w.sb, w.sp, w.gsb, steps,
+                                                            t, kept != nullptr);
       }
       GLOM_TRY(ln.launched("backward"));
       // ---- consensus attention backward: the five (n x n x d) GEMM families on tensor cores, softmax in fp32.  With

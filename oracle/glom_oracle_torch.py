@@ -85,8 +85,9 @@ def grads_at_states(P, tokens, pos, states, cot, *, return_all, steps=None, atte
 
     states: (>= T+1, B, n, L, d) with S_0..S_T (e.g. the engine's own return_all slabs; S_T is not read); T = the
     number of steps = cot.shape[0] - 1 with `return_all` (cot: one cotangent per slab), else states.shape[0] - 1 (cot:
-    the cotangent of S_T).  steps (B,) ints or None: image b is the identity at step t when steps[b] <= t (its cotangent
-    passes through and it adds nothing to any other gradient).  This is what the engine's backward computes: its fp32
+    the cotangent of S_T).  steps (B,) ints or None: image b is the identity at step t when steps[b] <= t: its cotangent
+    passes through, and the step runs on the other images only, so it adds nothing to any other gradient whatever its
+    states hold (NaN and inf included).  This is what the engine's backward computes: its fp32
     (or tensor-core) backward evaluated at its forward's states, so the forward's own rounding drops out.
     Returns float64 CPU tensors: d_state0 (dL/dS_0), d_tokens, d_pos (n, d) and one entry per MLP_KEYS name."""
     P = {k: _f64(P[k]).requires_grad_(True) for k in MLP_KEYS}
@@ -103,18 +104,17 @@ def grads_at_states(P, tokens, pos, states, cot, *, return_all, steps=None, atte
     acc["d_pos"] = torch.zeros_like(pos)
     g = cot[T] if return_all else cot
     for t in range(T - 1, -1, -1):
-        s = states[t].clone().requires_grad_(True)
-        gv = g
-        if live_all is not None:
-            live = (live_all > t).to(torch.float64)[:, None, None, None]
-            gv = g * live
-        out = column_step(s, tokens, pos, P, mask, attend_self)
-        leaves = [s, tokens, pos] + [P[k] for k in MLP_KEYS]
-        gr = torch.autograd.grad(out, leaves, gv, allow_unused=True)
-        for k, v in zip(["d_tokens", "d_pos"] + list(MLP_KEYS), gr[1:]):
-            if v is not None:
-                acc[k] += v
-        g = gr[0] + (g - gv)                                  # frozen images: the identity
+        live = slice(None) if live_all is None else (live_all > t).nonzero().flatten()
+        if live_all is None or live.numel():
+            s = states[t][live].clone().requires_grad_(True)
+            out = column_step(s, tokens[live], pos, P, mask, attend_self)
+            leaves = [s, tokens, pos] + [P[k] for k in MLP_KEYS]
+            gr = torch.autograd.grad(out, leaves, g[live], allow_unused=True)
+            for k, v in zip(["d_tokens", "d_pos"] + list(MLP_KEYS), gr[1:]):
+                if v is not None:
+                    acc[k] += v
+            g = g.clone()
+            g[live] = gr[0]                                   # frozen images: the identity
         if return_all:
             g = g + cot[t]
     acc["d_state0"] = g
